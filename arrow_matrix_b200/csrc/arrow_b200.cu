@@ -2291,6 +2291,10 @@ int arrow_dense_ptr(arrow_ctx *ctx, int buf, void **device_ptr, int64_t *rows, i
 int arrow_dense_wrap(arrow_ctx *ctx, void *device_ptr, int64_t rows, int k, int *buf_out) {
     CHECK_CTX(ctx);
     if (!device_ptr || !buf_out || rows < 0 || k < 1) return fail(ctx, ARROW_ERR_ARG, "bad wrap arguments");
+    // the vector kernels load and store float4 rows (and cp.async.bulk moves 16-byte units) when k % 4 == 0
+    const uintptr_t align = (k % 4 == 0) ? 16 : 4;
+    if ((uintptr_t)device_ptr % align != 0)
+        return fail(ctx, ARROW_ERR_ARG, "wrapped pointer %p is not %d-byte aligned (k = %d)", device_ptr, (int)align, k);
     DenseBuf d;
     d.p = (float *)device_ptr;
     d.rows = rows;

@@ -128,7 +128,8 @@ int  arrow_dense_h2d(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, const 
 int  arrow_dense_d2h(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, float *host);
 int  arrow_dense_copy(arrow_ctx *ctx, int dst, int64_t dst_row0, int src, int64_t src_row0, int64_t rows);
 int  arrow_dense_ptr(arrow_ctx *ctx, int buf, void **device_ptr, int64_t *rows, int *k);
-/* Wrap device memory owned by someone else (a torch tensor, an IPC-imported peer tile). */
+/* Wrap device memory owned by someone else (a torch tensor, an IPC-imported peer tile).  The pointer must be 16-byte
+ * aligned when k % 4 == 0 (float4 rows), else 4-byte aligned: ARROW_ERR_ARG otherwise. */
 int  arrow_dense_wrap(arrow_ctx *ctx, void *device_ptr, int64_t rows, int k, int *buf_out);
 /* Copy lanes: host<->device staging on side streams so that step i's download, step i+1's upload and the
  * compute in between overlap (PCIe is full duplex).  Lane 0 is the context's main stream.  arrow_lane_wait

@@ -1,8 +1,9 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the oracle on identical inputs.
 
-Tolerance: fp32, max |err| <= 1e-5 * max |ref| (BASELINE.json: "within 1e-5 relative") and
-np.allclose(rtol=1e-5, atol=1e-5*scale) element-wise -- the reference tests use np.allclose
-defaults (tests/test_arrowmpi.py:304, 329, 396).
+Every SpMM result is held element by element to the float64 bound of tests/spmm_bound.py (``assert_spmm``); the
+comparisons with the oracle stay as a second check with the parity tolerance: max |err| <= 1e-5 * max |ref|
+(BASELINE.json: "within 1e-5 relative") and np.allclose(rtol=1e-5, atol=1e-5*scale) element-wise -- the reference
+tests use np.allclose defaults (tests/test_arrowmpi.py:304, 329, 396).
 """
 import numpy as np
 import pytest
@@ -12,6 +13,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import oracle
 from arrow_matrix_b200 import _lib, synth
+from tests.spmm_bound import assert_spmm, ragged_csr, reference
 
 
 # kernel kinds; for the CSR-streaming tile kernel also force 1 / 2 / 4 float4 per lane (bits 4..7)
@@ -63,12 +65,15 @@ def test_spmm_vector_k(ctx, variant, k):
     dA, dX, dC = ctx.csr_from_scipy(A), ctx.dense_from_host(X), ctx.dense_alloc(n, k)
     ctx.spmm(dA, dX, dC, variant=variant)
     got = dC.d2h()
+    assert_spmm([got], reference(A, X, [np.zeros((n, k), np.float32)]))
     assert_close(got, oracle.csr_spmm_c(A, X))
     assert_close(got, A @ X)
     assert_close(got, ref_spmm64(A, X))
     # accumulate: C += A X   (arrow_slim_mpi.py:142-144)
     ctx.spmm(dA, dX, dC, accumulate=True, variant=variant)
-    assert_close(dC.d2h(), 2 * ref_spmm64(A, X))
+    got2 = dC.d2h()
+    assert_spmm([got2], reference(A, X, [got], accumulate=True))
+    assert_close(got2, 2 * ref_spmm64(A, X))
     for h in (dA, dX, dC):
         h.free()
 
@@ -82,15 +87,31 @@ def test_spmm_generic_k(ctx, k):
     X = synth.generate_dense_matrix(n, k, np.float32, rng)
     dA, dX, dC = ctx.csr_from_scipy(A), ctx.dense_from_host(X), ctx.dense_alloc(n, k)
     ctx.spmm(dA, dX, dC)
-    assert_close(dC.d2h(), oracle.csr_spmm_c(A, X))
+    got = dC.d2h()
+    assert_spmm([got], reference(A, X, [np.zeros((n, k), np.float32)]))
+    assert_close(got, oracle.csr_spmm_c(A, X))
     ctx.spmm(dA, dX, dC, accumulate=True)
-    assert_close(dC.d2h(), 2 * ref_spmm64(A, X))
+    got2 = dC.d2h()
+    assert_spmm([got2], reference(A, X, [got], accumulate=True))
+    assert_close(got2, 2 * ref_spmm64(A, X))
 
 
 @pytest.mark.parametrize("variant", ALL_VARIANTS)
 @pytest.mark.parametrize("k", [16, 128, 10])
 def test_spmm_ragged_and_long_rows(ctx, variant, k):
     """empty rows, 1-entry rows, rows above the long-row threshold (hub rows of the arrow head)."""
+    _ragged_and_long_rows(ctx, variant, k, decades=0)
+
+
+@pytest.mark.parametrize("variant", ALL_VARIANTS)
+@pytest.mark.parametrize("k", [16, 128, 10])
+def test_spmm_ragged_and_long_rows_dynamic_range(ctx, variant, k):
+    """the same rows with values scaled per row and per column over 10^+-2 each (products spread over 10^+-4) and X
+    rows over 10^+-2: a small-magnitude row is held to its own bound, not to the scale of the hub rows"""
+    _ragged_and_long_rows(ctx, variant, k, decades=2)
+
+
+def _ragged_and_long_rows(ctx, variant, k, decades):
     rng = np.random.default_rng(3)
     n = 5000
     lens = rng.integers(0, 12, size=n)
@@ -100,18 +121,26 @@ def test_spmm_ragged_and_long_rows(ctx, variant, k):
     lens[4999] = 513
     lens[10] = 512          # exactly at the threshold: regular path
     indptr = np.concatenate([[0], np.cumsum(lens)])
-    cols = np.concatenate([np.sort(rng.choice(n, size=l, replace=False)) for l in lens]).astype(np.int32)
-    vals = rng.random(cols.size, dtype=np.float32)
-    A = sparse.csr_matrix((vals, cols, indptr), shape=(n, n))
-    X = synth.generate_dense_matrix(n, k, np.float32, rng)
+    if decades:
+        A = ragged_csr(lens, n, rng, decades)
+        X = (synth.generate_dense_matrix(n, k, np.float32, rng) * 10.0 ** rng.uniform(-2, 2, (n, 1))).astype(np.float32)
+    else:
+        cols = np.concatenate([np.sort(rng.choice(n, size=l, replace=False)) for l in lens]).astype(np.int32)
+        vals = rng.random(cols.size, dtype=np.float32)
+        A = sparse.csr_matrix((vals, cols, indptr), shape=(n, n))
+        X = synth.generate_dense_matrix(n, k, np.float32, rng)
     dA, dX, dC = ctx.csr_from_scipy(A), ctx.dense_from_host(X), ctx.dense_alloc(n, k)
     info = dA.info()
     assert info["n_long_rows"] == 3 and info["max_row_nnz"] == 4097
     dC.fill(7.0)            # must be overwritten everywhere, also for empty rows
     ctx.spmm(dA, dX, dC, variant=variant)
-    assert_close(dC.d2h(), ref_spmm64(A, X))
+    got = dC.d2h()
+    assert_spmm([got], reference(A, X, [np.full((n, k), 7.0, np.float32)]))
+    assert_close(got, ref_spmm64(A, X))
     ctx.spmm(dA, dX, dC, accumulate=True, variant=variant)
-    assert_close(dC.d2h(), 2 * ref_spmm64(A, X))
+    got2 = dC.d2h()
+    assert_spmm([got2], reference(A, X, [got], accumulate=True))
+    assert_close(got2, 2 * ref_spmm64(A, X))
 
 
 def test_spmm_int64_inputs_missing_data_and_row_slice(ctx):
@@ -124,14 +153,18 @@ def test_spmm_int64_inputs_missing_data_and_row_slice(ctx):
     dX, dC = ctx.dense_from_host(X), ctx.dense_alloc(n, k)
     ctx.spmm(d64, dX, dC)
     ones = sparse.csr_matrix((np.ones_like(A.data), A.indices, A.indptr), shape=A.shape)
-    assert_close(dC.d2h(), ref_spmm64(ones, X))
+    got = dC.d2h()
+    assert_spmm([got], reference(ones, X, [np.zeros((n, k), np.float32)]))
+    assert_close(got, ref_spmm64(ones, X))
     # a row slice with un-rebased indptr (what a sharded loader hands over)
     r0, r1 = 300, 1700
     a, b = A.indptr[r0], A.indptr[r1]
     dS = ctx.csr_upload(r1 - r0, n, A.indptr[r0:r1 + 1], A.indices[a:b], A.data[a:b])
     dCs = ctx.dense_alloc(r1 - r0, k)
     ctx.spmm(dS, dX, dCs)
-    assert_close(dCs.d2h(), ref_spmm64(A[r0:r1], X))
+    got = dCs.d2h()
+    assert_spmm([got], reference(A[r0:r1], X, [np.zeros((r1 - r0, k), np.float32)]))
+    assert_close(got, ref_spmm64(A[r0:r1], X))
 
 
 @pytest.mark.parametrize("variant", ALL_VARIANTS)
@@ -160,13 +193,19 @@ def test_spmm_fused_permutations(ctx, variant, k):
     dAf = dA.remap_columns(m, n0)
     dX0, dC0 = ctx.dense_from_host(X0), ctx.dense_from_host(C0)
     ctx.spmm(dAf, dX0, dC0, rowmap=m, accumulate=True, variant=variant)
-    assert_close(dC0.d2h(), ref)
+    got = dC0.d2h()
+    col_map = np.where(valid, to_prev, -1)
+    rowmap = np.where(valid, to_prev, -1)
+    assert_spmm([got], reference(A, X0, [C0], col_map=col_map, rowmap=rowmap, accumulate=True))
+    assert_close(got, ref)
     # without accumulate only routed rows are written
     dC0.h2d(C0)
     ctx.spmm(dAf, dX0, dC0, rowmap=m, accumulate=False, variant=variant)
     ref2 = C0.copy()
     ref2[to_prev[valid]] = C1[valid]
-    assert_close(dC0.d2h(), ref2)
+    got = dC0.d2h()
+    assert_spmm([got], reference(A, X0, [C0], col_map=col_map, rowmap=rowmap))
+    assert_close(got, ref2)
 
 
 @pytest.mark.parametrize("k", [1, 4, 10, 16, 128])
@@ -266,7 +305,9 @@ def test_spmm_add_epilogue_gather(ctx, k):
     ref = ref_spmm64(A, X)
     ok = amap >= 0
     ref[ok] += add[amap[ok]]
-    assert_close(dC.d2h(), ref)
+    got = dC.d2h()
+    assert_spmm([got], reference(A, X, [np.full((n, k), 5.0, np.float32)], add=add, add_map=amap))
+    assert_close(got, ref)
 
 
 # ---- round 2: the fused multi-GPU step's building blocks, each against plain numpy ------------------------------
@@ -301,6 +342,9 @@ def test_spmm_ex_dual_operand_row_pointers_and_gather_add(ctx, k):
     sel = add_map >= 0
     ref[sel] += add[add_map[sel]]
     outs = [t0.d2h(), t1.d2h()]
+    zeros = np.zeros((900, k), np.float32)
+    assert_spmm(outs, reference(A, X1, [zeros, zeros], X2=X2, x_split=split, add=add, add_map=add_map,
+                                table=(which, row)))
     for t in (0, 1):
         s2 = np.flatnonzero(which == t)
         expect = np.zeros((900, k))
@@ -311,7 +355,9 @@ def test_spmm_ex_dual_operand_row_pointers_and_gather_add(ctx, k):
     # plain destination with a dual operand (no table)
     dC = ctx.dense_alloc(n, k)
     ctx.spmm_ex(dA, dX1, C=dC, X2=dX2, x_split=split)
-    assert_close(dC.d2h(), ref_spmm64(A, np.concatenate([X1[:split], X2])).astype(np.float32))
+    got = dC.d2h()
+    assert_spmm([got], reference(A, X1, [np.zeros((n, k), np.float32)], X2=X2, x_split=split))
+    assert_close(got, ref_spmm64(A, np.concatenate([X1[:split], X2])).astype(np.float32))
     for h in (tab, dmap, dA, dX1, dX2, dadd, t0, t1, dC):
         h.free()
 
@@ -398,3 +444,18 @@ def test_graph_capture_replays_a_two_lane_sequence(ctx):
     ctx.graph_free(g)
     with pytest.raises(_lib.ArrowError):
         ctx.graph_launch(g)
+
+
+def test_dense_wrap_rejects_misaligned_pointers(ctx):
+    """the vector kernels move float4 rows: a wrapped tile must start 16-byte aligned when k % 4 == 0, else 4-byte
+    aligned (nothing is launched)"""
+    import torch
+    t = torch.zeros(64, device="cuda")
+    base = t.data_ptr()
+    assert base % 16 == 0
+    for k, ptr in ((4, base + 4), (8, base + 8), (3, base + 2)):
+        with pytest.raises(_lib.ArrowError) as e:
+            ctx.dense_wrap(ptr, 2, k)
+        assert e.value.code == -2
+    ctx.dense_wrap(base + 16, 2, 4).free()
+    ctx.dense_wrap(base + 4, 2, 3).free()
