@@ -17,6 +17,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libarrow_b200.so")
 
 ACCUMULATE = 1
+F32, F64 = 0, 1                       # ARROW_F32 / ARROW_F64: element type of dense tiles and CSR values
+_DTYPE_CODE = {np.dtype(np.float32): F32, np.dtype(np.float64): F64}
 VARIANT_AUTO, VARIANT_DIRECT, VARIANT_SHFL, VARIANT_TMA, VARIANT_TILES = -1, 0, 1, 2, 3
 IPC_HANDLE_BYTES = 80
 
@@ -35,8 +37,9 @@ EXPORTS = [
     "arrow_ptrtable_upload", "arrow_ptrtable_free", "arrow_spmm_ex", "arrow_push_rows", "arrow_reduce_rows",
     "arrow_graph_begin", "arrow_graph_end", "arrow_graph_launch", "arrow_graph_free",
     "arrow_host_alloc_numa", "arrow_bind_thread_to_device_numa", "arrow_preload_kernels",
+    "arrow_csr_upload_f64", "arrow_dense_alloc_dtype", "arrow_dense_dtype",
 ]
-ABI_VERSION = 2          # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 3          # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -128,6 +131,9 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_host_alloc_numa": (c_int, [c_size_t, I, POINTER(P)]),
         "arrow_bind_thread_to_device_numa": (c_int, [I, pI, pI]),
         "arrow_preload_kernels": (c_int, [P, I]),
+        "arrow_csr_upload_f64": (c_int, [P, I64, I64, I64, P, I, P, I, P, pI]),
+        "arrow_dense_alloc_dtype": (c_int, [P, I64, I, I, pI]),
+        "arrow_dense_dtype": (c_int, [P, I, pI]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -139,6 +145,14 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
 
 def _ptr(a: Optional[np.ndarray]) -> c_void_p:
     return c_void_p(None) if a is None else c_void_p(a.ctypes.data)
+
+
+def element_type(dtype) -> np.dtype:
+    """``np.float32`` or ``np.float64`` (the element types the library computes in); anything else raises."""
+    dt = np.dtype(dtype)
+    if dt not in _DTYPE_CODE:
+        raise ValueError(f"unsupported element type {dt}: the library computes in float32 or float64")
+    return dt
 
 
 class PinnedArray:
@@ -234,8 +248,10 @@ class Context:
 
     # -- sparse -----------------------------------------------------------------------------
     def csr_upload(self, n_rows: int, n_cols: int, indptr: np.ndarray, indices: np.ndarray,
-                   data: Optional[np.ndarray]) -> "Csr":
-        """`indptr` may be a slice of a larger row pointer; indices/data are the matching slices."""
+                   data: Optional[np.ndarray], dtype=np.float32) -> "Csr":
+        """`indptr` may be a slice of a larger row pointer; indices/data are the matching slices.  ``dtype`` is the
+        precision of the block's values and of every launch on it (float32 or float64)."""
+        dtype = element_type(dtype)
         indptr = np.ascontiguousarray(indptr)
         if indptr.dtype not in (np.int32, np.int64):
             indptr = indptr.astype(np.int64)
@@ -246,13 +262,14 @@ class Context:
         if indices.size != nnz:
             raise ValueError(f"indices has {indices.size} entries, indptr spans {nnz}")
         if data is not None:
-            data = np.ascontiguousarray(data, dtype=np.float32)
+            data = np.ascontiguousarray(data, dtype=dtype)
             if data.size != nnz:
                 raise ValueError(f"data has {data.size} entries, indptr spans {nnz}")
+        upload = self.lib.arrow_csr_upload_f64 if dtype == np.float64 else self.lib.arrow_csr_upload
         h = c_int()
-        self._check(self.lib.arrow_csr_upload(self._h, int(n_rows), int(n_cols), nnz, _ptr(indptr), indptr.dtype.itemsize,
-                                              _ptr(indices), indices.dtype.itemsize, _ptr(data), byref(h)))
-        return Csr(self, h.value, int(n_rows), int(n_cols), nnz)
+        self._check(upload(self._h, int(n_rows), int(n_cols), nnz, _ptr(indptr), indptr.dtype.itemsize,
+                           _ptr(indices), indices.dtype.itemsize, _ptr(data), byref(h)))
+        return Csr(self, h.value, int(n_rows), int(n_cols), nnz, dtype)
 
     def csr_from_scipy(self, A) -> "Csr":
         from scipy import sparse
@@ -267,19 +284,23 @@ class Context:
         return RowMap(self, h.value, m.size, int(limit))
 
     # -- dense ------------------------------------------------------------------------------
-    def dense_alloc(self, rows: int, k: int) -> "Dense":
+    def dense_alloc(self, rows: int, k: int, dtype=np.float32) -> "Dense":
+        dtype = element_type(dtype)
         h = c_int()
-        self._check(self.lib.arrow_dense_alloc(self._h, int(rows), int(k), byref(h)))
-        return Dense(self, h.value, int(rows), int(k), owned=True)
+        if dtype == np.float32:
+            self._check(self.lib.arrow_dense_alloc(self._h, int(rows), int(k), byref(h)))
+        else:
+            self._check(self.lib.arrow_dense_alloc_dtype(self._h, int(rows), int(k), _DTYPE_CODE[dtype], byref(h)))
+        return Dense(self, h.value, int(rows), int(k), owned=True, dtype=dtype)
 
     def dense_wrap(self, device_ptr: int, rows: int, k: int) -> "Dense":
         h = c_int()
         self._check(self.lib.arrow_dense_wrap(self._h, c_void_p(device_ptr), int(rows), int(k), byref(h)))
         return Dense(self, h.value, int(rows), int(k), owned=False)
 
-    def dense_from_host(self, X: np.ndarray) -> "Dense":
-        X = np.ascontiguousarray(X, dtype=np.float32)
-        d = self.dense_alloc(X.shape[0], X.shape[1])
+    def dense_from_host(self, X: np.ndarray, dtype=np.float32) -> "Dense":
+        X = np.ascontiguousarray(X, dtype=element_type(dtype))
+        d = self.dense_alloc(X.shape[0], X.shape[1], X.dtype)
         d.h2d(X)
         self.sync()
         return d
@@ -367,11 +388,11 @@ class Context:
     LANE_MAIN, LANE_H2D, LANE_D2H = 0, 1, 2
 
     def h2d_lane(self, lane: int, dst: "Dense", X: np.ndarray, row0: int = 0):
-        assert X.dtype == np.float32 and X.flags.c_contiguous and X.shape[1] == dst.k
+        assert X.dtype == dst.dtype and X.flags.c_contiguous and X.shape[1] == dst.k
         self._check(self.lib.arrow_dense_h2d_lane(self._h, lane, dst.h, int(row0), X.shape[0], _ptr(X)))
 
     def d2h_lane(self, lane: int, src: "Dense", out: np.ndarray, row0: int = 0):
-        assert out.dtype == np.float32 and out.flags.c_contiguous and out.shape[1] == src.k
+        assert out.dtype == src.dtype and out.flags.c_contiguous and out.shape[1] == src.k
         self._check(self.lib.arrow_dense_d2h_lane(self._h, lane, src.h, int(row0), out.shape[0], _ptr(out)))
 
     def lane_wait(self, waiting_lane: int, signalling_lane: int):
@@ -421,9 +442,10 @@ class _Handle:
 
 
 class Csr(_Handle):
-    def __init__(self, ctx, h, n_rows, n_cols, nnz):
+    def __init__(self, ctx, h, n_rows, n_cols, nnz, dtype=np.float32):
         super().__init__(ctx, h)
         self.n_rows, self.n_cols, self.nnz = n_rows, n_cols, nnz
+        self.dtype = np.dtype(dtype)
 
     def info(self):
         v = [c_int64() for _ in range(5)]
@@ -433,7 +455,7 @@ class Csr(_Handle):
     def remap_columns(self, m: "RowMap", new_n_cols: int) -> "Csr":
         h = c_int()
         self.ctx._check(self.ctx.lib.arrow_csr_remap_columns(self.ctx._h, self.h, m.h, int(new_n_cols), byref(h)))
-        out = Csr(self.ctx, h.value, self.n_rows, int(new_n_cols), self.nnz)
+        out = Csr(self.ctx, h.value, self.n_rows, int(new_n_cols), self.nnz, self.dtype)
         out._parent = self           # shares indptr/values: keep the source alive
         return out
 
@@ -475,22 +497,30 @@ class PtrTable(_Handle):
 
 
 class Dense(_Handle):
-    def __init__(self, ctx, h, rows, k, owned):
+    def __init__(self, ctx, h, rows, k, owned, dtype=np.float32):
         super().__init__(ctx, h)
         self.rows, self.k, self.owned = rows, k, owned
+        self.dtype = np.dtype(dtype)
+
+    def device_dtype(self) -> np.dtype:
+        """the element type the library holds for this tile (``arrow_dense_dtype``)"""
+        code = c_int()
+        self.ctx._check(self.ctx.lib.arrow_dense_dtype(self.ctx._h, self.h, byref(code)))
+        return np.dtype(np.float64 if code.value == F64 else np.float32)
 
     def h2d(self, X: np.ndarray, row0: int = 0):
-        X = np.ascontiguousarray(X, dtype=np.float32)
+        """upload rows, converted to the tile's element type"""
+        X = np.ascontiguousarray(X, dtype=self.dtype)
         if X.ndim != 2 or X.shape[1] != self.k:
-            raise ValueError(f"expected [rows x {self.k}] fp32, got {X.shape}")
+            raise ValueError(f"expected [rows x {self.k}] {self.dtype}, got {X.shape}")
         self.ctx._check(self.ctx.lib.arrow_dense_h2d(self.ctx._h, self.h, int(row0), X.shape[0], _ptr(X)))
         self._keep = X                  # async copy: keep the host array alive until the next sync
 
     def d2h(self, out: Optional[np.ndarray] = None, row0: int = 0, rows: Optional[int] = None, sync: bool = True) -> np.ndarray:
         rows = self.rows - row0 if rows is None else rows
         if out is None:
-            out = np.empty((rows, self.k), dtype=np.float32)
-        assert out.dtype == np.float32 and out.flags.c_contiguous and out.shape == (rows, self.k)
+            out = np.empty((rows, self.k), dtype=self.dtype)
+        assert out.dtype == self.dtype and out.flags.c_contiguous and out.shape == (rows, self.k)
         self.ctx._check(self.ctx.lib.arrow_dense_d2h(self.ctx._h, self.h, int(row0), int(rows), _ptr(out)))
         if sync:
             self.ctx.sync()

@@ -68,7 +68,7 @@ def bench_spmm(path: Optional[str], width: int, n_features: int, iterations: int
         wb_logging.log({"actual_ranks": comm.Get_size()})
         tic = time.perf_counter()
         arrow.B.load_sparse_matrix_from_blocks(blocks)
-        arrow.B.zero_rhs(width, n_features)
+        arrow.B.zero_rhs(width, n_features, dtype=datatype)
         arrow.synchronize()
         comm.Barrier()
         wb_logging.log({"init_time": time.perf_counter() - tic})

@@ -28,11 +28,12 @@ from .engine import ArrowEngine
 class DecompositionBlocks:
     """What ``load_decomposition_new`` hands to ``load_sparse_matrix_from_blocks``."""
 
-    def __init__(self, decomposition, width, block_diagonal, n_blocks):
+    def __init__(self, decomposition, width, block_diagonal, n_blocks, dtype=np.float32):
         self.decomposition = decomposition
         self.width = width
         self.block_diagonal = block_diagonal
         self.n_blocks = n_blocks
+        self.dtype = np.dtype(dtype)          # precision of the values, the tiles and the arithmetic
 
 
 class ArrowDecompositionMPI:
@@ -87,6 +88,10 @@ class ArrowDecompositionMPI:
             raise TypeError("blocks must come from ArrowDecompositionMPI.load_decomposition_new")
         if blocks.width != self._n_rows_per_rank:
             raise ValueError(f"decomposition was loaded for width {blocks.width}, initialised for {self._n_rows_per_rank}")
+        dtype = getattr(blocks, "dtype", np.dtype(np.float32))
+        if self.comm.Get_size() > 1 and dtype != np.float32:
+            raise ValueError(f"a {dtype} decomposition runs on one GPU only: the multi-GPU engine computes in float32; "
+                             "load it with datatype=np.float32 or run a single process")
         if self._engine is not None:
             self._engine.close()
         if self.comm.Get_size() > 1:
@@ -105,7 +110,7 @@ class ArrowDecompositionMPI:
         else:
             self._engine = ArrowEngine(blocks.decomposition, blocks.width, self._n_feature_columns,
                                        block_diagonal=blocks.block_diagonal, mode=self._mode, n_blocks=self.n_blocks,
-                                       fused_style=getattr(self, "_fused_style", "gather"))
+                                       fused_style=getattr(self, "_fused_style", "gather"), dtype=dtype)
         self.decomposition_length = self._engine.L
 
     def load_data_from_blocks(self, blocked: DecompositionBlocks):
@@ -177,10 +182,13 @@ class ArrowDecompositionMPI:
                                slim=False, use_npy=True, use_mmap=True):
         """Open the level files (``:629-887``).  Returns ``(blocks, n_blocks, to_prev, to_next)`` like the
         reference; ``blocks`` is ``None`` (and ``n_blocks`` empty) when nothing was found.  Files are memory
-        mapped -- every process slices its own rows, nothing is scattered from a root."""
+        mapped -- every process slices its own rows, nothing is scattered from a root.  ``datatype`` (float32, the
+        reference's default, or float64) is the precision of the values, the tiles and the arithmetic of every step;
+        float32 values in the files become float64 exactly, missing value files mean ones.  float64 runs on one GPU."""
         assert not slim or is_block_diagonal
-        if np.dtype(datatype) != np.float32:
-            raise ValueError("only float32 decompositions are supported (reference default, arrow_bench.py:21)")
+        if np.dtype(datatype) not in (np.float32, np.float64):
+            raise ValueError(f"datatype must be float32 or float64 (numpy.random.Generator.random's types), got "
+                             f"{np.dtype(datatype)}")
         if use_npy:
             dec = graphio.load_decomposition_new(filename, width, block_diagonal=is_block_diagonal, mem_map=True)
         else:                                  # SciPy .npz per level (``:641-648``): read whole, then sliced per rank
@@ -190,5 +198,5 @@ class ArrowDecompositionMPI:
             return None, np.zeros(0, dtype=np.int32), None, None
         n_blocks = np.array([decomp.number_of_blocks(B, width) for B, _ in dec], dtype=np.int32)
         _, to_prev, to_next, _ = decomp.prepare_permutations([p for _, p in dec], n_blocks, width)
-        blocks = DecompositionBlocks(dec, width, is_block_diagonal, n_blocks)
+        blocks = DecompositionBlocks(dec, width, is_block_diagonal, n_blocks, datatype)
         return blocks, n_blocks, to_prev, to_next

@@ -52,12 +52,12 @@ class ArrowSlimMPI(ArrowMatrix):
         return self._engine.features(self._level)
 
     def set_features(self, X: np.ndarray) -> None:
-        """Upload this process's feature rows (level 0).  The reference keeps a reference to ``X``
-        (arrow_slim_mpi.py:285-293); here the rows are copied to the device at call time."""
+        """Upload this process's feature rows (level 0), converted to the decomposition's precision.  The reference
+        keeps a reference to ``X`` (arrow_slim_mpi.py:285-293); here the rows are copied to the device at call time."""
         assert X is not None
         if self._level != 0:
             raise ValueError("features enter at level 0; deeper levels receive them through the exchange")
-        self._engine.set_features(np.ascontiguousarray(X, dtype=np.float32))
+        self._engine.set_features(np.ascontiguousarray(X, dtype=_engine_dtype(self._engine)))
 
     def load_sparse_matrix_from_blocks(self, blocks) -> None:
         """``blocks`` is what ``ArrowDecompositionMPI.load_decomposition_new`` returned."""
@@ -66,9 +66,10 @@ class ArrowSlimMPI(ArrowMatrix):
 
     def zero_rhs(self, number_of_rows_per_rank: int, number_of_columns: int, dtype=np.float32) -> None:
         assert number_of_rows_per_rank >= 1 and number_of_columns >= 1
-        if np.dtype(dtype) != np.float32:
-            raise ValueError("the GPU path computes in float32 (like the reference's benchmark, arrow_bench.py:21)")
         eng = self._engine
+        if np.dtype(dtype) != _engine_dtype(eng):
+            raise ValueError(f"the decomposition was loaded as {_engine_dtype(eng)}, zero_rhs asks for {np.dtype(dtype)}: "
+                             "pass the datatype given to load_decomposition_new")
         if number_of_columns != eng.k or number_of_rows_per_rank != eng.width:
             raise ValueError(f"engine was initialised for width={eng.width}, k={eng.k}")
         eng.zero_rhs()
@@ -83,8 +84,8 @@ class ArrowSlimMPI(ArrowMatrix):
         mine = eng.result(self._level)
         parts = self.comm.allgather(mine) if self.comm.Get_size() > 1 else [mine]
         full = np.concatenate(parts) if len(parts) > 1 else parts[0]
-        if C.shape != full.shape or C.dtype != np.float32:
-            raise ValueError(f"C must be float32 of shape {full.shape}")
+        if C.shape != full.shape or C.dtype != full.dtype:
+            raise ValueError(f"C must be {full.dtype} of shape {full.shape}")
         C[:] = full
         return C
 
@@ -101,6 +102,11 @@ class ArrowSlimMPI(ArrowMatrix):
     @staticmethod
     def row_subgroup(tiles_per_side, group):
         return group
+
+
+def _engine_dtype(eng) -> np.dtype:
+    """precision of an engine (the multi-GPU engine computes in float32)"""
+    return np.dtype(getattr(eng, "dtype", np.float32))
 
 
 def _require_gpu(device: str):

@@ -37,9 +37,10 @@
 namespace {
 
 struct DenseBuf {
-    float *p = nullptr;
+    float *p = nullptr;               // element type per `dtype` (double * for ARROW_F64)
     int64_t rows = 0;
     int k = 0;
+    int dtype = ARROW_F32;
     bool owned = false;
     bool ipc = false;
     void *ipc_base = nullptr;
@@ -57,7 +58,8 @@ struct Csr {
     int64_t n_rows = 0, n_cols = 0, nnz = 0;
     int *indptr = nullptr;
     int *indices = nullptr;
-    float *vals = nullptr;
+    float *vals = nullptr;            // element type per `dtype` (double * for ARROW_F64)
+    int dtype = ARROW_F32;
     bool owns_indptr = false, owns_indices = false, owns_vals = false;
     bool may_skip = false;            // indices may contain -1 (remapped through a partial map)
     int64_t max_row_nnz = 0;
@@ -210,6 +212,11 @@ IdxMap *get_map(arrow_ctx *ctx, int h) {
 
 inline int ceil_div_i64(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+inline size_t dtype_size(int dtype) { return dtype == ARROW_F64 ? 8 : 4; }
+inline const char *dtype_name(int dtype) { return dtype == ARROW_F64 ? "float64" : "float32"; }
+// first byte of row `r` of a dense tile
+inline char *dense_row(const DenseBuf *d, int64_t r) { return (char *)d->p + (size_t)r * d->k * dtype_size(d->dtype); }
+
 // frees whatever device arrays the block owns (cudaFree waits for the device, so no launch can still read them)
 void csr_release(Csr &c) {
     if (c.owns_indptr) cudaFree(c.indptr);
@@ -242,6 +249,14 @@ __device__ __forceinline__ void f4_fma(float4 &acc, float a, const float4 &x) {
 }
 __device__ __forceinline__ void f4_add(float4 &acc, const float4 &x) {
     acc.x += x.x; acc.y += x.y; acc.z += x.z; acc.w += x.w;
+}
+__device__ __forceinline__ double2 d2_zero() { return make_double2(0.0, 0.0); }
+__device__ __forceinline__ void d2_fma(double2 &acc, double a, const double2 &x) {
+    acc.x = fma(a, x.x, acc.x);
+    acc.y = fma(a, x.y, acc.y);
+}
+__device__ __forceinline__ void d2_add(double2 &acc, const double2 &x) {
+    acc.x += x.x; acc.y += x.y;
 }
 
 struct SpmmArgs {
@@ -1273,6 +1288,322 @@ __global__ void __launch_bounds__(128) k_spmm_long_reduce(const int *__restrict_
 }
 
 // ------------------------------------------------------------------------------------------------
+// float64 (ARROW_F64 CSR values and tiles; one GPU).  The tile kernel keeps the pipeline of k_spmm_tiles_v1 -- the CSR
+// slices streamed by cp.async.bulk on an mbarrier, two stages, persistent CTAs on the atomic ticket, a lane group per
+// row -- with X and C moved as double2 (16 B: the vector path needs k % 2 == 0) and 8-byte values in shared memory.
+// Every element is one fma chain in entry order (after the old C row or the addend), so a result does not depend on
+// the grid.  The generic and long-row kernels are the fp32 ones in double.
+// ------------------------------------------------------------------------------------------------
+struct SpmmArgsF64 {
+    const int *__restrict__ indptr;
+    const int *__restrict__ indices;
+    const double *__restrict__ vals;
+    const double *__restrict__ X;
+    double *__restrict__ C;
+    const int *__restrict__ rowmap;      // nullptr: identity
+    long long n_rows;
+    int k;
+    int k2;                              // k / 2 (tile kernel)
+    int long_threshold;
+    const double *__restrict__ add_src;  // optional addend: C[r] = sum + add_src[add_map[r]] (add_map[r] >= 0)
+    const int *__restrict__ add_map;
+};
+
+struct TileArgsF64 {
+    SpmmArgsF64 a;
+    const int4 *__restrict__ tiles;
+    int n_tiles;
+    int skip;            // indices may hold -1
+    int *ticket;         // dynamic tile scheduler: [0] next tile
+    int l2_hints;        // bit 0: X gathers evict_last, bit 1: CSR / C streams evict_first
+};
+
+// one stage: row pointers (int) | indices (int) | values (double), every part 16-byte aligned for cp.async.bulk
+struct TileCfgF64 {
+    static constexpr int PTR_WORDS = TILE_ROWS + 8;
+    static constexpr int NNZ_WORDS = TILE_NNZ + 8;
+    static constexpr int IDX_OFF = PTR_WORDS * 4;
+    static constexpr int VAL_OFF = IDX_OFF + NNZ_WORDS * 4;
+    static constexpr int STAGE_BYTES = VAL_OFF + NNZ_WORDS * 8;
+    static constexpr size_t SMEM_BYTES = (size_t)TILE_STAGES * STAGE_BYTES + 64;
+    static_assert(IDX_OFF % 16 == 0 && VAL_OFF % 16 == 0 && STAGE_BYTES % 16 == 0, "bulk copies need 16-byte alignment");
+};
+
+__device__ __forceinline__ double2 ldg_d2_hint(const double2 *ptr, uint64_t pol) {
+    double2 r;
+    asm("ld.global.nc.L2::cache_hint.v2.f64 {%0,%1}, [%2], %3;" : "=d"(r.x), "=d"(r.y) : "l"(ptr), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ double2 ld_d2_hint(const double2 *ptr, uint64_t pol) {      // coherent load (C tile RMW)
+    double2 r;
+    asm("ld.global.L2::cache_hint.v2.f64 {%0,%1}, [%2], %3;" : "=d"(r.x), "=d"(r.y) : "l"(ptr), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ void st_d2_hint(double2 *ptr, const double2 &v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1,%2}, %3;" ::"l"(ptr), "d"(v.x), "d"(v.y), "l"(pol) : "memory");
+}
+
+// G lanes own a row, VPL double2 each.  A value takes 2 registers here (1 in fp32): the values are read from shared memory
+// only when the gathers of a batch are back, the UNROLL-8 batch of the narrow shapes shrinks to 4, and accumulate mode adds
+// the old C row after the products instead of starting from it: every instance stays inside the 64 registers of
+// __launch_bounds__(256, 4) without spills (-Xptxas -v).
+template <int G, int VPL, bool ROWMAP, bool ACC>
+__global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles_f64(TileArgsF64 t) {
+    using Cfg = TileCfgF64;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)TILE_STAGES * Cfg::STAGE_BYTES);
+    const SpmmArgsF64 &a = t.a;
+    constexpr int RPW = 32 / G;
+    constexpr int UNROLL = (VPL >= 4) ? 2 : 4;
+    constexpr int TAIL = (UNROLL >= 4) ? UNROLL / 2 : UNROLL;     // predicated tail batches
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const bool EXACT = (a.k2 == G * VPL);                         // every lane owns valid columns
+    const int gl = lane % G;
+    const int gi = lane / G;
+    const int k2 = a.k2;
+    const double2 *__restrict__ Xl = reinterpret_cast<const double2 *>(a.X) + gl;
+    double2 *__restrict__ Cl = reinterpret_cast<double2 *>(a.C) + gl;
+    const uint64_t pol_keep = (t.l2_hints & 1) ? l2_policy_evict_last() : l2_policy_evict_normal();
+    const uint64_t pol_stream = (t.l2_hints & 2) ? l2_policy_evict_first() : l2_policy_evict_normal();
+
+    if (threadIdx.x == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    // the slices start at the 4-entry boundary below the tile and round up to 4 entries: 16-byte copies of the 4-byte
+    // arrays, 32-byte copies of the values (the upload leaves 8 entries of slack behind every array)
+    auto issue_csr = [&](int tile, int st) {
+        const int4 d = __ldg(t.tiles + tile);
+        const int rb4 = d.x & ~3;
+        const int a0 = d.z & ~3;
+        const uint32_t ptr_bytes = (uint32_t)(((d.y - rb4 + 1) + 3) & ~3) * 4u;
+        const uint32_t n_nnz = (uint32_t)(((d.w - a0) + 3) & ~3);
+        unsigned char *sp = smem_raw + (size_t)st * Cfg::STAGE_BYTES;
+        mbar_expect_tx(&bars[st], ptr_bytes + n_nnz * 12u);
+        bulk_g2s_hint(sp, a.indptr + rb4, ptr_bytes, &bars[st], pol_stream);
+        if (n_nnz) {
+            bulk_g2s_hint(sp + Cfg::IDX_OFF, a.indices + a0, n_nnz * 4u, &bars[st], pol_stream);
+            bulk_g2s_hint(sp + Cfg::VAL_OFF, a.vals + a0, n_nnz * 8u, &bars[st], pol_stream);
+        }
+    };
+
+    __shared__ int s_next[TILE_STAGES];
+    uint32_t phase = 0u;                  // bit s = parity the next wait on stage s expects
+    int tile = blockIdx.x;
+    if (tile < t.n_tiles && threadIdx.x == 0) issue_csr(tile, 0);
+    for (int st = 0; tile < t.n_tiles; st ^= 1) {
+        if (threadIdx.x == 0) {
+            const int next = atomicAdd(t.ticket, 1) + (int)gridDim.x;
+            s_next[st] = next;
+            if (next < t.n_tiles) issue_csr(next, st ^ 1);
+        }
+        const int4 d = __ldg(t.tiles + tile);
+        mbar_wait(&bars[st], (phase >> st) & 1u);
+        phase ^= (1u << st);
+        const unsigned char *sp = smem_raw + (size_t)st * Cfg::STAGE_BYTES;
+        const int *s_ptr = reinterpret_cast<const int *>(sp) + (d.x - (d.x & ~3));
+        const int a0 = d.z & ~3;
+        const int *s_idx = reinterpret_cast<const int *>(sp + Cfg::IDX_OFF) - a0;        // index with global nnz offsets
+        const double *s_val = reinterpret_cast<const double *>(sp + Cfg::VAL_OFF) - a0;
+        const int n_rows_tile = d.y - d.x;
+
+        for (int lr = warp * RPW + gi; lr < n_rows_tile; lr += (TILE_THREADS / 32) * RPW) {
+            const int s = s_ptr[lr];
+            const int e = s_ptr[lr + 1];
+            if (e - s > a.long_threshold) continue;
+            const long long row = (long long)d.x + lr;
+            long long orow = row;
+            if (ROWMAP) {
+                orow = __ldg(a.rowmap + row);
+                if (orow < 0) continue;
+            }
+            // the addend is read first so that its latency hides behind the gathers
+            double2 acc[VPL];
+            double2 *cr = Cl + orow * k2;
+#pragma unroll
+            for (int i = 0; i < VPL; ++i) acc[i] = d2_zero();
+            if (a.add_map != nullptr) {
+                const int am = __ldg(a.add_map + row);
+                if (am >= 0) {
+                    const double2 *ar = reinterpret_cast<const double2 *>(a.add_src) + (long long)am * k2 + gl;
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i)
+                        if (gl + i * G < k2) d2_add(acc[i], ld_d2_hint(ar + i * G, pol_stream));
+                }
+            }
+            int p = s;
+            if (EXACT && !t.skip) {
+                // unpredicated batches: full UNROLL batches, then the remainder as 2 / 1
+                auto batch = [&](auto n_tag) {
+                    constexpr int N = decltype(n_tag)::value;
+                    double2 x[N][VPL];
+#pragma unroll
+                    for (int u = 0; u < N; ++u) {
+                        const double2 *xr = Xl + (long long)s_idx[p + u] * k2;
+#pragma unroll
+                        for (int i = 0; i < VPL; ++i) x[u][i] = ldg_d2_hint(xr + i * G, pol_keep);
+                    }
+#pragma unroll
+                    for (int u = 0; u < N; ++u) {
+                        const double v = s_val[p + u];
+#pragma unroll
+                        for (int i = 0; i < VPL; ++i) d2_fma(acc[i], v, x[u][i]);
+                    }
+                    p += N;
+                };
+                while (p + UNROLL <= e) batch(std::integral_constant<int, UNROLL>{});
+                if constexpr (UNROLL >= 4) { if (e - p >= 2) batch(std::integral_constant<int, 2>{}); }
+                if (e - p >= 1) batch(std::integral_constant<int, 1>{});
+            }
+            // tail (and the general case): predicated batches of TAIL; a skipped entry (column -1) adds nothing
+            for (; p < e; p += TAIL) {
+                double2 x[TAIL][VPL];
+#pragma unroll
+                for (int u = 0; u < TAIL; ++u) {
+                    const int c = (p + u < e) ? s_idx[p + u] : -1;
+                    const double2 *xr = Xl + (long long)c * k2;             // c = -1: address arithmetic only
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i)
+                        x[u][i] = (c >= 0 && gl + i * G < k2) ? ldg_d2_hint(xr + i * G, pol_keep) : d2_zero();
+                }
+#pragma unroll
+                for (int u = 0; u < TAIL; ++u) {
+                    const double v = (p + u < e) ? s_val[p + u] : 0.0;     // 0 * 0 added: no rounding
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i) d2_fma(acc[i], v, x[u][i]);
+                }
+            }
+            // accumulate mode: C += the products (only this group ever touches the row: the row maps are injective)
+#pragma unroll
+            for (int i = 0; i < VPL; ++i) {
+                if (gl + i * G < k2) {
+                    if (ACC) d2_add(acc[i], ld_d2_hint(cr + i * G, pol_stream));
+                    st_d2_hint(cr + i * G, acc[i], pol_stream);
+                }
+            }
+        }
+        __syncthreads();            // stage `st` may be refilled by the next iteration's copy
+        tile = s_next[st];
+    }
+}
+
+// odd k or k > 256: warp per row, lanes over columns, scalar accesses
+template <bool ROWMAP, bool ACC>
+__global__ void __launch_bounds__(256) k_spmm_generic_f64(SpmmArgsF64 a) {
+    const int lane = threadIdx.x & 31;
+    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
+    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    for (long long row = warp_id; row < a.n_rows; row += warps_total) {
+        const int s = __ldg(a.indptr + row);
+        const int e = __ldg(a.indptr + row + 1);
+        if (e - s > a.long_threshold) continue;
+        long long orow = row;
+        if (ROWMAP) {
+            orow = __ldg(a.rowmap + row);
+            if (orow < 0) continue;
+        }
+        double *crow = a.C + orow * a.k;
+        for (int c0 = 0; c0 < a.k; c0 += 128) {
+            double acc[4] = {0.0, 0.0, 0.0, 0.0};
+            for (int p = s; p < e; ++p) {
+                const int c = __ldg(a.indices + p);
+                const double v = __ldg(a.vals + p);
+                if (c < 0) continue;
+                const double *xr = a.X + (long long)c * a.k;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int col = c0 + lane + 32 * i;
+                    if (col < a.k) acc[i] = fma(v, __ldg(xr + col), acc[i]);
+                }
+            }
+            const int am = (a.add_map != nullptr) ? __ldg(a.add_map + row) : -1;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int col = c0 + lane + 32 * i;
+                if (col < a.k) {
+                    double *dst = crow + col;
+                    double r = ACC ? (*dst + acc[i]) : acc[i];
+                    if (am >= 0) r += a.add_src[(long long)am * a.k + col];
+                    *dst = r;
+                }
+            }
+        }
+    }
+}
+
+// long rows: segment partials to scratch, then the in-order reduction (k_spmm_long_partial / k_spmm_long_reduce)
+struct LongArgsF64 {
+    const LongTask *__restrict__ tasks;
+    const int *__restrict__ indices;
+    const double *__restrict__ vals;
+    const double *__restrict__ X;
+    double *__restrict__ scratch;     // [slot][k]
+    int k;
+};
+
+__global__ void __launch_bounds__(256) k_spmm_long_partial_f64(LongArgsF64 a) {
+    extern __shared__ double red_f64[];   // [warps][k]
+    const LongTask t = a.tasks[blockIdx.x];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    for (int c0 = 0; c0 < a.k; c0 += 128) {
+        double acc[4] = {0.0, 0.0, 0.0, 0.0};
+        for (int p = t.begin + warp; p < t.end; p += nwarps) {
+            const int c = __ldg(a.indices + p);
+            const double v = __ldg(a.vals + p);
+            if (c < 0) continue;
+            const double *xr = a.X + (long long)c * a.k;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int col = c0 + lane + 32 * i;
+                if (col < a.k) acc[i] = fma(v, __ldg(xr + col), acc[i]);
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int col = c0 + lane + 32 * i;
+            if (col < a.k) red_f64[warp * a.k + col] = acc[i];
+        }
+    }
+    __syncthreads();
+    for (int col = threadIdx.x; col < a.k; col += blockDim.x) {
+        double sum = 0.0;
+        for (int w = 0; w < nwarps; ++w) sum += red_f64[w * a.k + col];
+        a.scratch[(long long)t.slot * a.k + col] = sum;
+    }
+}
+
+template <bool ROWMAP, bool ACC>
+__global__ void __launch_bounds__(128) k_spmm_long_reduce_f64(const int *__restrict__ long_rows,
+                                                              const int *__restrict__ long_first,
+                                                              const double *__restrict__ scratch,
+                                                              double *__restrict__ C, const int *__restrict__ rowmap, int k,
+                                                              const double *__restrict__ add_src,
+                                                              const int *__restrict__ add_map) {
+    const int r = long_rows[blockIdx.x];
+    long long orow = r;
+    if (ROWMAP) {
+        orow = rowmap[r];
+        if (orow < 0) return;
+    }
+    double *crow = C + orow * k;
+    const int s0 = long_first[blockIdx.x], s1 = long_first[blockIdx.x + 1];
+    for (int col = threadIdx.x; col < k; col += blockDim.x) {
+        double sum = 0.0;
+        for (int s = s0; s < s1; ++s) sum += scratch[(long long)s * k + col];
+        if (add_map != nullptr) {
+            const int am = add_map[r];
+            if (am >= 0) sum += add_src[(long long)am * k + col];
+        }
+        double *dst = crow + col;
+        *dst = ACC ? (*dst + sum) : sum;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // exchange kernels: dst[r] (+)= src[map[r]]
 // ------------------------------------------------------------------------------------------------
 constexpr int MAX_SRC = 16;
@@ -1316,8 +1647,10 @@ __global__ void __launch_bounds__(256) k_gather_rows(VT *__restrict__ dst, const
                 if (v0 + j * G < vec_per_row) {
                     if (ACC) {
                         VT old = dp[v0 + j * G];
-                        if constexpr (sizeof(VT) == 16) {
+                        if constexpr (std::is_same<VT, float4>::value) {
                             f4_add(val[j], old);
+                        } else if constexpr (std::is_same<VT, double2>::value) {
+                            d2_add(val[j], old);
                         } else {
                             val[j] += old;
                         }
@@ -1704,6 +2037,133 @@ int pick_variant(int k) {
     return 3;
 }
 
+// ---- float64 dispatch (one GPU): the tile kernel for even k <= 256, the generic kernel otherwise, long rows as fp32 ----
+template <int G, int VPL, bool ROWMAP, bool ACC>
+int launch_tiles_f64_one(arrow_ctx *ctx, const TileArgsF64 &t) {
+    constexpr size_t SMEM = TileCfgF64::SMEM_BYTES;
+    auto fn = k_spmm_tiles_f64<G, VPL, ROWMAP, ACC>;
+    static bool attr_set[64] = {};            /* function attributes are per device */
+    static int occ_dev[64] = {};
+    const int dv = ctx->device & 63;
+    if (!attr_set[dv]) {
+        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
+        attr_set[dv] = true;
+    }
+    const int occ = occ_dev[dv];
+    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
+    int sms = ctx->sm_count;
+    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
+    int grid = (int)std::min<long long>((long long)per_sm * sms, t.n_tiles);
+    cudaMemsetAsync(t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
+    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(t);
+    ctx->launches++;
+    return ARROW_OK;
+}
+
+template <int G, int VPL>
+int launch_tiles_f64_epi(arrow_ctx *ctx, const TileArgsF64 &t, bool rowmap, bool acc) {
+    if (rowmap && acc) return launch_tiles_f64_one<G, VPL, true, true>(ctx, t);
+    if (rowmap) return launch_tiles_f64_one<G, VPL, true, false>(ctx, t);
+    if (acc) return launch_tiles_f64_one<G, VPL, false, true>(ctx, t);
+    return launch_tiles_f64_one<G, VPL, false, false>(ctx, t);
+}
+
+// (lanes per row, double2 per lane) from k2 = k/2 the way launch_tiles picks them from k/4: ~8 lanes per row
+int launch_tiles_f64(arrow_ctx *ctx, const TileArgsF64 &t, bool rowmap, bool acc) {
+    const int k2 = t.a.k2;
+    const int vpl = (k2 >= 32) ? 4 : (k2 >= 8 ? 2 : 1);
+    const int lanes = (k2 + vpl - 1) / vpl;           // <= 32: k2 <= 128
+    int g = 1;
+    while (g < lanes) g <<= 1;
+#define TF(GG, VV) \
+    if (g == GG && vpl == VV) return launch_tiles_f64_epi<GG, VV>(ctx, t, rowmap, acc)
+    TF(1, 1); TF(2, 1); TF(4, 1); TF(8, 1);
+    TF(4, 2); TF(8, 2); TF(16, 2);
+    TF(8, 4); TF(16, 4); TF(32, 4);
+#undef TF
+    return fail(ctx, ARROW_ERR_UNSUPPORTED, "no float64 tile kernel for k2=%d vpl=%d", k2, vpl);
+}
+
+// the product of spmm_impl for float64 operands; `a` carries the validated operands (value / tile pointers are double)
+int spmm_f64(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool rowmap, bool acc) {
+    SpmmArgsF64 b;
+    b.indptr = a.indptr;
+    b.indices = a.indices;
+    b.vals = reinterpret_cast<const double *>(a.vals);
+    b.X = reinterpret_cast<const double *>(a.X);
+    b.C = reinterpret_cast<double *>(a.C);
+    b.rowmap = a.rowmap;
+    b.n_rows = a.n_rows;
+    b.k = a.k;
+    b.k2 = a.k / 2;
+    b.long_threshold = a.long_threshold;
+    b.add_src = reinterpret_cast<const double *>(a.add_src);
+    b.add_map = a.add_map;
+    const int k = a.k;
+    const int lane = ctx->cur_lane;
+    cudaStream_t stream = cur_stream(ctx);
+    if (k % 2 != 0 || k > 256) {
+        const long long ctas = (A->n_rows + 7) / 8;
+#define LAUNCH_G64(KERNEL)                                                                            \
+    do {                                                                                              \
+        auto fn = KERNEL;                                                                             \
+        int grid = grid_for(ctx, (const void *)fn, 256, 0, ctas);                                     \
+        fn<<<grid, 256, 0, stream>>>(b);                                                              \
+    } while (0)
+        if (rowmap && acc) LAUNCH_G64((k_spmm_generic_f64<true, true>));
+        else if (rowmap) LAUNCH_G64((k_spmm_generic_f64<true, false>));
+        else if (acc) LAUNCH_G64((k_spmm_generic_f64<false, true>));
+        else LAUNCH_G64((k_spmm_generic_f64<false, false>));
+#undef LAUNCH_G64
+        ctx->launches++;
+    } else if (A->n_tiles > 0) {
+        TileArgsF64 t;
+        t.a = b;
+        t.tiles = A->tiles;
+        t.n_tiles = A->n_tiles;
+        t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
+        t.ticket = ctx->tile_ticket + 2 * lane;
+        t.l2_hints = (rowmap || acc) ? ctx->l2_hints_fused : ctx->l2_hints_plain;
+        const int rc = launch_tiles_f64(ctx, t, rowmap, acc);
+        if (rc != ARROW_OK) return rc;
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+
+    if (A->n_long_tasks > 0) {
+        const size_t need = (size_t)A->n_long_tasks * k * sizeof(double);
+        if (need > ctx->long_scratch_bytes[lane]) {
+            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
+            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
+            ctx->long_scratch[lane] = nullptr;
+            ctx->long_scratch_bytes[lane] = 0;
+            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
+            ctx->long_scratch_bytes[lane] = need;
+        }
+        double *scr = reinterpret_cast<double *>(ctx->long_scratch[lane]);
+        LongArgsF64 la;
+        la.tasks = A->long_tasks;
+        la.indices = b.indices;
+        la.vals = b.vals;
+        la.X = b.X;
+        la.scratch = scr;
+        la.k = k;
+        const size_t smem = (size_t)8 * k * sizeof(double);
+        if (smem > 48 * 1024)
+            CUDA_TRY(ctx, cudaFuncSetAttribute(k_spmm_long_partial_f64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_spmm_long_partial_f64<<<A->n_long_tasks, 256, smem, stream>>>(la);
+        ctx->launches++;
+        if (rowmap && acc) k_spmm_long_reduce_f64<true, true><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
+        else if (rowmap) k_spmm_long_reduce_f64<true, false><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
+        else if (acc) k_spmm_long_reduce_f64<false, true><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
+        else k_spmm_long_reduce_f64<false, false><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
+    return ARROW_OK;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1921,7 +2381,9 @@ static int build_long_rows(arrow_ctx *ctx, Csr &c, const std::vector<int> &h_ind
 
 // device side of arrow_csr_upload; on failure the caller releases whatever `c` already owns
 static int csr_fill(arrow_ctx *ctx, Csr &c, int64_t n_rows, int64_t n_cols, int64_t nnz, const std::vector<int> &h_indptr,
-                    const void *indices, int indices_bytes, const float *data) {
+                    const void *indices, int indices_bytes, const void *data, int dtype) {
+    const size_t esize = dtype_size(dtype);
+    c.dtype = dtype;
     c.n_rows = n_rows;
     c.n_cols = n_cols;
     c.nnz = nnz;
@@ -1931,9 +2393,9 @@ static int csr_fill(arrow_ctx *ctx, Csr &c, int64_t n_rows, int64_t n_cols, int6
     CUDA_TRY(ctx, cudaMemcpyAsync(c.indptr, h_indptr.data(), ((size_t)n_rows + 1) * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     const size_t nz = (size_t)nnz + 8;                       // slack: bulk copies round up to 16 bytes
     CUDA_TRY(ctx, cudaMalloc(&c.indices, nz * sizeof(int)));
-    CUDA_TRY(ctx, cudaMalloc(&c.vals, nz * sizeof(float)));
+    CUDA_TRY(ctx, cudaMalloc(&c.vals, nz * esize));
     CUDA_TRY(ctx, cudaMemsetAsync(c.indices, 0, nz * sizeof(int), ctx->stream));
-    CUDA_TRY(ctx, cudaMemsetAsync(c.vals, 0, nz * sizeof(float), ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(c.vals, 0, nz * esize, ctx->stream));
     DevTmp wide, bad;
     int hbad = 0;
     if (nnz > 0) {
@@ -1952,7 +2414,10 @@ static int csr_fill(arrow_ctx *ctx, Csr &c, int64_t n_rows, int64_t n_cols, int6
         ctx->launches++;
         CUDA_TRY(ctx, cudaMemcpyAsync(&hbad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
         if (data) {
-            CUDA_TRY(ctx, cudaMemcpyAsync(c.vals, data, (size_t)nnz * 4, cudaMemcpyHostToDevice, ctx->stream));
+            CUDA_TRY(ctx, cudaMemcpyAsync(c.vals, data, (size_t)nnz * esize, cudaMemcpyHostToDevice, ctx->stream));
+        } else if (dtype == ARROW_F64) {
+            k_fill<double><<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(reinterpret_cast<double *>(c.vals), 1.0, nnz);
+            ctx->launches++;
         } else {
             k_fill<float><<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(c.vals, 1.0f, nnz);
             ctx->launches++;
@@ -1966,8 +2431,8 @@ static int csr_fill(arrow_ctx *ctx, Csr &c, int64_t n_rows, int64_t n_cols, int6
     return ARROW_OK;
 }
 
-int arrow_csr_upload(arrow_ctx *ctx, int64_t n_rows, int64_t n_cols, int64_t nnz, const void *indptr, int indptr_bytes,
-                     const void *indices, int indices_bytes, const float *data, int *csr_out) {
+static int csr_upload(arrow_ctx *ctx, int64_t n_rows, int64_t n_cols, int64_t nnz, const void *indptr, int indptr_bytes,
+                      const void *indices, int indices_bytes, const void *data, int dtype, int *csr_out) {
     CHECK_CTX(ctx);
     if (!csr_out || !indptr || (nnz > 0 && !indices)) return fail(ctx, ARROW_ERR_ARG, "null pointer argument");
     if (n_rows < 0 || n_cols < 0 || nnz < 0) return fail(ctx, ARROW_ERR_ARG, "negative size");
@@ -2002,7 +2467,7 @@ int arrow_csr_upload(arrow_ctx *ctx, int64_t n_rows, int64_t n_cols, int64_t nnz
         return fail(ctx, ARROW_ERR_ARG, "indptr[n_rows]-indptr[0] = %d but nnz = %lld", h_indptr[n_rows], (long long)nnz);
 
     Csr c;
-    const int rc = csr_fill(ctx, c, n_rows, n_cols, nnz, h_indptr, indices, indices_bytes, data);
+    const int rc = csr_fill(ctx, c, n_rows, n_cols, nnz, h_indptr, indices, indices_bytes, data, dtype);
     if (rc != ARROW_OK) {
         cudaStreamSynchronize(ctx->stream);                  // nothing may still write into what is released next
         cudaGetLastError();
@@ -2014,6 +2479,16 @@ int arrow_csr_upload(arrow_ctx *ctx, int64_t n_rows, int64_t n_cols, int64_t nnz
     ctx->csrs[h] = c;
     *csr_out = h;
     return ARROW_OK;
+}
+
+int arrow_csr_upload(arrow_ctx *ctx, int64_t n_rows, int64_t n_cols, int64_t nnz, const void *indptr, int indptr_bytes,
+                     const void *indices, int indices_bytes, const float *data, int *csr_out) {
+    return csr_upload(ctx, n_rows, n_cols, nnz, indptr, indptr_bytes, indices, indices_bytes, data, ARROW_F32, csr_out);
+}
+
+int arrow_csr_upload_f64(arrow_ctx *ctx, int64_t n_rows, int64_t n_cols, int64_t nnz, const void *indptr, int indptr_bytes,
+                         const void *indices, int indices_bytes, const double *data, int *csr_out) {
+    return csr_upload(ctx, n_rows, n_cols, nnz, indptr, indptr_bytes, indices, indices_bytes, data, ARROW_F64, csr_out);
 }
 
 int arrow_csr_free(arrow_ctx *ctx, int csr) {
@@ -2194,13 +2669,15 @@ int arrow_map_d2h(arrow_ctx *ctx, int map, int32_t *host, int64_t n) {
 }
 
 // ---- dense --------------------------------------------------------------------------------------
-int arrow_dense_alloc(arrow_ctx *ctx, int64_t rows, int k, int *buf_out) {
+int arrow_dense_alloc_dtype(arrow_ctx *ctx, int64_t rows, int k, int dtype, int *buf_out) {
     CHECK_CTX(ctx);
     if (!buf_out || rows < 0 || k < 1) return fail(ctx, ARROW_ERR_ARG, "bad dense shape %lld x %d", (long long)rows, k);
+    if (dtype != ARROW_F32 && dtype != ARROW_F64) return fail(ctx, ARROW_ERR_ARG, "unknown dtype %d", dtype);
     DenseBuf d;
     d.rows = rows;
     d.k = k;
-    const size_t bytes = std::max<size_t>((size_t)rows * (size_t)k * 4, 16);
+    d.dtype = dtype;
+    const size_t bytes = std::max<size_t>((size_t)rows * (size_t)k * dtype_size(dtype), 16);
     cudaError_t e = cudaMalloc(&d.p, bytes);
     if (e != cudaSuccess) {
         cudaGetLastError();
@@ -2213,6 +2690,19 @@ int arrow_dense_alloc(arrow_ctx *ctx, int64_t rows, int k, int *buf_out) {
     const int h = new_slot(ctx->dense);
     ctx->dense[h] = d;
     *buf_out = h;
+    return ARROW_OK;
+}
+
+int arrow_dense_alloc(arrow_ctx *ctx, int64_t rows, int k, int *buf_out) {
+    return arrow_dense_alloc_dtype(ctx, rows, k, ARROW_F32, buf_out);
+}
+
+int arrow_dense_dtype(arrow_ctx *ctx, int buf, int *dtype) {
+    CHECK_CTX(ctx);
+    DenseBuf *d = get_dense(ctx, buf);
+    if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", buf);
+    if (!dtype) return fail(ctx, ARROW_ERR_ARG, "dtype is null");
+    *dtype = d->dtype;
     return ARROW_OK;
 }
 
@@ -2234,7 +2724,11 @@ int arrow_dense_fill(arrow_ctx *ctx, int buf, float value) {
     const long long n = (long long)d->rows * d->k;
     if (n == 0) return ARROW_OK;
     if (value == 0.f) {
-        CUDA_TRY(ctx, cudaMemsetAsync(d->p, 0, (size_t)n * 4, ctx->stream));
+        CUDA_TRY(ctx, cudaMemsetAsync(d->p, 0, (size_t)n * dtype_size(d->dtype), ctx->stream));
+    } else if (d->dtype == ARROW_F64) {
+        k_fill<double><<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(reinterpret_cast<double *>(d->p), (double)value, n);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
     } else {
         k_fill<float><<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(d->p, value, n);
         ctx->launches++;
@@ -2243,25 +2737,25 @@ int arrow_dense_fill(arrow_ctx *ctx, int buf, float value) {
     return ARROW_OK;
 }
 
-int arrow_dense_h2d(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, const float *host) {
+int arrow_dense_h2d(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, const void *host) {
     CHECK_CTX(ctx);
     DenseBuf *d = get_dense(ctx, buf);
     if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", buf);
     if (!host || row0 < 0 || rows < 0 || row0 + rows > d->rows)
         return fail(ctx, ARROW_ERR_ARG, "h2d rows [%lld,%lld) outside tile of %lld rows", (long long)row0, (long long)(row0 + rows), (long long)d->rows);
     if (rows == 0) return ARROW_OK;
-    CUDA_TRY(ctx, cudaMemcpyAsync(d->p + (size_t)row0 * d->k, host, (size_t)rows * d->k * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(d, row0), host, (size_t)rows * d->k * dtype_size(d->dtype), cudaMemcpyHostToDevice, ctx->stream));
     return ARROW_OK;
 }
 
-int arrow_dense_d2h(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, float *host) {
+int arrow_dense_d2h(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, void *host) {
     CHECK_CTX(ctx);
     DenseBuf *d = get_dense(ctx, buf);
     if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", buf);
     if (!host || row0 < 0 || rows < 0 || row0 + rows > d->rows)
         return fail(ctx, ARROW_ERR_ARG, "d2h rows [%lld,%lld) outside tile of %lld rows", (long long)row0, (long long)(row0 + rows), (long long)d->rows);
     if (rows == 0) return ARROW_OK;
-    CUDA_TRY(ctx, cudaMemcpyAsync(host, d->p + (size_t)row0 * d->k, (size_t)rows * d->k * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(host, dense_row(d, row0), (size_t)rows * d->k * dtype_size(d->dtype), cudaMemcpyDeviceToHost, ctx->stream));
     return ARROW_OK;
 }
 
@@ -2270,10 +2764,11 @@ int arrow_dense_copy(arrow_ctx *ctx, int dst, int64_t dst_row0, int src, int64_t
     DenseBuf *a = get_dense(ctx, dst), *b = get_dense(ctx, src);
     if (!a || !b) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle");
     if (a->k != b->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch %d vs %d", a->k, b->k);
+    if (a->dtype != b->dtype) return fail(ctx, ARROW_ERR_ARG, "dtype mismatch: %s vs %s", dtype_name(a->dtype), dtype_name(b->dtype));
     if (rows < 0 || dst_row0 < 0 || src_row0 < 0 || dst_row0 + rows > a->rows || src_row0 + rows > b->rows)
         return fail(ctx, ARROW_ERR_ARG, "copy range outside tiles");
     if (rows == 0) return ARROW_OK;
-    CUDA_TRY(ctx, cudaMemcpyAsync(a->p + (size_t)dst_row0 * a->k, b->p + (size_t)src_row0 * b->k, (size_t)rows * a->k * 4,
+    CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(a, dst_row0), dense_row(b, src_row0), (size_t)rows * a->k * dtype_size(a->dtype),
                                   cudaMemcpyDeviceToDevice, cur_stream(ctx)));
     return ARROW_OK;
 }
@@ -2376,6 +2871,10 @@ static int spmm_impl(arrow_ctx *ctx, const SpmmCall &q) {
     DenseBuf *C = q.c_buf >= 0 ? get_dense(ctx, q.c_buf) : nullptr;
     if (!A) return fail(ctx, ARROW_ERR_HANDLE, "bad csr handle %d", q.csr);
     if (!X) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x=%d)", q.x_buf);
+    // every operand of a launch has the block's precision
+    if (X->dtype != A->dtype || (C && C->dtype != A->dtype))
+        return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, X is %s, C is %s", dtype_name(A->dtype),
+                    dtype_name(X->dtype), C ? dtype_name(C->dtype) : "-");
     PtrTable *OT = nullptr;
     if (q.out_table >= 0) {
         if (q.out_table >= (int)ctx->ptrtabs.size() || !ctx->ptrtabs[q.out_table].live)
@@ -2395,6 +2894,7 @@ static int spmm_impl(arrow_ctx *ctx, const SpmmCall &q) {
     if (q.x2_buf >= 0) {
         X2 = get_dense(ctx, q.x2_buf);
         if (!X2) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x2=%d)", q.x2_buf);
+        if (X2->dtype != A->dtype) return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, X2 is %s", dtype_name(A->dtype), dtype_name(X2->dtype));
         if (X2->k != X->k) return fail(ctx, ARROW_ERR_ARG, "X2 has %d feature columns, X has %d", X2->k, X->k);
         if (q.x_split < 0 || q.x_split > X->rows || q.x_split > A->n_cols)
             return fail(ctx, ARROW_ERR_ARG, "x_split %lld outside X (%lld rows) / the block's %lld columns", (long long)q.x_split, (long long)X->rows, (long long)A->n_cols);
@@ -2439,11 +2939,19 @@ static int spmm_impl(arrow_ctx *ctx, const SpmmCall &q) {
         IdxMap *am = get_map(ctx, q.add_map);
         if (!S || !am) return fail(ctx, ARROW_ERR_HANDLE, "bad addend handles (buf=%d map=%d)", q.add_buf, q.add_map);
         if (S->k != k) return fail(ctx, ARROW_ERR_ARG, "addend has %d feature columns, expected %d", S->k, k);
+        if (S->dtype != A->dtype) return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, the addend is %s", dtype_name(A->dtype), dtype_name(S->dtype));
         if (am->n < A->n_rows) return fail(ctx, ARROW_ERR_ARG, "addend map has %lld entries, block has %lld rows", (long long)am->n, (long long)A->n_rows);
         if (am->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "addend map reaches row %lld, addend tile has %lld rows", (long long)am->limit, (long long)S->rows);
         if (C && S->p == C->p) return fail(ctx, ARROW_ERR_ARG, "addend and C must not alias");
         a.add_src = S->p;
         a.add_map = am->p;
+    }
+    if (A->dtype == ARROW_F64) {
+        // float64 runs the one-GPU product: no two-part operand, no pointer table, no kernel override
+        if (X2 || OT) return fail(ctx, ARROW_ERR_UNSUPPORTED, "float64 has no two-part X operand or pointer-table epilogue (one GPU only)");
+        if (q.variant != ARROW_VARIANT_AUTO && q.variant != ARROW_VARIANT_TILES)
+            return fail(ctx, ARROW_ERR_UNSUPPORTED, "float64 has no kernel variant override (variant %d)", q.variant);
+        return spmm_f64(ctx, A, a, rm != nullptr, acc);
     }
     int variant = q.variant;
     if (variant == ARROW_VARIANT_AUTO) variant = pick_variant(k);
@@ -2557,6 +3065,7 @@ int arrow_ptrtable_upload(arrow_ctx *ctx, const int *bufs, int n_bufs, const int
         if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", bufs[b]);
         if (b == 0) k = d->k;
         else if (d->k != k) return fail(ctx, ARROW_ERR_ARG, "tiles of a pointer table must share the feature width");
+        if (d->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "pointer tables are float32 only");
         bases[b] = (unsigned long long)d->p;
         rows_of[b] = d->rows;
     }
@@ -2617,8 +3126,9 @@ static int gather_common(arrow_ctx *ctx, DenseBuf *D, const float *src, const Mu
     const long long n_rows = m->n;
     if (n_rows == 0) return ARROW_OK;
     const int k = D->k;
-    const bool vec = (k % 4 == 0);
-    const int vpr = vec ? k / 4 : k;
+    const bool f64 = D->dtype == ARROW_F64;
+    const bool vec = f64 ? (k % 2 == 0) : (k % 4 == 0);        // 16-byte vectors: float4 / double2
+    const int vpr = vec ? (f64 ? k / 2 : k / 4) : k;
     int g = 1;
     while (g < vpr && g < 32) g <<= 1;                       // lanes per row
     if (g > 8 && vpr <= 32) g = 8;                           // 8 lanes x 4 vectors cover k <= 128 in one pass
@@ -2640,7 +3150,10 @@ static int gather_common(arrow_ctx *ctx, DenseBuf *D, const float *src, const Mu
             default: LAUNCH_GA(VT, 32, ACCV, MULTIV); break;                                                     \
         }                                                                                                        \
     } while (0)
-    if (vec) {
+    if (f64) {                                                // one GPU: no multi-source gather
+        if (vec) { if (acc) DISPATCH_G(double2, true, false); else DISPATCH_G(double2, false, false); }
+        else     { if (acc) DISPATCH_G(double, true, false); else DISPATCH_G(double, false, false); }
+    } else if (vec) {
         if (multi) { if (acc) DISPATCH_G(float4, true, true); else DISPATCH_G(float4, false, true); }
         else       { if (acc) DISPATCH_G(float4, true, false); else DISPATCH_G(float4, false, false); }
     } else {
@@ -2661,6 +3174,7 @@ int arrow_gather_rows(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int fla
     if (!D || !S) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (dst=%d src=%d)", dst_buf, src_buf);
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
     if (D->k != S->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch %d vs %d", D->k, S->k);
+    if (D->dtype != S->dtype) return fail(ctx, ARROW_ERR_ARG, "dtype mismatch: destination %s, source %s", dtype_name(D->dtype), dtype_name(S->dtype));
     if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "gather source and destination must not alias");
     if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
     if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
@@ -2676,6 +3190,7 @@ int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, co
     if (!D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", dst_buf);
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
     if (!src_bufs || !row_bounds || n_src < 1 || n_src > MAX_SRC) return fail(ctx, ARROW_ERR_ARG, "need 1..%d sources", MAX_SRC);
+    if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the multi-source gather is float32 only");
     if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
     MultiSrc ms;
     memset(&ms, 0, sizeof ms);
@@ -2684,6 +3199,7 @@ int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, co
         DenseBuf *S = get_dense(ctx, src_bufs[s]);
         if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad source handle %d", src_bufs[s]);
         if (S->k != D->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in source %d", s);
+        if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the multi-source gather is float32 only");
         if (row_bounds[s + 1] < row_bounds[s] || row_bounds[s + 1] - row_bounds[s] > S->rows)
             return fail(ctx, ARROW_ERR_ARG, "source %d owns %lld rows but its tile has %lld", s, (long long)(row_bounds[s + 1] - row_bounds[s]), (long long)S->rows);
         if (S->p == D->p) return fail(ctx, ARROW_ERR_ARG, "gather source and destination must not alias");
@@ -2702,6 +3218,7 @@ int arrow_push_rows(arrow_ctx *ctx, const int *dst_bufs, const int64_t *item_bou
     IdxMap *m = get_map(ctx, map);
     if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", src_buf);
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
+    if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_push_rows is float32 only");
     if (!dst_bufs || !item_bounds || n_dst < 1 || n_dst > MAX_SRC) return fail(ctx, ARROW_ERR_ARG, "need 1..%d destinations", MAX_SRC);
     if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
     if (item_bounds[0] != 0 || item_bounds[n_dst] != m->n) return fail(ctx, ARROW_ERR_ARG, "item bounds must span [0, %lld]", (long long)m->n);
@@ -2716,6 +3233,7 @@ int arrow_push_rows(arrow_ctx *ctx, const int *dst_bufs, const int64_t *item_bou
         DenseBuf *D = get_dense(ctx, dst_bufs[d]);
         if (!D) return fail(ctx, ARROW_ERR_HANDLE, "bad destination handle %d", dst_bufs[d]);
         if (D->k != S->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in destination %d", d);
+        if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_push_rows is float32 only");
         if (cnt > D->rows) return fail(ctx, ARROW_ERR_ARG, "destination %d receives %lld rows but its region has %lld", d, (long long)cnt, (long long)D->rows);
         if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "push source and destination must not alias");
         md.p[d] = D->p;
@@ -2762,6 +3280,7 @@ int arrow_reduce_rows(arrow_ctx *ctx, int dst_buf, int out_table, const int *src
     if (!src_bufs || n_src < 1 || n_src > MAX_SRC || rows < 0) return fail(ctx, ARROW_ERR_ARG, "need 1..%d sources", MAX_SRC);
     DenseBuf *D = dst_buf >= 0 ? get_dense(ctx, dst_buf) : nullptr;
     if (dst_buf >= 0 && !D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", dst_buf);
+    if (D && D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_reduce_rows is float32 only");
     PtrTable *OT = nullptr;
     if (out_table >= 0) {
         if (out_table >= (int)ctx->ptrtabs.size() || !ctx->ptrtabs[out_table].live)
@@ -2780,6 +3299,7 @@ int arrow_reduce_rows(arrow_ctx *ctx, int dst_buf, int out_table, const int *src
         if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad source handle %d", src_bufs[s2]);
         if (s2 == 0) k = S->k;
         if (S->k != k || (D && D->k != k) || (OT && OT->k != k)) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in source %d", s2);
+        if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_reduce_rows is float32 only");
         if (S->rows < rows) return fail(ctx, ARROW_ERR_ARG, "source %d has %lld rows, %lld are reduced", s2, (long long)S->rows, (long long)rows);
         ms.p[s2] = S->p;
     }
@@ -2891,7 +3411,7 @@ static int lane_stream(arrow_ctx *ctx, int lane, cudaStream_t *out) {
     return ARROW_OK;
 }
 
-int arrow_dense_h2d_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_t rows, const float *host) {
+int arrow_dense_h2d_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_t rows, const void *host) {
     CHECK_CTX(ctx);
     DenseBuf *d = get_dense(ctx, buf);
     if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", buf);
@@ -2899,11 +3419,11 @@ int arrow_dense_h2d_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_
     cudaStream_t st;
     int rc = lane_stream(ctx, lane, &st);
     if (rc != ARROW_OK) return rc;
-    if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(d->p + (size_t)row0 * d->k, host, (size_t)rows * d->k * 4, cudaMemcpyHostToDevice, st));
+    if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(d, row0), host, (size_t)rows * d->k * dtype_size(d->dtype), cudaMemcpyHostToDevice, st));
     return ARROW_OK;
 }
 
-int arrow_dense_d2h_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_t rows, float *host) {
+int arrow_dense_d2h_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_t rows, void *host) {
     CHECK_CTX(ctx);
     DenseBuf *d = get_dense(ctx, buf);
     if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", buf);
@@ -2911,7 +3431,7 @@ int arrow_dense_d2h_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_
     cudaStream_t st;
     int rc = lane_stream(ctx, lane, &st);
     if (rc != ARROW_OK) return rc;
-    if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(host, d->p + (size_t)row0 * d->k, (size_t)rows * d->k * 4, cudaMemcpyDeviceToHost, st));
+    if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(host, dense_row(d, row0), (size_t)rows * d->k * dtype_size(d->dtype), cudaMemcpyDeviceToHost, st));
     return ARROW_OK;
 }
 

@@ -76,13 +76,14 @@ def prepare_permutations(perms: Sequence[np.ndarray], n_blocks: Sequence[int], w
 
 
 def arrow_rows(level: Level, width: int, n_blocks: int, block_diagonal: bool, row_begin: int, row_end: int,
-               chunk_rows: int = 1 << 21):
+               chunk_rows: int = 1 << 21, dtype=np.float32):
     """CSR arrays of rows ``[row_begin, row_end)`` of a level, restricted to what the reference multiplies.
 
     The reference only ever materialises blocks (0,j), (i,0), (i,i) and, in banded mode, (i,i+-1)
     (``graphio.py:382-383``), truncated to ``n_blocks`` block-rows/columns (``arrow_dec_mpi.py:728-731``);
     rows at or beyond the end of the file are empty (the ``indptr`` edge padding of ``graphio.py:394-399``).
-    Returns ``(indptr[int64, rebased], indices, data|None, dropped_nnz)``.
+    Returns ``(indptr[int64, rebased], indices, data|None, dropped_nnz)``; ``data`` has element type ``dtype`` (float32
+    values become float64 exactly when ``dtype`` is float64).
     """
     data, indices, indptr = level_triplet(level)
     n = n_blocks * width
@@ -131,10 +132,10 @@ def arrow_rows(level: Level, width: int, n_blocks: int, block_diagonal: bool, ro
     if data is None:
         dat = None
     elif not dat_parts:
-        dat = np.zeros(0, dtype=np.float32)
+        dat = np.zeros(0, dtype=dtype)
     else:
         dat = np.concatenate(dat_parts) if len(dat_parts) != 1 else dat_parts[0]
-        dat = np.ascontiguousarray(dat, dtype=np.float32)
+        dat = np.ascontiguousarray(dat, dtype=dtype)
     return out_ptr, np.ascontiguousarray(idx), dat, dropped
 
 

@@ -17,6 +17,9 @@ Two execution modes, same results:
   (``C_0[map_j[r]] += ...``); no gather kernel runs and levels > 0 never materialise their tiles.
   Chosen automatically when no non-zero of a level reads a row behind the sentinel (then both
   modes are mathematically identical); otherwise the engine stays in ``exchange`` mode.
+
+The precision (``dtype``, float32 or float64) is fixed at construction: the CSR values, every tile and the arithmetic
+of every launch share it.
 """
 from __future__ import annotations
 
@@ -47,9 +50,10 @@ class ArrowEngine:
     def __init__(self, decomposition: Sequence[Tuple[decomp.Level, np.ndarray]], width: int, k: int,
                  block_diagonal: bool = True, device: int = 0, mode: str = "auto", stream: Optional[int] = None,
                  variant: int = _lib.VARIANT_AUTO, n_blocks: Optional[Sequence[int]] = None,
-                 ctx: Optional[_lib.Context] = None, fused_style: str = "gather"):
+                 ctx: Optional[_lib.Context] = None, fused_style: str = "gather", dtype=np.float32):
         if mode not in ("auto", "fused", "exchange"):
             raise ValueError(f"mode must be auto|fused|exchange, got {mode!r}")
+        self.dtype = _lib.element_type(dtype)
         self.ctx = ctx if ctx is not None else _lib.Context(device, stream)
         self.width, self.k, self.variant = int(width), int(k), variant
         if fused_style not in ("gather", "scatter"):
@@ -70,10 +74,10 @@ class ArrowEngine:
             st = _LevelState()
             st.n_blocks = self.n_blocks[j]
             st.rows = st.n_blocks * width
-            ip, idx, dat, dropped = decomp.arrow_rows(B, width, st.n_blocks, block_diagonal, 0, st.rows)
+            ip, idx, dat, dropped = decomp.arrow_rows(B, width, st.n_blocks, block_diagonal, 0, st.rows, dtype=self.dtype)
             st.dropped = dropped
             st.nnz = int(ip[-1])
-            st.csr = self.ctx.csr_upload(st.rows, st.rows, ip, idx, dat)
+            st.csr = self.ctx.csr_upload(st.rows, st.rows, ip, idx, dat, dtype=self.dtype)
             if j > 0:
                 tp = self.to_prev[j][: st.rows]
                 prev_rows = self.levels[j - 1].rows
@@ -106,12 +110,12 @@ class ArrowEngine:
     def _alloc_buffers(self):
         for j, st in enumerate(self.levels):
             if j == 0 or self.mode == "exchange":
-                st.bufs = [self.ctx.dense_alloc(st.rows, self.k), self.ctx.dense_alloc(st.rows, self.k)]
+                st.bufs = [self.ctx.dense_alloc(st.rows, self.k, self.dtype), self.ctx.dense_alloc(st.rows, self.k, self.dtype)]
                 st.xi, st.ci = 0, 0             # zero_rhs: X and C both zero (arrow_slim_mpi.py:354-394)
             if j > 0 and self.mode == "fused":
                 st.csr_fused = st.csr.remap_columns(st.cmap_dev, self.levels[0].rows)
                 if self.fused_style == "gather":
-                    st.cbuf = self.ctx.dense_alloc(st.rows, self.k)     # this level's result tile, written once per step
+                    st.cbuf = self.ctx.dense_alloc(st.rows, self.k, self.dtype)     # this level's result tile, written once per step
 
     def set_mode(self, mode: str):
         """Switch between 'fused' and 'exchange' (re-allocates level tiles; features are reset)."""
@@ -289,15 +293,18 @@ class ArrowEngine:
         """Enqueue one full iteration on host data: upload ``X_host`` -> ``step()`` -> download level-0 result
         into ``out_host``.  Returns immediately; uploads, compute and downloads of consecutive calls overlap
         (side copy streams ordered with events, two device slots).  Both arrays must be pinned
-        (``_lib.PinnedArray``) and must stay untouched until ``stream_drain()``; use at least two
+        (``_lib.PinnedArray``) of the engine's dtype and must stay untouched until ``stream_drain()``; use at least two
         (X, out) pairs in rotation.  Results are identical to ``set_features(X); step(); result()``."""
         st = self.levels[0]
         if X_host.shape != (st.rows, self.k) or out_host.shape != (st.rows, self.k):
             raise ValueError(f"expected host arrays of shape {(st.rows, self.k)}")
+        if X_host.dtype != self.dtype or out_host.dtype != self.dtype:
+            raise ValueError(f"expected {self.dtype} host arrays, got {X_host.dtype} / {out_host.dtype}")
         ctx = self.ctx
         if not hasattr(self, "_slots"):
             # slot 0 re-uses the engine's own level-0 tiles, slot 1 gets two more
-            self._slots = [list(st.bufs), [ctx.dense_alloc(st.rows, self.k), ctx.dense_alloc(st.rows, self.k)]]
+            self._slots = [list(st.bufs), [ctx.dense_alloc(st.rows, self.k, self.dtype),
+                                           ctx.dense_alloc(st.rows, self.k, self.dtype)]]
             self._slot_i = 0
         s = self._slot_i % 2
         slot = self._slots[s]
@@ -327,15 +334,16 @@ class ArrowEngine:
         return 2.0 * self.total_nnz * self.k
 
     def algorithmic_bytes_per_step(self) -> float:
-        """Per level nnz*8 + (R+1)*4 + U*k*4 + R*k*4 (U = R = active rows), plus the exchanges
-        (forward 2 passes, backward 3 passes over the routed rows) -- the figure a fused
-        implementation still reports against."""
+        """Per level nnz*(4+e) + (R+1)*4 + U*k*e + R*k*e (U = R = active rows, e = 4 or 8 bytes per element), plus the
+        exchanges (forward 2 passes, backward 3 passes over the routed rows) -- the figure a fused implementation still
+        reports against."""
+        e = self.dtype.itemsize
         total = 0.0
         for j, st in enumerate(self.levels):
-            total += st.nnz * 8 + (st.rows + 1) * 4 + 2.0 * st.rows * self.k * 4
+            total += st.nnz * (4 + e) + (st.rows + 1) * 4 + 2.0 * st.rows * self.k * e
             if j > 0:
                 m = int(np.count_nonzero(st.to_prev < self.levels[j - 1].rows))
-                total += 5.0 * m * self.k * 4
+                total += 5.0 * m * self.k * e
         return total
 
     def _launch_level_as_in_step(self, j: int, src, dst):
@@ -353,7 +361,7 @@ class ArrowEngine:
         if j > 0 and self.mode == "fused":
             raise ValueError("levels > 0 are timed through step() in fused mode")
         src = st.bufs[st.xi]
-        scratch = self.ctx.dense_alloc(st.rows, self.k)
+        scratch = self.ctx.dense_alloc(st.rows, self.k, self.dtype)
         for _ in range(warmup):
             self._launch_level_as_in_step(j, src, scratch)
         self.ctx.timer_start(5)
@@ -365,14 +373,15 @@ class ArrowEngine:
         return ms
 
     def level_bytes(self, j: int) -> float:
-        """algorithmic bytes of level ``j``'s launch: nnz*8 + (R+1)*4 + R*k*4 (X) + R*k*4 (C), plus -- when the launch
-        carries the epilogue gather-add -- one read of the routed rows of the deeper level's tile (the other two passes
-        of the reference's backward exchange do not exist in this launch)"""
+        """algorithmic bytes of level ``j``'s launch: nnz*(4+e) + (R+1)*4 + R*k*e (X) + R*k*e (C) with e = 4 or 8 bytes
+        per element, plus -- when the launch carries the epilogue gather-add -- one read of the routed rows of the deeper
+        level's tile (the other two passes of the reference's backward exchange do not exist in this launch)"""
+        e = self.dtype.itemsize
         st = self.levels[j]
-        b = st.nnz * 8 + (st.rows + 1) * 4 + 2.0 * st.rows * self.k * 4
+        b = st.nnz * (4 + e) + (st.rows + 1) * 4 + 2.0 * st.rows * self.k * e
         if self.mode == "fused" and self.fused_style == "gather" and j + 1 < self.L:
             nxt = self.levels[j + 1]
-            b += float(np.count_nonzero(nxt.to_prev < st.rows)) * self.k * 4
+            b += float(np.count_nonzero(nxt.to_prev < st.rows)) * self.k * e
         return b
 
     def close(self):

@@ -14,7 +14,10 @@
  * arrow_last_error), no exceptions cross the boundary.  The caller owns host memory; the library
  * owns device memory (handles are small non-negative ints, valid for one context).  All work is
  * stream-ordered on the context's stream; arrow_sync() waits for it.  One host thread per context.
- * Dense tiles are row-major fp32 [rows x k]; CSR is fp32 values with int32 indices on the device.
+ * Dense tiles are row-major [rows x k] of fp32 or fp64; CSR is fp32 or fp64 values with int32 indices on the device.
+ * The precision is fixed when a tile is allocated / a block uploaded (ARROW_F32 / ARROW_F64), and every operand of one
+ * launch has the same precision.  fp64 covers the one-GPU product (arrow_spmm, arrow_spmm_add, arrow_gather_rows); the
+ * multi-GPU entry points (two-part operand, pointer tables, push / reduce, multi-source gather) are fp32 only.
  */
 #ifndef ARROW_B200_H
 #define ARROW_B200_H
@@ -28,7 +31,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 2
+#define ARROW_ABI_VERSION 3
 
 /* error codes */
 #define ARROW_OK              0
@@ -38,6 +41,10 @@ typedef struct arrow_ctx arrow_ctx;
 #define ARROW_ERR_RANGE      -4   /* index / size exceeds the int32 device layout */
 #define ARROW_ERR_NOMEM      -5
 #define ARROW_ERR_UNSUPPORTED -6
+
+/* element types of dense tiles and CSR values */
+#define ARROW_F32             0
+#define ARROW_F64             1
 
 /* flags for arrow_spmm / arrow_gather_rows */
 #define ARROW_ACCUMULATE      1   /* C += ... instead of C = ...  (reference: `C_i += A_i0 @ X_0`,
@@ -99,11 +106,16 @@ int  arrow_csr_upload(arrow_ctx *ctx, int64_t n_rows, int64_t n_cols, int64_t nn
                       const void *indptr, int indptr_bytes,
                       const void *indices, int indices_bytes,
                       const float *data, int *csr_out);
+/* The same with float64 values: the block's launches compute in float64 on float64 tiles. */
+int  arrow_csr_upload_f64(arrow_ctx *ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,
+                          const void *indptr, int indptr_bytes,
+                          const void *indices, int indices_bytes,
+                          const double *data, int *csr_out);
 /* Refused (ARROW_ERR_ARG) while remapped copies made by arrow_csr_remap_columns still share the block's arrays. */
 int  arrow_csr_free(arrow_ctx *ctx, int csr);
 int  arrow_csr_info(arrow_ctx *ctx, int csr, int64_t *n_rows, int64_t *n_cols, int64_t *nnz,
                     int64_t *max_row_nnz, int64_t *n_long_rows);
-/* New CSR sharing indptr/values with `csr`, columns sent through `map` (col' = map[col]; entries
+/* New CSR sharing indptr/values (whatever their precision) with `csr`, columns sent through `map` (col' = map[col]; entries
  * whose image is invalid are skipped by the kernels).  This folds the forward permutation gather
  * (arrow_dec_mpi.py:526, 544) into the SpMM's X read.  `map`'s limit must not exceed new_n_cols; the copy must be
  * freed before its source. */
@@ -121,14 +133,18 @@ int  arrow_map_invert(arrow_ctx *ctx, int map, int64_t n_out, int *map_out);
 int  arrow_map_d2h(arrow_ctx *ctx, int map, int32_t *host, int64_t n);
 
 /* ---- dense tiles (X_i / C_i / X_0 / C_0 of arrow_slim_mpi.py:354-394, concatenated) ----------- */
-int  arrow_dense_alloc(arrow_ctx *ctx, int64_t rows, int k, int *buf_out);      /* zero filled */
+int  arrow_dense_alloc(arrow_ctx *ctx, int64_t rows, int k, int *buf_out);      /* fp32, zero filled */
+int  arrow_dense_alloc_dtype(arrow_ctx *ctx, int64_t rows, int k, int dtype, int *buf_out);   /* ARROW_F32 / ARROW_F64 */
+int  arrow_dense_dtype(arrow_ctx *ctx, int buf, int *dtype);
 int  arrow_dense_free(arrow_ctx *ctx, int buf);
-int  arrow_dense_fill(arrow_ctx *ctx, int buf, float value);
-int  arrow_dense_h2d(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, const float *host);
-int  arrow_dense_d2h(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, float *host);
+int  arrow_dense_fill(arrow_ctx *ctx, int buf, float value);                    /* converted to the tile's type */
+/* host rows are of the tile's element type (float or double) */
+int  arrow_dense_h2d(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, const void *host);
+int  arrow_dense_d2h(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, void *host);
+/* both tiles have the same element type, else ARROW_ERR_ARG */
 int  arrow_dense_copy(arrow_ctx *ctx, int dst, int64_t dst_row0, int src, int64_t src_row0, int64_t rows);
 int  arrow_dense_ptr(arrow_ctx *ctx, int buf, void **device_ptr, int64_t *rows, int *k);
-/* Wrap device memory owned by someone else (a torch tensor, an IPC-imported peer tile).  The pointer must be 16-byte
+/* Wrap fp32 device memory owned by someone else (a torch tensor, an IPC-imported peer tile).  The pointer must be 16-byte
  * aligned when k % 4 == 0 (float4 rows), else 4-byte aligned: ARROW_ERR_ARG otherwise. */
 int  arrow_dense_wrap(arrow_ctx *ctx, void *device_ptr, int64_t rows, int k, int *buf_out);
 /* Copy lanes: host<->device staging on side streams so that step i's download, step i+1's upload and the
@@ -140,8 +156,8 @@ int  arrow_dense_wrap(arrow_ctx *ctx, void *device_ptr, int64_t rows, int k, int
 #define ARROW_LANE_D2H  2
 #define ARROW_LANE_SIDE 3   /* compute-side lane: exchange kernels overlapping the main lane's SpMM */
 #define ARROW_N_LANES   4
-int  arrow_dense_h2d_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_t rows, const float *host);
-int  arrow_dense_d2h_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_t rows, float *host);
+int  arrow_dense_h2d_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_t rows, const void *host);
+int  arrow_dense_d2h_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_t rows, void *host);
 int  arrow_lane_wait(arrow_ctx *ctx, int waiting_lane, int signalling_lane);
 int  arrow_lane_sync(arrow_ctx *ctx, int lane);
 /* Select the lane on which the following arrow_spmm* / arrow_gather_rows[_multi] / arrow_push_rows / arrow_reduce_rows /
@@ -166,7 +182,9 @@ int  arrow_bind_thread_to_device_numa(int device, int *node_out, int *n_cpus_out
 /* C[out(r), :] (+)= sum_p A[r, col_p] * X[col_p, :]   for every row r of `csr`
  *   out(r) = r, or rowmap[r] when rowmap >= 0 (rows with rowmap[r] == -1 are dropped): the backward
  *   scatter-add of arrow_dec_mpi.py:421-437 folded into the SpMM epilogue.
- * X must have >= n_cols rows; C must cover every out(r); X and C must not alias. */
+ * X must have >= n_cols rows; C must cover every out(r); X and C must not alias.
+ * The block, X, C (and the addend of arrow_spmm_add) share one element type, else ARROW_ERR_ARG.  An fp64 launch runs
+ * with ARROW_VARIANT_AUTO or ARROW_VARIANT_TILES only (any other variant: ARROW_ERR_UNSUPPORTED). */
 int  arrow_spmm(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int rowmap, int flags, int variant);
 
 /* C[r, :] = sum_p A[r, col_p] * X[col_p, :] + add[add_map[r], :]   (rows with add_map[r] == -1 get the product only).
@@ -174,7 +192,8 @@ int  arrow_spmm(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int rowmap, int f
  * a gather-add: levels are multiplied deepest first, each writes its tile once, nothing is read-modify-written. */
 int  arrow_spmm_add(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, int add_map, int variant);
 
-/* dst[r, :] (+)= src[map[r], :] for r in [0, map length); rows with map[r] == -1 are left alone
+/* dst[r, :] (+)= src[map[r], :] for r in [0, map length); rows with map[r] == -1 are left alone; dst and src share
+ * one element type (ARROW_ERR_ARG otherwise)
  * (the reference's stale-row behaviour, arrow_dec_mpi.py:544).  Forward exchange with to_prev,
  * backward exchange (as a gather-add) with to_next. */
 int  arrow_gather_rows(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int flags);
@@ -195,7 +214,8 @@ int  arrow_ptrtable_free(arrow_ctx *ctx, int table);
 /* Generalised product.  Columns < x_split read X[col], columns >= x_split read X2[col - x_split] (x2_buf < 0: X only):
  * the feature operand of a level > 0 is [this GPU's level-0 tile | receive region filled by its peers], never
  * materialised as a tile of its own (forward exchange, arrow_dec_mpi.py:507-550, folded into the column indices).
- * out_table >= 0: row r is written to table[r] (c_buf may be -1); else to C[r].  add_buf / add_map as arrow_spmm_add. */
+ * out_table >= 0: row r is written to table[r] (c_buf may be -1); else to C[r].  add_buf / add_map as arrow_spmm_add.
+ * An fp64 launch with x2_buf or out_table returns ARROW_ERR_UNSUPPORTED. */
 int  arrow_spmm_ex(arrow_ctx *ctx, int csr, int x_buf, int x2_buf, int64_t x_split, int c_buf, int out_table,
                    int add_buf, int add_map, int variant);
 /* Push: for item i in [item_bounds[d], item_bounds[d+1]):  dst_bufs[d][i - item_bounds[d]] = src[map[i]].
