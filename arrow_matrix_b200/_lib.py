@@ -20,6 +20,8 @@ ACCUMULATE = 1
 F32, F64 = 0, 1                       # ARROW_F32 / ARROW_F64: element type of dense tiles and CSR values
 _DTYPE_CODE = {np.dtype(np.float32): F32, np.dtype(np.float64): F64}
 VARIANT_AUTO, VARIANT_DIRECT, VARIANT_SHFL, VARIANT_TMA, VARIANT_TILES = -1, 0, 1, 2, 3
+SR_PLUS_TIMES, SR_MIN_PLUS, SR_MAX_PLUS = 0, 1, 2     # ARROW_SR_*: the semiring of arrow_spmm_sr / arrow_gather_rows_sr
+SEMIRINGS = {"plus_times": SR_PLUS_TIMES, "min_plus": SR_MIN_PLUS, "max_plus": SR_MAX_PLUS}
 IPC_HANDLE_BYTES = 80
 
 EXPORTS = [
@@ -38,8 +40,9 @@ EXPORTS = [
     "arrow_graph_begin", "arrow_graph_end", "arrow_graph_launch", "arrow_graph_free",
     "arrow_host_alloc_numa", "arrow_bind_thread_to_device_numa", "arrow_preload_kernels",
     "arrow_csr_upload_f64", "arrow_dense_alloc_dtype", "arrow_dense_dtype",
+    "arrow_spmm_sr", "arrow_gather_rows_sr", "arrow_dense_count_diff",
 ]
-ABI_VERSION = 3          # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 4          # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -134,6 +137,9 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_csr_upload_f64": (c_int, [P, I64, I64, I64, P, I, P, I, P, pI]),
         "arrow_dense_alloc_dtype": (c_int, [P, I64, I, I, pI]),
         "arrow_dense_dtype": (c_int, [P, I, pI]),
+        "arrow_spmm_sr": (c_int, [P, I, I, I, I, I, I]),
+        "arrow_gather_rows_sr": (c_int, [P, I, I, I, I]),
+        "arrow_dense_count_diff": (c_int, [P, I, I, pI64]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -322,6 +328,12 @@ class Context:
         """C[r] = (A X)[r] + add[add_map[r]] (where add_map[r] >= 0)"""
         self._check(self.lib.arrow_spmm_add(self._h, A.h, X.h, C.h, add.h, add_map.h, int(variant)))
 
+    def spmm_sr(self, A: "Csr", X: "Dense", C: "Dense", add: Optional["Dense"] = None,
+                add_map: Optional["RowMap"] = None, semiring: int = SR_PLUS_TIMES):
+        """C[r] = (⊕_p A[r,p] ⊗ X[col_p]) ⊕ add[add_map[r]] in the semiring ``SR_*`` (``arrow_spmm_sr``)"""
+        self._check(self.lib.arrow_spmm_sr(self._h, A.h, X.h, C.h, add.h if add is not None else -1,
+                                           add_map.h if add_map is not None else -1, int(semiring)))
+
     def spmm_ex(self, A: "Csr", X: "Dense", C: Optional["Dense"] = None, X2: Optional["Dense"] = None, x_split: int = 0,
                 out_table: Optional["PtrTable"] = None, add: Optional["Dense"] = None, add_map: Optional["RowMap"] = None,
                 variant: int = VARIANT_AUTO):
@@ -371,6 +383,16 @@ class Context:
 
     def gather_rows(self, dst: "Dense", src: "Dense", m: "RowMap", accumulate: bool = False):
         self._check(self.lib.arrow_gather_rows(self._h, dst.h, src.h, m.h, ACCUMULATE if accumulate else 0))
+
+    def gather_rows_sr(self, dst: "Dense", src: "Dense", m: "RowMap", semiring: int = SR_PLUS_TIMES):
+        """dst[r] = dst[r] ⊕ src[m[r]] where m[r] >= 0 (``arrow_gather_rows_sr``)"""
+        self._check(self.lib.arrow_gather_rows_sr(self._h, dst.h, src.h, m.h, int(semiring)))
+
+    def count_diff(self, a: "Dense", b: "Dense") -> int:
+        """rows in which two equally shaped tiles differ in some element (-0 == +0, NaN != NaN); synchronises"""
+        n = c_int64()
+        self._check(self.lib.arrow_dense_count_diff(self._h, a.h, b.h, byref(n)))
+        return int(n.value)
 
     def gather_rows_multi(self, dst: "Dense", srcs: Sequence["Dense"], row_bounds: Sequence[int], m: "RowMap",
                           accumulate: bool = False):

@@ -22,7 +22,7 @@ import numpy as np
 from . import decomp, graphio, wb_logging
 from .arrow_mpi import ArrowMPI
 from .arrow_slim_mpi import ArrowSlimMPI, _require_gpu
-from .engine import ArrowEngine
+from .engine import ArrowEngine, semiring_code
 
 
 class DecompositionBlocks:
@@ -44,7 +44,8 @@ class ArrowDecompositionMPI:
 
     def __init__(self, comm, B: ArrowSlimMPI, matrix_index: int, number_of_rows_per_rank: int,
                  number_of_feature_columns: int, groups, to_previous_permutation, to_next_mapping,
-                 device='gpu', slim=True, block_diagonal=True, n_blocks=None, mode="auto", exchange="p2p", overlap=1):
+                 device='gpu', slim=True, block_diagonal=True, n_blocks=None, mode="auto", exchange="p2p", overlap=1,
+                 semiring: str = "plus_times", add_identity: bool = False):
         _require_gpu(device)
         self.comm = comm
         self.B = B
@@ -61,6 +62,8 @@ class ArrowDecompositionMPI:
         self._mode = mode
         self._exchange = exchange
         self._overlap = overlap
+        self._semiring = semiring
+        self._add_identity = bool(add_identity)
         self._engine = None
         self.levels: List[ArrowSlimMPI] = [B]
         B._owner = self
@@ -69,9 +72,12 @@ class ArrowDecompositionMPI:
     @staticmethod
     def initialize(comm, n_blocks: np.ndarray, to_prev_permutation, to_next_permutation, rows_per_rank: int,
                    feature_columns: int, device='gpu', block_diagonal: bool = True, slim: bool = False, mode: str = "auto",
-                   exchange: str = "p2p", overlap: int = 1):
+                   exchange: str = "p2p", overlap: int = 1, semiring: str = "plus_times", add_identity: bool = False):
         """Same arguments as the reference (``:106-115``).  ``slim`` only selects the reference's rank
-        layout; on a GPU both layouts are the same row-partitioned kernels, so it is accepted and ignored."""
+        layout; on a GPU both layouts are the same row-partitioned kernels, so it is accepted and ignored.
+        Extensions (one GPU): ``semiring`` -- ``"plus_times"`` (the reference's product), ``"min_plus"`` or
+        ``"max_plus"`` (float32) -- and ``add_identity``, which makes a step compute ``X ⊕ (A ⊗ X)`` (see
+        ``engine.py``)."""
         assert not slim or block_diagonal
         assert np.sum(n_blocks) > 0
         def level_operator(owner, j):           # the reference hands out ArrowSlimMPI or ArrowMPI (``:166-197``)
@@ -79,7 +85,8 @@ class ArrowDecompositionMPI:
         B = level_operator(None, 0)
         arrow = ArrowDecompositionMPI(comm, B, 0, rows_per_rank, feature_columns, None, to_prev_permutation,
                                       to_next_permutation, device=device, slim=slim, block_diagonal=block_diagonal,
-                                      n_blocks=[int(b) for b in n_blocks], mode=mode, exchange=exchange, overlap=overlap)
+                                      n_blocks=[int(b) for b in n_blocks], mode=mode, exchange=exchange, overlap=overlap,
+                                      semiring=semiring, add_identity=add_identity)
         arrow.levels = [B] + [level_operator(arrow, j) for j in range(1, len(n_blocks))]
         return arrow
 
@@ -92,6 +99,11 @@ class ArrowDecompositionMPI:
         if self.comm.Get_size() > 1 and dtype != np.float32:
             raise ValueError(f"a {dtype} decomposition runs on one GPU only: the multi-GPU engine computes in float32; "
                              "load it with datatype=np.float32 or run a single process")
+        fused_style = getattr(self, "_fused_style", "gather")
+        semiring_code(self._semiring, dtype, fused_style)
+        if self.comm.Get_size() > 1 and (self._semiring != "plus_times" or self._add_identity):
+            raise ValueError(f"semiring={self._semiring!r} / add_identity={self._add_identity} run on one GPU only: the "
+                             "multi-GPU engine computes (+, x) without the identity; run a single process")
         if self._engine is not None:
             self._engine.close()
         if self.comm.Get_size() > 1:
@@ -110,7 +122,8 @@ class ArrowDecompositionMPI:
         else:
             self._engine = ArrowEngine(blocks.decomposition, blocks.width, self._n_feature_columns,
                                        block_diagonal=blocks.block_diagonal, mode=self._mode, n_blocks=self.n_blocks,
-                                       fused_style=getattr(self, "_fused_style", "gather"), dtype=dtype)
+                                       fused_style=fused_style, dtype=dtype, semiring=self._semiring,
+                                       add_identity=self._add_identity)
         self.decomposition_length = self._engine.L
 
     def load_data_from_blocks(self, blocked: DecompositionBlocks):

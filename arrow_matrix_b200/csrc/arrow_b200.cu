@@ -2164,6 +2164,473 @@ int spmm_f64(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool rowmap, bool 
     return ARROW_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// tropical semirings (one GPU, fp32): C[r] = (⊕_p A[r,p] ⊗ X[col_p]) ⊕ add[add_map[r]] with ⊗ = the fp32 add (one
+// rounding per term) and ⊕ = min / max.  ⊕ is exact and does not depend on the order of the terms, so every kernel below
+// gives the same bits on every grid, tile size and lane split.  A semiring is a type with zero() (the ⊕ identity), plus()
+// and times(); (+, x) keeps the kernels above.
+// ------------------------------------------------------------------------------------------------
+struct SrMinPlus {
+    __device__ __forceinline__ static float zero() { return __int_as_float(0x7f800000); }       // +inf
+    __device__ __forceinline__ static float plus(float a, float b) { return fminf(a, b); }
+    __device__ __forceinline__ static float times(float a, float x) { return __fadd_rn(a, x); }
+};
+struct SrMaxPlus {
+    __device__ __forceinline__ static float zero() { return __int_as_float(0xff800000); }       // -inf
+    __device__ __forceinline__ static float plus(float a, float b) { return fmaxf(a, b); }
+    __device__ __forceinline__ static float times(float a, float x) { return __fadd_rn(a, x); }
+};
+
+template <class SR>
+__device__ __forceinline__ float4 sr4_zero() {
+    const float z = SR::zero();
+    return make_float4(z, z, z, z);
+}
+template <class SR>
+__device__ __forceinline__ void sr_plus(float4 &acc, const float4 &x) {
+    acc.x = SR::plus(acc.x, x.x);
+    acc.y = SR::plus(acc.y, x.y);
+    acc.z = SR::plus(acc.z, x.z);
+    acc.w = SR::plus(acc.w, x.w);
+}
+template <class SR>
+__device__ __forceinline__ void sr_plus(float &acc, const float &x) {
+    acc = SR::plus(acc, x);
+}
+// acc = acc ⊕ (a ⊗ x): FADD + FMNMX per element
+template <class SR>
+__device__ __forceinline__ void sr4_mac(float4 &acc, float a, const float4 &x) {
+    acc.x = SR::plus(acc.x, SR::times(a, x.x));
+    acc.y = SR::plus(acc.y, SR::times(a, x.y));
+    acc.z = SR::plus(acc.z, SR::times(a, x.z));
+    acc.w = SR::plus(acc.w, SR::times(a, x.w));
+}
+
+// The k_spmm_tiles_v1 pipeline (CSR slices by cp.async.bulk on an mbarrier, two stages, persistent CTAs on the atomic
+// ticket, a lane group per row, float4 gathers under the L2 policies) with the semiring's inner step and one epilogue:
+// C[r] = the product, ⊕ the addend row when add_map[r] >= 0.
+template <int G, int VPL, class SR, int TR, int TN>
+__global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles_sr(TileArgs t) {
+    constexpr int TILE_PTR_WORDS = TileCfg<TR, TN>::PTR_WORDS;
+    constexpr int TILE_NNZ_WORDS = TileCfg<TR, TN>::NNZ_WORDS;
+    constexpr int TILE_STAGE_WORDS = TileCfg<TR, TN>::STAGE_WORDS;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    int *stage_base = reinterpret_cast<int *>(smem_raw);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)2 * TILE_STAGE_WORDS * 4);
+    const SpmmArgs &a = t.a;
+    constexpr int RPW = 32 / G;
+    constexpr int UNROLL = (VPL >= 4) ? 2 : (VPL == 2 ? 4 : 8);
+    constexpr int TAIL = (UNROLL >= 4) ? UNROLL / 2 : UNROLL;     // predicated tail batches
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const bool EXACT = (t.a.k4 == G * VPL);                       // every lane owns valid columns
+    const int gl = lane % G;
+    const int gi = lane / G;
+    const int k4 = a.k4;
+    const float4 *__restrict__ Xl = reinterpret_cast<const float4 *>(a.X) + gl;
+    float4 *__restrict__ Cl = reinterpret_cast<float4 *>(a.C) + gl;
+    const uint64_t pol_keep = (t.l2_hints & 1) ? l2_policy_evict_last() : l2_policy_evict_normal();
+    const uint64_t pol_stream = (t.l2_hints & 2) ? l2_policy_evict_first() : l2_policy_evict_normal();
+
+    if (threadIdx.x == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    auto issue_csr = [&](int tile, int st) {
+        const int4 d = __ldg(t.tiles + tile);
+        const int rb4 = d.x & ~3;
+        const int a0 = d.z & ~3;
+        const uint32_t ptr_bytes = (uint32_t)(((d.y - rb4 + 1) + 3) & ~3) * 4u;
+        const uint32_t nnz_bytes = (uint32_t)(((d.w - a0) + 3) & ~3) * 4u;
+        int *sp = stage_base + (size_t)st * TILE_STAGE_WORDS;
+        mbar_expect_tx(&bars[st], ptr_bytes + 2u * nnz_bytes);
+        bulk_g2s_hint(sp, a.indptr + rb4, ptr_bytes, &bars[st], pol_stream);
+        if (nnz_bytes) {
+            bulk_g2s_hint(sp + TILE_PTR_WORDS, a.indices + a0, nnz_bytes, &bars[st], pol_stream);
+            bulk_g2s_hint(sp + TILE_PTR_WORDS + TILE_NNZ_WORDS, a.vals + a0, nnz_bytes, &bars[st], pol_stream);
+        }
+    };
+
+    // the n-th tile of a CTA uses stage n & 1 and waits for completion (n >> 1) & 1 of that stage's barrier: one counter
+    // instead of a stage index and a parity word keeps the VPL = 4 instances free of spills
+    __shared__ int s_next[TILE_STAGES];
+    int tile = blockIdx.x;
+    if (tile < t.n_tiles && threadIdx.x == 0) issue_csr(tile, 0);
+    for (unsigned int n = 0; tile < t.n_tiles; ++n) {
+        const int st = (int)(n & 1u);
+        if (threadIdx.x == 0) {
+            const int next = atomicAdd(t.ticket, 1) + (int)gridDim.x;
+            s_next[st] = next;
+            if (next < t.n_tiles) issue_csr(next, st ^ 1);
+        }
+        const int4 d = __ldg(t.tiles + tile);
+        mbar_wait(&bars[st], (n >> 1) & 1u);
+        const int *sp = stage_base + (size_t)st * TILE_STAGE_WORDS;
+        const int *s_ptr = sp + (d.x - (d.x & ~3));
+        const int a0 = d.z & ~3;
+        const int *s_idx = sp + TILE_PTR_WORDS - a0;                    // index with global nnz offsets
+        const float *s_val = reinterpret_cast<const float *>(sp + TILE_PTR_WORDS + TILE_NNZ_WORDS) - a0;
+        const int n_rows_tile = d.y - d.x;
+
+        for (int lr = warp * RPW + gi; lr < n_rows_tile; lr += (TILE_THREADS / 32) * RPW) {
+            const int s = s_ptr[lr];
+            const int e = s_ptr[lr + 1];
+            if (e - s > a.long_threshold) continue;
+            const long long row = (long long)d.x + lr;
+            float4 acc[VPL];
+#pragma unroll
+            for (int i = 0; i < VPL; ++i) acc[i] = sr4_zero<SR>();
+            if (a.add_map != nullptr) {
+                // the addend is requested first so that its latency hides behind the gathers
+                const int am = __ldg(a.add_map + row);
+                if (am >= 0) {
+                    const float4 *ar = reinterpret_cast<const float4 *>(a.add_src) + (long long)am * k4 + gl;
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i)
+                        if (gl + i * G < k4) acc[i] = ld_f4_hint(ar + i * G, pol_stream);
+                }
+            }
+            int p = s;
+            if (EXACT && !t.skip) {
+                // unpredicated batches: full UNROLL batches, then the remainder as 4 / 2 / 1
+                auto batch = [&](auto n_tag) {
+                    constexpr int N = decltype(n_tag)::value;
+                    float4 x[N][VPL];
+#pragma unroll
+                    for (int u = 0; u < N; ++u) {
+                        const float4 *xr = Xl + (long long)s_idx[p + u] * k4;
+#pragma unroll
+                        for (int i = 0; i < VPL; ++i) x[u][i] = ldg_f4_hint(xr + i * G, pol_keep);
+                    }
+#pragma unroll
+                    for (int u = 0; u < N; ++u) {
+                        const float v = s_val[p + u];
+#pragma unroll
+                        for (int i = 0; i < VPL; ++i) sr4_mac<SR>(acc[i], v, x[u][i]);
+                    }
+                    p += N;
+                };
+                while (p + UNROLL <= e) batch(std::integral_constant<int, UNROLL>{});
+                if constexpr (UNROLL >= 8) { if (e - p >= 4) batch(std::integral_constant<int, 4>{}); }
+                if constexpr (UNROLL >= 4) { if (e - p >= 2) batch(std::integral_constant<int, 2>{}); }
+                if (e - p >= 1) batch(std::integral_constant<int, 1>{});
+            }
+            // tail (and the general case): predicated batches of TAIL.  A skipped entry (column -1) or a slot past the
+            // row's end gets the ⊕ identity as its weight and zeros as its X row: ∓inf + 0 = ∓inf leaves acc unchanged
+            // (one select per slot instead of one per element).  Columns past k4 are computed on zeros and never stored.
+            // Here and in the batches the weights are read from shared memory once the gathers are back (fewer live
+            // registers across the gathers).
+            for (; p < e; p += TAIL) {
+                float4 x[TAIL][VPL];
+#pragma unroll
+                for (int u = 0; u < TAIL; ++u) {
+                    const int c = (p + u < e) ? s_idx[p + u] : -1;
+                    const float4 *xr = Xl + (long long)c * k4;              // c = -1: address arithmetic only
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i)
+                        x[u][i] = (c >= 0 && gl + i * G < k4) ? ldg_f4_hint(xr + i * G, pol_keep) : f4_zero();
+                }
+#pragma unroll
+                for (int u = 0; u < TAIL; ++u) {
+                    const int c = (p + u < e) ? s_idx[p + u] : -1;
+                    const float v = (c >= 0) ? s_val[p + u] : SR::zero();
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i) sr4_mac<SR>(acc[i], v, x[u][i]);
+                }
+            }
+            float4 *cr = Cl + row * k4;
+#pragma unroll
+            for (int i = 0; i < VPL; ++i)
+                if (gl + i * G < k4) st_f4_hint(cr + i * G, acc[i], pol_stream);
+        }
+        __syncthreads();            // stage `st` may be refilled by the next iteration's copy
+        tile = s_next[st];
+    }
+}
+
+// k not a multiple of 4 or k > 256: warp per row, lanes over columns, scalar accesses
+template <class SR>
+__global__ void __launch_bounds__(256) k_spmm_generic_sr(SpmmArgs a) {
+    const int lane = threadIdx.x & 31;
+    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
+    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    for (long long row = warp_id; row < a.n_rows; row += warps_total) {
+        const int s = __ldg(a.indptr + row);
+        const int e = __ldg(a.indptr + row + 1);
+        if (e - s > a.long_threshold) continue;
+        float *crow = a.C + row * a.k;
+        const int am = (a.add_map != nullptr) ? __ldg(a.add_map + row) : -1;
+        for (int c0 = 0; c0 < a.k; c0 += 128) {
+            float acc[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
+            for (int p = s; p < e; ++p) {
+                const int c = __ldg(a.indices + p);
+                const float v = __ldg(a.vals + p);
+                if (c < 0) continue;
+                const float *xr = a.X + (long long)c * a.k;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int col = c0 + lane + 32 * i;
+                    if (col < a.k) acc[i] = SR::plus(acc[i], SR::times(v, __ldg(xr + col)));
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int col = c0 + lane + 32 * i;
+                if (col < a.k) {
+                    float r = acc[i];
+                    if (am >= 0) r = SR::plus(r, a.add_src[(long long)am * a.k + col]);
+                    crow[col] = r;
+                }
+            }
+        }
+    }
+}
+
+// long rows: one CTA per segment ⊕-reduces its entries into a scratch slot, then one CTA per row ⊕-reduces the slots and
+// the addend (k_spmm_long_partial / k_spmm_long_reduce)
+template <class SR>
+__global__ void __launch_bounds__(256) k_spmm_long_partial_sr(LongArgs a) {
+    extern __shared__ float red_sr[];   // [warps][k]
+    const LongTask t = a.tasks[blockIdx.x];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    for (int c0 = 0; c0 < a.k; c0 += 128) {
+        float acc[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
+        for (int p = t.begin + warp; p < t.end; p += nwarps) {
+            const int c = __ldg(a.indices + p);
+            const float v = __ldg(a.vals + p);
+            if (c < 0) continue;
+            const float *xr = a.X + (long long)c * a.k;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int col = c0 + lane + 32 * i;
+                if (col < a.k) acc[i] = SR::plus(acc[i], SR::times(v, __ldg(xr + col)));
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int col = c0 + lane + 32 * i;
+            if (col < a.k) red_sr[warp * a.k + col] = acc[i];
+        }
+    }
+    __syncthreads();
+    for (int col = threadIdx.x; col < a.k; col += blockDim.x) {
+        float r = SR::zero();
+        for (int w = 0; w < nwarps; ++w) r = SR::plus(r, red_sr[w * a.k + col]);
+        a.scratch[(long long)t.slot * a.k + col] = r;
+    }
+}
+
+template <class SR>
+__global__ void __launch_bounds__(128) k_spmm_long_reduce_sr(const int *__restrict__ long_rows,
+                                                             const int *__restrict__ long_first,
+                                                             const float *__restrict__ scratch, float *__restrict__ C,
+                                                             int k, const float *__restrict__ add_src,
+                                                             const int *__restrict__ add_map) {
+    const int r = long_rows[blockIdx.x];
+    float *crow = C + (long long)r * k;
+    const int am = (add_map != nullptr) ? add_map[r] : -1;
+    const int s0 = long_first[blockIdx.x], s1 = long_first[blockIdx.x + 1];
+    for (int col = threadIdx.x; col < k; col += blockDim.x) {
+        float acc = SR::zero();
+        for (int s = s0; s < s1; ++s) acc = SR::plus(acc, scratch[(long long)s * k + col]);
+        if (am >= 0) acc = SR::plus(acc, add_src[(long long)am * k + col]);
+        crow[col] = acc;
+    }
+}
+
+// dst[r] = dst[r] ⊕ src[map[r]] (map[r] >= 0): the backward exchange of a semiring step (k_gather_rows without peers)
+template <typename VT, int G, class SR>
+__global__ void __launch_bounds__(256) k_gather_rows_sr(VT *__restrict__ dst, const VT *__restrict__ src,
+                                                        const int *__restrict__ map, long long n_rows, int vec_per_row) {
+    constexpr int RPW = 32 / G;
+    const int lane = threadIdx.x & 31;
+    const int gl = lane % G, gi = lane / G;
+    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
+    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    for (long long r = warp_id * RPW + gi; r < n_rows; r += warps_total * RPW) {
+        const int m = __ldg(map + r);
+        if (m < 0) continue;
+        const VT *sp = src + (long long)m * vec_per_row;
+        VT *dp = dst + r * vec_per_row;
+        for (int v0 = gl; v0 < vec_per_row; v0 += 4 * G) {
+            VT val[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (v0 + j * G < vec_per_row) val[j] = sp[v0 + j * G];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (v0 + j * G < vec_per_row) {
+                    VT old = dp[v0 + j * G];
+                    sr_plus<SR>(old, val[j]);
+                    dp[v0 + j * G] = old;
+                }
+            }
+        }
+    }
+}
+
+// rows (warp per row) in which two equally shaped tiles differ in some element, compared by value (-0 == +0, NaN != NaN)
+template <typename T>
+__global__ void __launch_bounds__(256) k_count_diff(const T *__restrict__ a, const T *__restrict__ b, long long rows,
+                                                    int k, unsigned long long *__restrict__ count) {
+    __shared__ unsigned int s_count;
+    if (threadIdx.x == 0) s_count = 0u;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
+    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    for (long long r = warp_id; r < rows; r += warps_total) {
+        bool diff = false;
+        for (int c = lane; c < k; c += 32) diff |= (a[r * k + c] != b[r * k + c]);
+        if (__any_sync(0xffffffffu, diff) && lane == 0) atomicAdd(&s_count, 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && s_count) atomicAdd(count, (unsigned long long)s_count);
+}
+
+template <int G, int VPL, class SR, int TR, int TN>
+int launch_tiles_sr_one(arrow_ctx *ctx, const TileArgs &t) {
+    constexpr size_t SMEM = TileCfg<TR, TN>::SMEM_BYTES;
+    auto fn = k_spmm_tiles_sr<G, VPL, SR, TR, TN>;
+    static bool attr_set[64] = {};            /* function attributes are per device */
+    static int occ_dev[64] = {};
+    const int dv = ctx->device & 63;
+    if (!attr_set[dv]) {
+        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
+        attr_set[dv] = true;
+    }
+    const int occ = occ_dev[dv];
+    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
+    int sms = ctx->sm_count;
+    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
+    int grid = (int)std::min<long long>((long long)per_sm * sms, t.n_tiles);
+    cudaMemsetAsync(t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
+    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(t);
+    ctx->launches++;
+    return ARROW_OK;
+}
+
+// (lanes per row, float4 per lane) and tile size as launch_tiles picks them for a plain launch with the default options
+int launch_tiles_sr_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A, bool min_plus) {
+    const int k4 = t.a.k4;
+    const int vpl = (k4 >= 32) ? 4 : (k4 >= 8 ? 2 : 1);
+    const int lanes = (k4 + vpl - 1) / vpl;           // <= 16: k4 <= 64
+    int g = 1;
+    while (g < lanes) g <<= 1;
+    const bool big = (k4 <= 8) && ctx->big_tiles && A->n_tiles_big > 0;     // k <= 32
+    if (big) { t.tiles = A->tiles_big; t.n_tiles = A->n_tiles_big; }
+#define TSR(GG, VV, TR, TN)                                                                              \
+    return min_plus ? launch_tiles_sr_one<GG, VV, SrMinPlus, TR, TN>(ctx, t) : launch_tiles_sr_one<GG, VV, SrMaxPlus, TR, TN>(ctx, t)
+#define SRB(GG, VV) if (big && g == GG && vpl == VV) TSR(GG, VV, TILE_ROWS_BIG, TILE_NNZ_BIG)
+#define SRS(GG, VV) if (g == GG && vpl == VV) TSR(GG, VV, TILE_ROWS, TILE_NNZ)
+    SRB(1, 1); SRB(2, 1); SRB(4, 1); SRB(8, 1); SRB(4, 2);
+    SRS(1, 1); SRS(2, 1); SRS(4, 1); SRS(8, 1); SRS(4, 2); SRS(8, 2); SRS(16, 2); SRS(8, 4); SRS(16, 4);
+#undef SRS
+#undef SRB
+#undef TSR
+    return fail(ctx, ARROW_ERR_UNSUPPORTED, "no semiring tile kernel for k4=%d vpl=%d", k4, vpl);
+}
+
+// the product of arrow_spmm_sr for (min, +) / (max, +); `a` carries the validated fp32 operands (identity output rows)
+template <class SR>
+int spmm_sr(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool min_plus) {
+    const int k = a.k;
+    const int lane = ctx->cur_lane;
+    cudaStream_t stream = cur_stream(ctx);
+    if (k % 4 != 0 || k > 256) {
+        const long long ctas = (A->n_rows + 7) / 8;
+        auto fn = k_spmm_generic_sr<SR>;
+        const int grid = grid_for(ctx, (const void *)fn, 256, 0, ctas);
+        fn<<<grid, 256, 0, stream>>>(a);
+        ctx->launches++;
+    } else if (A->n_tiles > 0) {
+        TileArgs t;
+        t.a = a;
+        t.tiles = A->tiles;
+        t.n_tiles = A->n_tiles;
+        t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
+        t.ticket = ctx->tile_ticket + 2 * lane;
+        t.l2_hints = ctx->l2_hints_plain;
+        t.prefetch = 0;
+        const int rc = launch_tiles_sr_shape(ctx, t, A, min_plus);
+        if (rc != ARROW_OK) return rc;
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+
+    if (A->n_long_tasks > 0) {
+        const size_t need = (size_t)A->n_long_tasks * k * 4;
+        if (need > ctx->long_scratch_bytes[lane]) {
+            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
+            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
+            ctx->long_scratch[lane] = nullptr;
+            ctx->long_scratch_bytes[lane] = 0;
+            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
+            ctx->long_scratch_bytes[lane] = need;
+        }
+        LongArgs la;
+        la.tasks = A->long_tasks;
+        la.indices = a.indices;
+        la.vals = a.vals;
+        la.X = a.X;
+        la.scratch = ctx->long_scratch[lane];
+        la.k = k;
+        la.X2 = nullptr;
+        la.x_split = 0;
+        const size_t smem = (size_t)8 * k * 4;
+        if (smem > 48 * 1024)
+            CUDA_TRY(ctx, cudaFuncSetAttribute(k_spmm_long_partial_sr<SR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_spmm_long_partial_sr<SR><<<A->n_long_tasks, 256, smem, stream>>>(la);
+        ctx->launches++;
+        k_spmm_long_reduce_sr<SR><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, la.scratch, a.C, k,
+                                                                       a.add_src, a.add_map);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
+    return ARROW_OK;
+}
+
+template <class SR>
+int gather_rows_sr(arrow_ctx *ctx, DenseBuf *D, const DenseBuf *S, const IdxMap *m) {
+    const long long n_rows = m->n;
+    if (n_rows == 0) return ARROW_OK;
+    const int k = D->k;
+    const bool vec = (k % 4 == 0);
+    const int vpr = vec ? k / 4 : k;
+    int g = 1;
+    while (g < vpr && g < 32) g <<= 1;                       // lanes per row
+    if (g > 8 && vpr <= 32) g = 8;                           // 8 lanes x 4 vectors cover k <= 128 in one pass
+    const int threads = 256;
+    const long long rows_per_cta = (threads / 32) * (32 / g);
+    int grid = (int)std::min<long long>((n_rows + rows_per_cta - 1) / rows_per_cta, (long long)ctx->sm_count * 8);
+    grid = std::max(grid, 1);
+#define LAUNCH_GS(VT, GG)                                                                                        \
+    k_gather_rows_sr<VT, GG, SR><<<grid, threads, 0, cur_stream(ctx)>>>(reinterpret_cast<VT *>(D->p),            \
+                                                                        reinterpret_cast<const VT *>(S->p), m->p, n_rows, vpr)
+#define DISPATCH_GS(VT)                                                                                          \
+    do {                                                                                                         \
+        switch (g) {                                                                                             \
+            case 1: LAUNCH_GS(VT, 1); break;                                                                     \
+            case 2: LAUNCH_GS(VT, 2); break;                                                                     \
+            case 4: LAUNCH_GS(VT, 4); break;                                                                     \
+            case 8: LAUNCH_GS(VT, 8); break;                                                                     \
+            case 16: LAUNCH_GS(VT, 16); break;                                                                   \
+            default: LAUNCH_GS(VT, 32); break;                                                                   \
+        }                                                                                                        \
+    } while (0)
+    if (vec) DISPATCH_GS(float4);
+    else DISPATCH_GS(float);
+#undef DISPATCH_GS
+#undef LAUNCH_GS
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return ARROW_OK;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -3181,6 +3648,108 @@ int arrow_gather_rows(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int fla
     MultiSrc ms;
     memset(&ms, 0, sizeof ms);
     return gather_common(ctx, D, S->p, ms, false, m, (flags & ARROW_ACCUMULATE) != 0);
+}
+
+// ---- semirings ------------------------------------------------------------------------------------
+int arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, int add_map, int semiring) {
+    CHECK_CTX(ctx);
+    if (semiring == ARROW_SR_PLUS_TIMES) {
+        if (add_buf < 0 && add_map < 0) return arrow_spmm(ctx, csr, x_buf, c_buf, -1, 0, ARROW_VARIANT_AUTO);
+        return arrow_spmm_add(ctx, csr, x_buf, c_buf, add_buf, add_map, ARROW_VARIANT_AUTO);
+    }
+    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS)
+        return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
+    CHECK_POISON(ctx);
+    Csr *A = get_csr(ctx, csr);
+    DenseBuf *X = get_dense(ctx, x_buf);
+    DenseBuf *C = get_dense(ctx, c_buf);
+    if (!A) return fail(ctx, ARROW_ERR_HANDLE, "bad csr handle %d", csr);
+    if (!X || !C) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x=%d c=%d)", x_buf, c_buf);
+    if (X->dtype != A->dtype || C->dtype != A->dtype)
+        return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, X is %s, C is %s", dtype_name(A->dtype),
+                    dtype_name(X->dtype), dtype_name(C->dtype));
+    if (X->k != C->k) return fail(ctx, ARROW_ERR_ARG, "X has %d feature columns, C has %d", X->k, C->k);
+    if (X->p == C->p) return fail(ctx, ARROW_ERR_ARG, "X and C must not alias");
+    if (X->rows < A->n_cols) return fail(ctx, ARROW_ERR_ARG, "X has %lld rows, block has %lld columns", (long long)X->rows, (long long)A->n_cols);
+    if (C->rows < A->n_rows) return fail(ctx, ARROW_ERR_ARG, "C has %lld rows, block has %lld rows", (long long)C->rows, (long long)A->n_rows);
+    const int k = X->k;
+    SpmmArgs a;
+    memset(&a, 0, sizeof a);
+    if (add_buf >= 0 || add_map >= 0) {
+        DenseBuf *S = get_dense(ctx, add_buf);
+        IdxMap *am = get_map(ctx, add_map);
+        if (!S || !am) return fail(ctx, ARROW_ERR_HANDLE, "bad addend handles (buf=%d map=%d)", add_buf, add_map);
+        if (S->k != k) return fail(ctx, ARROW_ERR_ARG, "addend has %d feature columns, expected %d", S->k, k);
+        if (S->dtype != A->dtype) return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, the addend is %s", dtype_name(A->dtype), dtype_name(S->dtype));
+        if (am->n < A->n_rows) return fail(ctx, ARROW_ERR_ARG, "addend map has %lld entries, block has %lld rows", (long long)am->n, (long long)A->n_rows);
+        if (am->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "addend map reaches row %lld, addend tile has %lld rows", (long long)am->limit, (long long)S->rows);
+        if (S->p == C->p) return fail(ctx, ARROW_ERR_ARG, "addend and C must not alias");
+        a.add_src = S->p;
+        a.add_map = am->p;
+    }
+    if (A->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the (min, +) / (max, +) semirings are float32 only");
+    if (A->n_rows == 0) return ARROW_OK;
+    a.indptr = A->indptr;
+    a.indices = A->indices;
+    a.vals = A->vals;
+    a.X = X->p;
+    a.C = C->p;
+    a.n_rows = A->n_rows;
+    a.k = k;
+    a.k4 = k / 4;
+    a.long_threshold = A->long_threshold;
+    if (semiring == ARROW_SR_MIN_PLUS) return spmm_sr<SrMinPlus>(ctx, A, a, true);
+    return spmm_sr<SrMaxPlus>(ctx, A, a, false);
+}
+
+int arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int semiring) {
+    CHECK_CTX(ctx);
+    if (semiring == ARROW_SR_PLUS_TIMES) return arrow_gather_rows(ctx, dst_buf, src_buf, map, ARROW_ACCUMULATE);
+    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS)
+        return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
+    CHECK_POISON(ctx);
+    DenseBuf *D = get_dense(ctx, dst_buf), *S = get_dense(ctx, src_buf);
+    IdxMap *m = get_map(ctx, map);
+    if (!D || !S) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (dst=%d src=%d)", dst_buf, src_buf);
+    if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
+    if (D->k != S->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch %d vs %d", D->k, S->k);
+    if (D->dtype != S->dtype) return fail(ctx, ARROW_ERR_ARG, "dtype mismatch: destination %s, source %s", dtype_name(D->dtype), dtype_name(S->dtype));
+    if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "gather source and destination must not alias");
+    if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
+    if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
+    if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the (min, +) / (max, +) semirings are float32 only");
+    if (semiring == ARROW_SR_MIN_PLUS) return gather_rows_sr<SrMinPlus>(ctx, D, S, m);
+    return gather_rows_sr<SrMaxPlus>(ctx, D, S, m);
+}
+
+int arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    DenseBuf *A = get_dense(ctx, a), *B = get_dense(ctx, b);
+    if (!A || !B) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (a=%d b=%d)", a, b);
+    if (!rows_changed) return fail(ctx, ARROW_ERR_ARG, "null rows_changed");
+    if (A->rows != B->rows || A->k != B->k || A->dtype != B->dtype)
+        return fail(ctx, ARROW_ERR_ARG, "tiles differ in shape or type: %lld x %d %s vs %lld x %d %s", (long long)A->rows, A->k,
+                    dtype_name(A->dtype), (long long)B->rows, B->k, dtype_name(B->dtype));
+    *rows_changed = 0;
+    if (A->rows == 0 || A->k == 0) return ARROW_OK;
+    cudaStream_t stream = cur_stream(ctx);
+    DevTmp cnt;
+    CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof(unsigned long long)));
+    CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof(unsigned long long), stream));
+    const int grid = (int)std::min<long long>((A->rows + 7) / 8, (long long)ctx->sm_count * 8);
+    unsigned long long *c = reinterpret_cast<unsigned long long *>(cnt.p);
+    if (A->dtype == ARROW_F64)
+        k_count_diff<double><<<grid, 256, 0, stream>>>(reinterpret_cast<const double *>(A->p), reinterpret_cast<const double *>(B->p), A->rows, A->k, c);
+    else
+        k_count_diff<float><<<grid, 256, 0, stream>>>(A->p, B->p, A->rows, A->k, c);
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    unsigned long long h = 0;
+    CUDA_TRY(ctx, cudaMemcpyAsync(&h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+    *rows_changed = (int64_t)h;
+    return ARROW_OK;
 }
 
 int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, const int64_t *row_bounds, int n_src, int map, int flags) {

@@ -139,6 +139,28 @@ def arrow_rows(level: Level, width: int, n_blocks: int, block_diagonal: bool, ro
     return out_ptr, np.ascontiguousarray(idx), dat, dropped
 
 
+def with_diagonal(indptr: np.ndarray, indices: np.ndarray, data: Optional[np.ndarray], rows: int, value: float,
+                  dtype=np.float32):
+    """CSR arrays (as ``arrow_rows`` returns them) with an entry ``(r, r)`` of ``value`` in front of every row ``r <
+    rows``, next to any entry the row already has there.  ``data`` None means ones.  In a semiring whose ⊗ identity is
+    ``value`` the block then computes ``X ⊕ (A ⊗ X)`` on its rows; the diagonal lies in the blocks (i, i), which every
+    arrow level keeps."""
+    ip = np.asarray(indptr, dtype=np.int64)
+    assert ip.size == rows + 1
+    out_ptr = ip + np.arange(rows + 1, dtype=np.int64)
+    nnz = int(out_ptr[-1])
+    diag = out_ptr[:-1]
+    rest = np.ones(nnz, dtype=bool)
+    rest[diag] = False
+    idx = np.empty(nnz, dtype=np.result_type(np.asarray(indices).dtype, np.int32))
+    idx[diag] = np.arange(rows)
+    idx[rest] = indices
+    dat = np.empty(nnz, dtype=dtype)
+    dat[diag] = value
+    dat[rest] = 1 if data is None else data
+    return out_ptr, idx, dat
+
+
 def block_partition(n_blocks: int, parts: int) -> np.ndarray:
     """Contiguous, as-even-as-possible split of ``n_blocks`` block-rows over ``parts`` GPUs (bounds array).
 

@@ -20,6 +20,12 @@ Two execution modes, same results:
 
 The precision (``dtype``, float32 or float64) is fixed at construction: the CSR values, every tile and the arithmetic
 of every launch share it.
+
+The semiring is fixed at construction too: ``plus_times`` (+, x), or the tropical ``min_plus`` / ``max_plus`` (float32),
+where ⊗ is the float32 add and ⊕ is min / max.  The decomposition carries over unchanged (the operator is the ⊕ of its
+levels in any semiring): the forward exchange only moves rows, the backward aggregation becomes a ⊕, and the stale rows
+behind the sentinel are the same.  ``add_identity`` puts the ⊗ identity on level 0's diagonal, so that a step computes
+``X ⊕ (A ⊗ X)``: the relaxation step of BFS and Bellman-Ford (``(I + A) X`` in ``plus_times``).
 """
 from __future__ import annotations
 
@@ -29,6 +35,26 @@ import numpy as np
 
 from . import _lib
 from . import decomp
+
+
+# the semiring's ⊕ identity (its "zero": what zero_rhs and fresh tiles hold) and ⊗ identity (what add_identity puts on
+# level 0's diagonal)
+_PLUS_ZERO = {_lib.SR_PLUS_TIMES: 0.0, _lib.SR_MIN_PLUS: float("inf"), _lib.SR_MAX_PLUS: float("-inf")}
+_TIMES_ONE = {_lib.SR_PLUS_TIMES: 1.0, _lib.SR_MIN_PLUS: 0.0, _lib.SR_MAX_PLUS: 0.0}
+
+
+def semiring_code(semiring: str, dtype, fused_style: str = "gather") -> int:
+    """``_lib.SR_*`` of a semiring name; raises ``ValueError`` (before any CUDA work) for an unknown name and for the
+    combinations that do not exist: the tropical semirings are float32 and run the gather style of the fused step."""
+    if semiring not in _lib.SEMIRINGS:
+        raise ValueError(f"unknown semiring {semiring!r}: expected one of {', '.join(_lib.SEMIRINGS)}")
+    code = _lib.SEMIRINGS[semiring]
+    if code != _lib.SR_PLUS_TIMES:
+        if np.dtype(dtype) != np.float32:
+            raise ValueError(f"the {semiring} semiring computes in float32, the decomposition is {np.dtype(dtype)}")
+        if fused_style != "gather":
+            raise ValueError(f"the {semiring} semiring runs the gather style of the fused step, not {fused_style!r}")
+    return code
 
 
 class _LevelState:
@@ -50,10 +76,14 @@ class ArrowEngine:
     def __init__(self, decomposition: Sequence[Tuple[decomp.Level, np.ndarray]], width: int, k: int,
                  block_diagonal: bool = True, device: int = 0, mode: str = "auto", stream: Optional[int] = None,
                  variant: int = _lib.VARIANT_AUTO, n_blocks: Optional[Sequence[int]] = None,
-                 ctx: Optional[_lib.Context] = None, fused_style: str = "gather", dtype=np.float32):
+                 ctx: Optional[_lib.Context] = None, fused_style: str = "gather", dtype=np.float32,
+                 semiring: str = "plus_times", add_identity: bool = False):
         if mode not in ("auto", "fused", "exchange"):
             raise ValueError(f"mode must be auto|fused|exchange, got {mode!r}")
         self.dtype = _lib.element_type(dtype)
+        self.sr = semiring_code(semiring, self.dtype, fused_style)
+        self.semiring = semiring
+        self.add_identity = bool(add_identity)
         self.ctx = ctx if ctx is not None else _lib.Context(device, stream)
         self.width, self.k, self.variant = int(width), int(k), variant
         if fused_style not in ("gather", "scatter"):
@@ -76,6 +106,8 @@ class ArrowEngine:
             st.rows = st.n_blocks * width
             ip, idx, dat, dropped = decomp.arrow_rows(B, width, st.n_blocks, block_diagonal, 0, st.rows, dtype=self.dtype)
             st.dropped = dropped
+            if j == 0 and self.add_identity:
+                ip, idx, dat = decomp.with_diagonal(ip, idx, dat, st.rows, _TIMES_ONE[self.sr], self.dtype)
             st.nnz = int(ip[-1])
             st.csr = self.ctx.csr_upload(st.rows, st.rows, ip, idx, dat, dtype=self.dtype)
             if j > 0:
@@ -107,15 +139,22 @@ class ArrowEngine:
         self.ctx.sync()
 
     # -- buffers ---------------------------------------------------------------------------------
+    def _alloc(self, rows: int) -> _lib.Dense:
+        """a tile holding the semiring's zero (the ⊕ identity)"""
+        b = self.ctx.dense_alloc(rows, self.k, self.dtype)
+        if self.sr != _lib.SR_PLUS_TIMES:
+            b.fill(_PLUS_ZERO[self.sr])
+        return b
+
     def _alloc_buffers(self):
         for j, st in enumerate(self.levels):
             if j == 0 or self.mode == "exchange":
-                st.bufs = [self.ctx.dense_alloc(st.rows, self.k, self.dtype), self.ctx.dense_alloc(st.rows, self.k, self.dtype)]
+                st.bufs = [self._alloc(st.rows), self._alloc(st.rows)]
                 st.xi, st.ci = 0, 0             # zero_rhs: X and C both zero (arrow_slim_mpi.py:354-394)
             if j > 0 and self.mode == "fused":
                 st.csr_fused = st.csr.remap_columns(st.cmap_dev, self.levels[0].rows)
                 if self.fused_style == "gather":
-                    st.cbuf = self.ctx.dense_alloc(st.rows, self.k, self.dtype)     # this level's result tile, written once per step
+                    st.cbuf = self._alloc(st.rows)     # this level's result tile, written once per step
 
     def set_mode(self, mode: str):
         """Switch between 'fused' and 'exchange' (re-allocates level tiles; features are reset)."""
@@ -187,11 +226,11 @@ class ArrowEngine:
         return self.levels[level].rows
 
     def zero_rhs(self):
-        """``zero_rhs`` on every rank of every level (arrow_slim_mpi.py:354-394)."""
+        """``zero_rhs`` on every rank of every level (arrow_slim_mpi.py:354-394): the semiring's zero (the ⊕ identity)."""
         for st in self.levels:
             for b in st.bufs:
                 if b is not None:
-                    b.fill(0.0)
+                    b.fill(_PLUS_ZERO[self.sr])
             st.xi = st.ci = 0
 
     def features(self, level: int = 0, out: Optional[np.ndarray] = None) -> np.ndarray:
@@ -205,7 +244,7 @@ class ArrowEngine:
         self.ensure_level_tiles()
         st = self.levels[level]
         out = 1 - st.xi
-        self.ctx.spmm(st.csr, st.bufs[st.xi], st.bufs[out], variant=self.variant)
+        self._product(st.csr, st.bufs[st.xi], st.bufs[out])
         st.ci = out
 
     def ensure_level_tiles(self):
@@ -228,6 +267,16 @@ class ArrowEngine:
         self.ctx.sync()
 
     # -- the iteration ----------------------------------------------------------------------------------
+    def _product(self, A: _lib.Csr, X: _lib.Dense, C: _lib.Dense, add: Optional[_lib.Dense] = None,
+                 add_map: Optional[_lib.RowMap] = None):
+        """C = A ⊗ X, ⊕ add[add_map] when given, in the engine's semiring ((+, x) honours the kernel variant)"""
+        if self.sr != _lib.SR_PLUS_TIMES:
+            self.ctx.spmm_sr(A, X, C, add, add_map, self.sr)
+        elif add is None:
+            self.ctx.spmm(A, X, C, variant=self.variant)
+        else:
+            self.ctx.spmm_add(A, X, C, add, add_map, variant=self.variant)
+
     def propagate_features(self):
         """Forward exchange (``_propagate_features_forwards``, arrow_dec_mpi.py:507-550)."""
         if self.mode == "fused":
@@ -249,15 +298,15 @@ class ArrowEngine:
                 for j in range(self.L - 1, 0, -1):
                     st = self.levels[j]
                     if j == self.L - 1:
-                        self.ctx.spmm(st.csr_fused, x, st.cbuf, variant=self.variant)
+                        self._product(st.csr_fused, x, st.cbuf)
                     else:
                         nxt = self.levels[j + 1]
-                        self.ctx.spmm_add(st.csr_fused, x, st.cbuf, nxt.cbuf, nxt.to_next_dev, variant=self.variant)
+                        self._product(st.csr_fused, x, st.cbuf, nxt.cbuf, nxt.to_next_dev)
                 if self.L > 1:
                     nxt = self.levels[1]
-                    self.ctx.spmm_add(st0.csr, x, st0.bufs[out], nxt.cbuf, nxt.to_next_dev, variant=self.variant)
+                    self._product(st0.csr, x, st0.bufs[out], nxt.cbuf, nxt.to_next_dev)
                 else:
-                    self.ctx.spmm(st0.csr, x, st0.bufs[out], variant=self.variant)
+                    self._product(st0.csr, x, st0.bufs[out])
             else:
                 self.ctx.spmm(st0.csr, x, st0.bufs[out], variant=self.variant)
                 for st in self.levels[1:]:
@@ -267,7 +316,7 @@ class ArrowEngine:
             return
         for st in self.levels:
             out = 1 - st.xi
-            self.ctx.spmm(st.csr, st.bufs[st.xi], st.bufs[out], variant=self.variant)     # C_i = A @ X_i: fresh tile
+            self._product(st.csr, st.bufs[st.xi], st.bufs[out])                          # C_i = A @ X_i: fresh tile
             st.ci = out
 
     def aggregate(self):
@@ -279,7 +328,10 @@ class ArrowEngine:
         for j in range(self.L - 1, 0, -1):
             st, prev = self.levels[j], self.levels[j - 1]
             # C_{j-1}[to_prev[r]] += C_j[r], written as a gather-add over level j-1 rows (to_prev is injective)
-            self.ctx.gather_rows(prev.bufs[prev.ci], st.bufs[st.ci], st.to_next_dev, accumulate=True)
+            if self.sr == _lib.SR_PLUS_TIMES:
+                self.ctx.gather_rows(prev.bufs[prev.ci], st.bufs[st.ci], st.to_next_dev, accumulate=True)
+            else:
+                self.ctx.gather_rows_sr(prev.bufs[prev.ci], st.bufs[st.ci], st.to_next_dev, self.sr)
             prev.xi = prev.ci                                                             # set_features(C_i) (:438)
 
     def step(self):
@@ -287,6 +339,21 @@ class ArrowEngine:
         self.propagate_features()
         self.spmm()
         self.aggregate()
+
+    def count_changed(self) -> int:
+        """Level-0 rows in which the last ``step()`` changed the features (synchronises).  A step reads one level-0 tile
+        and leaves the result in the other, in both modes, so the two tiles are compared on the device."""
+        st = self.levels[0]
+        return self.ctx.count_diff(st.bufs[0], st.bufs[1])
+
+    def iterate_to_fixed_point(self, max_steps: int) -> int:
+        """``step()`` until a step changes no level-0 row (BFS levels, shortest paths, reachability), at most
+        ``max_steps`` times; returns the number of steps taken (the last one changed nothing unless it hit the limit)."""
+        for n in range(1, int(max_steps) + 1):
+            self.step()
+            if self.count_changed() == 0:
+                return n
+        return int(max_steps)
 
     # -- streaming iteration for host-resident features ------------------------------------------------------
     def stream_step(self, X_host: np.ndarray, out_host: np.ndarray):
@@ -303,8 +370,7 @@ class ArrowEngine:
         ctx = self.ctx
         if not hasattr(self, "_slots"):
             # slot 0 re-uses the engine's own level-0 tiles, slot 1 gets two more
-            self._slots = [list(st.bufs), [ctx.dense_alloc(st.rows, self.k, self.dtype),
-                                           ctx.dense_alloc(st.rows, self.k, self.dtype)]]
+            self._slots = [list(st.bufs), [self._alloc(st.rows), self._alloc(st.rows)]]
             self._slot_i = 0
         s = self._slot_i % 2
         slot = self._slots[s]
@@ -331,6 +397,7 @@ class ArrowEngine:
 
     # -- accounting (SURVEY.md 8d) ------------------------------------------------------------------------
     def flops_per_step(self) -> float:
+        """one ⊗ and one ⊕ per term, in every semiring"""
         return 2.0 * self.total_nnz * self.k
 
     def algorithmic_bytes_per_step(self) -> float:
@@ -350,9 +417,9 @@ class ArrowEngine:
         st = self.levels[j]
         if self.mode == "fused" and self.fused_style == "gather" and j + 1 < self.L:
             nxt = self.levels[j + 1]
-            self.ctx.spmm_add(st.csr, src, dst, nxt.cbuf, nxt.to_next_dev, variant=self.variant)
+            self._product(st.csr, src, dst, nxt.cbuf, nxt.to_next_dev)
         else:
-            self.ctx.spmm(st.csr, src, dst, variant=self.variant)
+            self._product(st.csr, src, dst)
 
     def time_level_spmm(self, j: int, iters: int, warmup: int = 3) -> float:
         """Average duration (ms) of level ``j``'s launch exactly as ``step()`` issues it (level 0 of the fused/gather

@@ -31,7 +31,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 3
+#define ARROW_ABI_VERSION 4
 
 /* error codes */
 #define ARROW_OK              0
@@ -197,6 +197,24 @@ int  arrow_spmm_add(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, 
  * (the reference's stale-row behaviour, arrow_dec_mpi.py:544).  Forward exchange with to_prev,
  * backward exchange (as a gather-add) with to_next. */
 int  arrow_gather_rows(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int flags);
+
+/* ---- semirings (one GPU) --------------------------------------------------------------------------- */
+/* (min, +) / (max, +): ⊗ is the fp32 add (round to nearest, identity 0), ⊕ is fminf / fmaxf (identity +inf / -inf).
+ * ARROW_SR_PLUS_TIMES forwards to arrow_spmm / arrow_spmm_add (ARROW_VARIANT_AUTO, either precision) and to the
+ * accumulating arrow_gather_rows.  MIN_PLUS / MAX_PLUS validate their operands like arrow_spmm_add: mixed precision,
+ * aliasing, bad shapes or an unknown semiring code return ARROW_ERR_ARG, fp64 operands ARROW_ERR_UNSUPPORTED.
+ * Each result element is ⊕ over once-rounded terms, so it does not depend on the kernel, the grid or the order. */
+#define ARROW_SR_PLUS_TIMES 0
+#define ARROW_SR_MIN_PLUS   1
+#define ARROW_SR_MAX_PLUS   2
+/* C[r] = (⊕_p A[r,p] ⊗ X[col_p]) ⊕ add[add_map[r]]  (add_buf / add_map may be -1; rows with add_map[r] == -1 get the
+ * product only; a row without entries, or whose entries are all skipped columns, gets the ⊕ identity) */
+int  arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, int add_map, int semiring);
+/* dst[r] = dst[r] ⊕ src[map[r]] for map[r] >= 0 (the backward exchange of a semiring step) */
+int  arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int semiring);
+/* number of rows of two equally shaped tiles (same rows, k and element type) that differ in some element, compared by
+ * value (-0 == +0, NaN != NaN); synchronises the context's current lane */
+int  arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed);
 
 /* Multi-source gather over NVLink peer memory: `map` holds GLOBAL source rows; source s owns global
  * rows [row_bounds[s], row_bounds[s+1]) and src_bufs[s] is its (wrapped / IPC-imported) tile. */
