@@ -18,7 +18,10 @@ LIB_PATH = os.path.join(_HERE, "libarrow_b200.so")
 
 ACCUMULATE = 1
 F32, F64 = 0, 1                       # ARROW_F32 / ARROW_F64: element type of dense tiles and CSR values
+I32 = 2                               # ARROW_I32: dense tiles of labels / parents (arrow_spmm_sr_witness)
 _DTYPE_CODE = {np.dtype(np.float32): F32, np.dtype(np.float64): F64}
+_TILE_CODE = {**_DTYPE_CODE, np.dtype(np.int32): I32}
+_CODE_TILE = {c: dt for dt, c in _TILE_CODE.items()}
 VARIANT_AUTO, VARIANT_DIRECT, VARIANT_SHFL, VARIANT_TMA, VARIANT_TILES = -1, 0, 1, 2, 3
 SR_PLUS_TIMES, SR_MIN_PLUS, SR_MAX_PLUS = 0, 1, 2     # ARROW_SR_*: the semiring of arrow_spmm_sr / arrow_gather_rows_sr
 SEMIRINGS = {"plus_times": SR_PLUS_TIMES, "min_plus": SR_MIN_PLUS, "max_plus": SR_MAX_PLUS}
@@ -41,8 +44,9 @@ EXPORTS = [
     "arrow_host_alloc_numa", "arrow_bind_thread_to_device_numa", "arrow_preload_kernels",
     "arrow_csr_upload_f64", "arrow_dense_alloc_dtype", "arrow_dense_dtype",
     "arrow_spmm_sr", "arrow_gather_rows_sr", "arrow_dense_count_diff",
+    "arrow_spmm_sr_witness",
 ]
-ABI_VERSION = 4          # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 5          # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -140,6 +144,7 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_spmm_sr": (c_int, [P, I, I, I, I, I, I]),
         "arrow_gather_rows_sr": (c_int, [P, I, I, I, I]),
         "arrow_dense_count_diff": (c_int, [P, I, I, pI64]),
+        "arrow_spmm_sr_witness": (c_int, [P, I, I, I, I, I, I, I, I, I, I]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -291,12 +296,13 @@ class Context:
 
     # -- dense ------------------------------------------------------------------------------
     def dense_alloc(self, rows: int, k: int, dtype=np.float32) -> "Dense":
-        dtype = element_type(dtype)
+        """a zero-filled tile of float32 / float64 features or of int32 labels (``arrow_spmm_sr_witness``)"""
+        dtype = np.dtype(np.int32) if np.dtype(dtype) == np.int32 else element_type(dtype)
         h = c_int()
         if dtype == np.float32:
             self._check(self.lib.arrow_dense_alloc(self._h, int(rows), int(k), byref(h)))
         else:
-            self._check(self.lib.arrow_dense_alloc_dtype(self._h, int(rows), int(k), _DTYPE_CODE[dtype], byref(h)))
+            self._check(self.lib.arrow_dense_alloc_dtype(self._h, int(rows), int(k), _TILE_CODE[dtype], byref(h)))
         return Dense(self, h.value, int(rows), int(k), owned=True, dtype=dtype)
 
     def dense_wrap(self, device_ptr: int, rows: int, k: int) -> "Dense":
@@ -333,6 +339,19 @@ class Context:
         """C[r] = (⊕_p A[r,p] ⊗ X[col_p]) ⊕ add[add_map[r]] in the semiring ``SR_*`` (``arrow_spmm_sr``)"""
         self._check(self.lib.arrow_spmm_sr(self._h, A.h, X.h, C.h, add.h if add is not None else -1,
                                            add_map.h if add_map is not None else -1, int(semiring)))
+
+    def spmm_sr_witness(self, A: "Csr", X: "Dense", labels: "Dense", values: Optional["Dense"] = None,
+                        add_values: Optional["Dense"] = None, add_labels: Optional["Dense"] = None,
+                        add_map: Optional["RowMap"] = None, dist: Optional["Dense"] = None,
+                        row_labels: Optional["RowMap"] = None, semiring: int = SR_MIN_PLUS):
+        """The product of ``spmm_sr`` over (value, label) pairs (``arrow_spmm_sr_witness``): the lexicographic ⊕ of the
+        candidates (fl(A[r,p] + X[c]), c) with c != row_labels[r] (the row index when ``row_labels`` is None), ⊕ the
+        addend pair at add_map[r].  Without ``dist`` the pair goes to ``values`` / ``labels``; with it ``labels``
+        receives the parents (the witness label where dist[r] is not the ⊕ identity and equals the witness value, else
+        -1) and ``values``, when given, the witness values."""
+        h = lambda o: o.h if o is not None else -1
+        self._check(self.lib.arrow_spmm_sr_witness(self._h, A.h, X.h, h(row_labels), h(values), labels.h, h(add_values),
+                                                   h(add_labels), h(add_map), h(dist), int(semiring)))
 
     def spmm_ex(self, A: "Csr", X: "Dense", C: Optional["Dense"] = None, X2: Optional["Dense"] = None, x_split: int = 0,
                 out_table: Optional["PtrTable"] = None, add: Optional["Dense"] = None, add_map: Optional["RowMap"] = None,
@@ -528,7 +547,7 @@ class Dense(_Handle):
         """the element type the library holds for this tile (``arrow_dense_dtype``)"""
         code = c_int()
         self.ctx._check(self.ctx.lib.arrow_dense_dtype(self.ctx._h, self.h, byref(code)))
-        return np.dtype(np.float64 if code.value == F64 else np.float32)
+        return _CODE_TILE[code.value]
 
     def h2d(self, X: np.ndarray, row0: int = 0):
         """upload rows, converted to the tile's element type"""

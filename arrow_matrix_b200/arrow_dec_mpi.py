@@ -158,6 +158,15 @@ class ArrowDecompositionMPI:
         Call ``synchronize()`` before reading ``out_host``.  On N GPUs every rank passes its own rows."""
         self._require_engine().stream_step(X_host, out_host)
 
+    def predecessors(self, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension (one GPU, ``min_plus`` / ``max_plus``): the parent of every element of the level-0 features, int32
+        in ``result_tile()`` row order, ``-1`` for sources and unreachable vertices (see ``ArrowEngine.predecessors``).
+        Entries are level-0 rows; level 0's permutation maps them to vertex ids like the distances."""
+        eng = self._require_engine()
+        if not isinstance(eng, ArrowEngine):
+            raise ValueError("predecessors run on one GPU only")
+        return eng.predecessors(out)
+
     def synchronize(self):
         self._require_engine().sync()
 

@@ -37,7 +37,7 @@
 namespace {
 
 struct DenseBuf {
-    float *p = nullptr;               // element type per `dtype` (double * for ARROW_F64)
+    float *p = nullptr;               // element type per `dtype` (double * for ARROW_F64, int * for ARROW_I32)
     int64_t rows = 0;
     int k = 0;
     int dtype = ARROW_F32;
@@ -213,7 +213,13 @@ IdxMap *get_map(arrow_ctx *ctx, int h) {
 inline int ceil_div_i64(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
 inline size_t dtype_size(int dtype) { return dtype == ARROW_F64 ? 8 : 4; }
-inline const char *dtype_name(int dtype) { return dtype == ARROW_F64 ? "float64" : "float32"; }
+inline const char *dtype_name(int dtype) { return dtype == ARROW_F64 ? "float64" : (dtype == ARROW_I32 ? "int32" : "float32"); }
+// int32 tiles hold labels (arrow_spmm_sr_witness): only the allocation, copies and that launch accept them
+#define REFUSE_I32(ctx, d, what)                                                                                   \
+    do {                                                                                                           \
+        if ((d) != nullptr && (d)->dtype == ARROW_I32)                                                             \
+            return fail((ctx), ARROW_ERR_ARG, "%s: int32 tiles hold labels, no arithmetic runs on them", (what));  \
+    } while (0)
 // first byte of row `r` of a dense tile
 inline char *dense_row(const DenseBuf *d, int64_t r) { return (char *)d->p + (size_t)r * d->k * dtype_size(d->dtype); }
 
@@ -2631,6 +2637,410 @@ int gather_rows_sr(arrow_ctx *ctx, DenseBuf *D, const DenseBuf *S, const IdxMap 
     return ARROW_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// predecessors of the tropical semirings: the product of arrow_spmm_sr carried over (value, label) pairs.  A candidate
+// of row r is an entry p with a valid column c != self(r); its value is fl(A[r,p] + X[c]) and its label is c.  Pairs are
+// ⊕-reduced lexicographically: the better value wins (smaller for (min, +), larger for (max, +)), equal values (by value,
+// -0 == +0) go to the smaller label.  Labels compare as unsigned, so (⊕ identity, -1) is the identity of this ⊕ and a
+// skipped slot is a no-op; a NaN term never wins.  The reduction is therefore exact, associative and commutative: the
+// result does not depend on the kernel, the grid or the order of the terms.
+// ------------------------------------------------------------------------------------------------
+struct WitArgs {
+    TileArgs t;                          // t.a: the product's operands; a.C = the value tile (nullptr: none), a.add_src =
+                                         // the addend's values
+    const int *__restrict__ self;        // row -> the label its own entries carry (-1: none); nullptr: the row index
+    int *__restrict__ lab_out;           // labels (pair out) or parents (dist != nullptr)
+    const int *__restrict__ add_lab;     // the addend's labels (same rows as a.add_src)
+    const float *__restrict__ dist;      // parent epilogue: row r of dist is D[r]; nullptr: pair out
+};
+
+template <class SR>
+__device__ __forceinline__ bool wit_better(float t, float acc) {
+    if constexpr (std::is_same<SR, SrMinPlus>::value) return t < acc;
+    else return t > acc;
+}
+// (av, al) = (av, al) ⊕ (t, l)
+template <class SR>
+__device__ __forceinline__ void wit_plus(float &av, int &al, float t, int l) {
+    const bool take = wit_better<SR>(t, av) || (t == av && (unsigned)l < (unsigned)al);
+    av = take ? t : av;
+    al = take ? l : al;
+}
+template <class SR>
+__device__ __forceinline__ void wit4_mac(float4 &av, int4 &al, float a, const float4 &x, int l) {
+    wit_plus<SR>(av.x, al.x, SR::times(a, x.x), l);
+    wit_plus<SR>(av.y, al.y, SR::times(a, x.y), l);
+    wit_plus<SR>(av.z, al.z, SR::times(a, x.z), l);
+    wit_plus<SR>(av.w, al.w, SR::times(a, x.w), l);
+}
+// the parent of one element: the witness label where D is not the ⊕ identity and the witness value equals it
+template <class SR>
+__device__ __forceinline__ int wit_parent(float d, float v, int l) {
+    return (d != SR::zero() && v == d) ? l : -1;
+}
+__device__ __forceinline__ int4 i4_none() { return make_int4(-1, -1, -1, -1); }
+
+// The k_spmm_tiles_sr pipeline with a label per element.  Epilogues (runtime): the addend pair ⊕-ed in where
+// add_map[r] >= 0; out: the pair (values to a.C when given, labels to lab_out) or, with dist, the parents.
+template <int G, int VPL, class SR, int TR, int TN>
+__global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles_wit(WitArgs w) {
+    constexpr int TILE_PTR_WORDS = TileCfg<TR, TN>::PTR_WORDS;
+    constexpr int TILE_NNZ_WORDS = TileCfg<TR, TN>::NNZ_WORDS;
+    constexpr int TILE_STAGE_WORDS = TileCfg<TR, TN>::STAGE_WORDS;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    int *stage_base = reinterpret_cast<int *>(smem_raw);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)2 * TILE_STAGE_WORDS * 4);
+    const TileArgs &t = w.t;
+    const SpmmArgs &a = t.a;
+    constexpr int RPW = 32 / G;
+    constexpr int UNROLL = (VPL >= 2) ? 2 : 4;                    // a label per element doubles the accumulator
+    constexpr int TAIL = 2;                                       // predicated tail batches
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const bool EXACT = (t.a.k4 == G * VPL);                       // every lane owns valid columns
+    const int gl = lane % G;
+    const int gi = lane / G;
+    const int k4 = a.k4;
+    const float4 *__restrict__ Xl = reinterpret_cast<const float4 *>(a.X) + gl;
+    const uint64_t pol_keep = (t.l2_hints & 1) ? l2_policy_evict_last() : l2_policy_evict_normal();
+    const uint64_t pol_stream = (t.l2_hints & 2) ? l2_policy_evict_first() : l2_policy_evict_normal();
+
+    if (threadIdx.x == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    auto issue_csr = [&](int tile, int st) {
+        const int4 d = __ldg(t.tiles + tile);
+        const int rb4 = d.x & ~3;
+        const int a0 = d.z & ~3;
+        const uint32_t ptr_bytes = (uint32_t)(((d.y - rb4 + 1) + 3) & ~3) * 4u;
+        const uint32_t nnz_bytes = (uint32_t)(((d.w - a0) + 3) & ~3) * 4u;
+        int *sp = stage_base + (size_t)st * TILE_STAGE_WORDS;
+        mbar_expect_tx(&bars[st], ptr_bytes + 2u * nnz_bytes);
+        bulk_g2s_hint(sp, a.indptr + rb4, ptr_bytes, &bars[st], pol_stream);
+        if (nnz_bytes) {
+            bulk_g2s_hint(sp + TILE_PTR_WORDS, a.indices + a0, nnz_bytes, &bars[st], pol_stream);
+            bulk_g2s_hint(sp + TILE_PTR_WORDS + TILE_NNZ_WORDS, a.vals + a0, nnz_bytes, &bars[st], pol_stream);
+        }
+    };
+
+    __shared__ int s_next[TILE_STAGES];
+    int tile = blockIdx.x;
+    if (tile < t.n_tiles && threadIdx.x == 0) issue_csr(tile, 0);
+    for (unsigned int n = 0; tile < t.n_tiles; ++n) {
+        const int st = (int)(n & 1u);
+        if (threadIdx.x == 0) {
+            const int next = atomicAdd(t.ticket, 1) + (int)gridDim.x;
+            s_next[st] = next;
+            if (next < t.n_tiles) issue_csr(next, st ^ 1);
+        }
+        const int4 d = __ldg(t.tiles + tile);
+        mbar_wait(&bars[st], (n >> 1) & 1u);
+        const int *sp = stage_base + (size_t)st * TILE_STAGE_WORDS;
+        const int *s_ptr = sp + (d.x - (d.x & ~3));
+        const int a0 = d.z & ~3;
+        const int *s_idx = sp + TILE_PTR_WORDS - a0;                    // index with global nnz offsets
+        const float *s_val = reinterpret_cast<const float *>(sp + TILE_PTR_WORDS + TILE_NNZ_WORDS) - a0;
+        const int n_rows_tile = d.y - d.x;
+
+        for (int lr = warp * RPW + gi; lr < n_rows_tile; lr += (TILE_THREADS / 32) * RPW) {
+            const int s = s_ptr[lr];
+            const int e = s_ptr[lr + 1];
+            if (e - s > a.long_threshold) continue;
+            const long long row = (long long)d.x + lr;
+            const int own = (w.self != nullptr) ? __ldg(w.self + row) : (int)row;
+            float4 av[VPL];
+            int4 al[VPL];
+#pragma unroll
+            for (int i = 0; i < VPL; ++i) { av[i] = sr4_zero<SR>(); al[i] = i4_none(); }
+            if (a.add_map != nullptr) {
+                const int am = __ldg(a.add_map + row);
+                if (am >= 0) {
+                    const float4 *ar = reinterpret_cast<const float4 *>(a.add_src) + (long long)am * k4 + gl;
+                    const int4 *lr4 = reinterpret_cast<const int4 *>(w.add_lab) + (long long)am * k4 + gl;
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i)
+                        if (gl + i * G < k4) { av[i] = ld_f4_hint(ar + i * G, pol_stream); al[i] = __ldg(lr4 + i * G); }
+                }
+            }
+            int p = s;
+            if (EXACT && !t.skip) {
+                // unpredicated batches; an entry in the row's own column gets the ⊕ identity and label -1 (a no-op)
+                auto batch = [&](auto n_tag) {
+                    constexpr int N = decltype(n_tag)::value;
+                    float4 x[N][VPL];
+#pragma unroll
+                    for (int u = 0; u < N; ++u) {
+                        const float4 *xr = Xl + (long long)s_idx[p + u] * k4;
+#pragma unroll
+                        for (int i = 0; i < VPL; ++i) x[u][i] = ldg_f4_hint(xr + i * G, pol_keep);
+                    }
+#pragma unroll
+                    for (int u = 0; u < N; ++u) {
+                        const int c = s_idx[p + u];
+                        const bool cand = (c != own);
+                        const float v = cand ? s_val[p + u] : SR::zero();
+#pragma unroll
+                        for (int i = 0; i < VPL; ++i) wit4_mac<SR>(av[i], al[i], v, x[u][i], cand ? c : -1);
+                    }
+                    p += N;
+                };
+                while (p + UNROLL <= e) batch(std::integral_constant<int, UNROLL>{});
+                if constexpr (UNROLL >= 4) { if (e - p >= 2) batch(std::integral_constant<int, 2>{}); }
+                if (e - p >= 1) batch(std::integral_constant<int, 1>{});
+            }
+            // tail (and the general case): predicated batches.  A skipped entry (column -1), an entry in the row's own
+            // column or a slot past the row's end is the identity pair (⊕ identity, -1) on zeros: a no-op.
+            for (; p < e; p += TAIL) {
+                float4 x[TAIL][VPL];
+#pragma unroll
+                for (int u = 0; u < TAIL; ++u) {
+                    const int c = (p + u < e) ? s_idx[p + u] : -1;
+                    const float4 *xr = Xl + (long long)c * k4;              // c = -1: address arithmetic only
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i)
+                        x[u][i] = (c >= 0 && gl + i * G < k4) ? ldg_f4_hint(xr + i * G, pol_keep) : f4_zero();
+                }
+#pragma unroll
+                for (int u = 0; u < TAIL; ++u) {
+                    const int c = (p + u < e) ? s_idx[p + u] : -1;
+                    const bool cand = (c >= 0 && c != own);
+                    const float v = cand ? s_val[p + u] : SR::zero();
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i) wit4_mac<SR>(av[i], al[i], v, x[u][i], cand ? c : -1);
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < VPL; ++i) {
+                if (gl + i * G < k4) {
+                    const long long off = row * k4 + gl + i * G;
+                    int4 o = al[i];
+                    if (w.dist != nullptr) {
+                        const float4 dd = __ldg(reinterpret_cast<const float4 *>(w.dist) + off);
+                        o = make_int4(wit_parent<SR>(dd.x, av[i].x, o.x), wit_parent<SR>(dd.y, av[i].y, o.y),
+                                      wit_parent<SR>(dd.z, av[i].z, o.z), wit_parent<SR>(dd.w, av[i].w, o.w));
+                    }
+                    if (a.C != nullptr) st_f4_hint(reinterpret_cast<float4 *>(a.C) + off, av[i], pol_stream);
+                    reinterpret_cast<int4 *>(w.lab_out)[off] = o;
+                }
+            }
+        }
+        __syncthreads();            // stage `st` may be refilled by the next iteration's copy
+        tile = s_next[st];
+    }
+}
+
+// k not a multiple of 4 or k > 256: warp per row, lanes over columns, scalar accesses
+template <class SR>
+__global__ void __launch_bounds__(256) k_spmm_generic_wit(WitArgs w) {
+    const SpmmArgs &a = w.t.a;
+    const int lane = threadIdx.x & 31;
+    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
+    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    for (long long row = warp_id; row < a.n_rows; row += warps_total) {
+        const int s = __ldg(a.indptr + row);
+        const int e = __ldg(a.indptr + row + 1);
+        if (e - s > a.long_threshold) continue;
+        const int own = (w.self != nullptr) ? __ldg(w.self + row) : (int)row;
+        const int am = (a.add_map != nullptr) ? __ldg(a.add_map + row) : -1;
+        for (int c0 = 0; c0 < a.k; c0 += 128) {
+            float av[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
+            int al[4] = {-1, -1, -1, -1};
+            for (int p = s; p < e; ++p) {
+                const int c = __ldg(a.indices + p);
+                const float v = __ldg(a.vals + p);
+                if (c < 0 || c == own) continue;
+                const float *xr = a.X + (long long)c * a.k;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int col = c0 + lane + 32 * i;
+                    if (col < a.k) wit_plus<SR>(av[i], al[i], SR::times(v, __ldg(xr + col)), c);
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int col = c0 + lane + 32 * i;
+                if (col < a.k) {
+                    const long long off = row * a.k + col;
+                    if (am >= 0) wit_plus<SR>(av[i], al[i], a.add_src[(long long)am * a.k + col], w.add_lab[(long long)am * a.k + col]);
+                    if (a.C != nullptr) a.C[off] = av[i];
+                    w.lab_out[off] = (w.dist != nullptr) ? wit_parent<SR>(w.dist[off], av[i], al[i]) : al[i];
+                }
+            }
+        }
+    }
+}
+
+// long rows: one CTA per segment ⊕-reduces its entries into a scratch slot (values, then labels), then one CTA per row
+// ⊕-reduces the slots and the addend and applies the epilogue (k_spmm_long_partial_sr / k_spmm_long_reduce_sr)
+template <class SR>
+__global__ void __launch_bounds__(256) k_spmm_long_partial_wit(LongArgs a, const int *__restrict__ self,
+                                                               int *__restrict__ lab_scratch) {
+    extern __shared__ float red_wv[];   // [warps][k] values, then [warps][k] labels
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    int *red_wl = reinterpret_cast<int *>(red_wv + nwarps * a.k);
+    const LongTask t = a.tasks[blockIdx.x];
+    const int own = (self != nullptr) ? self[t.row] : t.row;
+    for (int c0 = 0; c0 < a.k; c0 += 128) {
+        float av[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
+        int al[4] = {-1, -1, -1, -1};
+        for (int p = t.begin + warp; p < t.end; p += nwarps) {
+            const int c = __ldg(a.indices + p);
+            const float v = __ldg(a.vals + p);
+            if (c < 0 || c == own) continue;
+            const float *xr = a.X + (long long)c * a.k;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int col = c0 + lane + 32 * i;
+                if (col < a.k) wit_plus<SR>(av[i], al[i], SR::times(v, __ldg(xr + col)), c);
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int col = c0 + lane + 32 * i;
+            if (col < a.k) { red_wv[warp * a.k + col] = av[i]; red_wl[warp * a.k + col] = al[i]; }
+        }
+    }
+    __syncthreads();
+    for (int col = threadIdx.x; col < a.k; col += blockDim.x) {
+        float v = SR::zero();
+        int l = -1;
+        for (int w = 0; w < nwarps; ++w) wit_plus<SR>(v, l, red_wv[w * a.k + col], red_wl[w * a.k + col]);
+        a.scratch[(long long)t.slot * a.k + col] = v;
+        lab_scratch[(long long)t.slot * a.k + col] = l;
+    }
+}
+
+template <class SR>
+__global__ void __launch_bounds__(128) k_spmm_long_reduce_wit(const int *__restrict__ long_rows,
+                                                              const int *__restrict__ long_first,
+                                                              const float *__restrict__ scratch,
+                                                              const int *__restrict__ lab_scratch, WitArgs w) {
+    const SpmmArgs &a = w.t.a;
+    const int r = long_rows[blockIdx.x];
+    const int am = (a.add_map != nullptr) ? a.add_map[r] : -1;
+    const int s0 = long_first[blockIdx.x], s1 = long_first[blockIdx.x + 1];
+    const int k = a.k;
+    for (int col = threadIdx.x; col < k; col += blockDim.x) {
+        float v = SR::zero();
+        int l = -1;
+        for (int s = s0; s < s1; ++s) wit_plus<SR>(v, l, scratch[(long long)s * k + col], lab_scratch[(long long)s * k + col]);
+        if (am >= 0) wit_plus<SR>(v, l, a.add_src[(long long)am * k + col], w.add_lab[(long long)am * k + col]);
+        const long long off = (long long)r * k + col;
+        if (a.C != nullptr) a.C[off] = v;
+        w.lab_out[off] = (w.dist != nullptr) ? wit_parent<SR>(w.dist[off], v, l) : l;
+    }
+}
+
+template <int G, int VPL, class SR, int TR, int TN>
+int launch_tiles_wit_one(arrow_ctx *ctx, const WitArgs &w) {
+    constexpr size_t SMEM = TileCfg<TR, TN>::SMEM_BYTES;
+    auto fn = k_spmm_tiles_wit<G, VPL, SR, TR, TN>;
+    static bool attr_set[64] = {};            /* function attributes are per device */
+    static int occ_dev[64] = {};
+    const int dv = ctx->device & 63;
+    if (!attr_set[dv]) {
+        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
+        attr_set[dv] = true;
+    }
+    const int occ = occ_dev[dv];
+    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
+    int sms = ctx->sm_count;
+    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
+    int grid = (int)std::min<long long>((long long)per_sm * sms, w.t.n_tiles);
+    cudaMemsetAsync(w.t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
+    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(w);
+    ctx->launches++;
+    return ARROW_OK;
+}
+
+// (lanes per row, float4 per lane): one float4 per lane up to 32 lanes (k <= 128), then two (k <= 256); big tiles as
+// launch_tiles picks them (k <= 32)
+int launch_tiles_wit_shape(arrow_ctx *ctx, WitArgs &w, const Csr *A, bool min_plus) {
+    TileArgs &t = w.t;
+    const int k4 = t.a.k4;
+    const int vpl = (k4 > 32) ? 2 : 1;
+    const int lanes = (k4 + vpl - 1) / vpl;           // <= 32: k4 <= 64
+    int g = 1;
+    while (g < lanes) g <<= 1;
+    const bool big = (k4 <= 8) && ctx->big_tiles && A->n_tiles_big > 0;
+    if (big) { t.tiles = A->tiles_big; t.n_tiles = A->n_tiles_big; }
+#define TWI(GG, VV, TR, TN)                                                                              \
+    return min_plus ? launch_tiles_wit_one<GG, VV, SrMinPlus, TR, TN>(ctx, w) : launch_tiles_wit_one<GG, VV, SrMaxPlus, TR, TN>(ctx, w)
+#define WIB(GG, VV) if (big && g == GG && vpl == VV) TWI(GG, VV, TILE_ROWS_BIG, TILE_NNZ_BIG)
+#define WIS(GG, VV) if (g == GG && vpl == VV) TWI(GG, VV, TILE_ROWS, TILE_NNZ)
+    WIB(1, 1); WIB(2, 1); WIB(4, 1); WIB(8, 1);
+    WIS(1, 1); WIS(2, 1); WIS(4, 1); WIS(8, 1); WIS(16, 1); WIS(32, 1); WIS(32, 2);
+#undef WIS
+#undef WIB
+#undef TWI
+    return fail(ctx, ARROW_ERR_UNSUPPORTED, "no witness tile kernel for k4=%d vpl=%d", k4, vpl);
+}
+
+// the launches of arrow_spmm_sr_witness; `w` carries the validated fp32 operands
+template <class SR>
+int spmm_wit(arrow_ctx *ctx, const Csr *A, WitArgs &w, bool min_plus) {
+    const SpmmArgs &a = w.t.a;
+    const int k = a.k;
+    const int lane = ctx->cur_lane;
+    cudaStream_t stream = cur_stream(ctx);
+    if (k % 4 != 0 || k > 256) {
+        const long long ctas = (A->n_rows + 7) / 8;
+        auto fn = k_spmm_generic_wit<SR>;
+        const int grid = grid_for(ctx, (const void *)fn, 256, 0, ctas);
+        fn<<<grid, 256, 0, stream>>>(w);
+        ctx->launches++;
+    } else if (A->n_tiles > 0) {
+        w.t.tiles = A->tiles;
+        w.t.n_tiles = A->n_tiles;
+        w.t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
+        w.t.ticket = ctx->tile_ticket + 2 * lane;
+        w.t.l2_hints = ctx->l2_hints_plain;
+        w.t.prefetch = 0;
+        const int rc = launch_tiles_wit_shape(ctx, w, A, min_plus);
+        if (rc != ARROW_OK) return rc;
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+
+    if (A->n_long_tasks > 0) {
+        const size_t slots = (size_t)A->n_long_tasks * k;
+        const size_t need = slots * 8;                     // values, then labels
+        if (need > ctx->long_scratch_bytes[lane]) {
+            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
+            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
+            ctx->long_scratch[lane] = nullptr;
+            ctx->long_scratch_bytes[lane] = 0;
+            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
+            ctx->long_scratch_bytes[lane] = need;
+        }
+        LongArgs la;
+        la.tasks = A->long_tasks;
+        la.indices = a.indices;
+        la.vals = a.vals;
+        la.X = a.X;
+        la.scratch = ctx->long_scratch[lane];
+        la.k = k;
+        la.X2 = nullptr;
+        la.x_split = 0;
+        int *lab_scratch = reinterpret_cast<int *>(ctx->long_scratch[lane] + slots);
+        const size_t smem = (size_t)8 * k * 8;
+        if (smem > 48 * 1024)
+            CUDA_TRY(ctx, cudaFuncSetAttribute(k_spmm_long_partial_wit<SR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_spmm_long_partial_wit<SR><<<A->n_long_tasks, 256, smem, stream>>>(la, w.self, lab_scratch);
+        ctx->launches++;
+        k_spmm_long_reduce_wit<SR><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, la.scratch,
+                                                                        lab_scratch, w);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
+    return ARROW_OK;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -3139,7 +3549,7 @@ int arrow_map_d2h(arrow_ctx *ctx, int map, int32_t *host, int64_t n) {
 int arrow_dense_alloc_dtype(arrow_ctx *ctx, int64_t rows, int k, int dtype, int *buf_out) {
     CHECK_CTX(ctx);
     if (!buf_out || rows < 0 || k < 1) return fail(ctx, ARROW_ERR_ARG, "bad dense shape %lld x %d", (long long)rows, k);
-    if (dtype != ARROW_F32 && dtype != ARROW_F64) return fail(ctx, ARROW_ERR_ARG, "unknown dtype %d", dtype);
+    if (dtype != ARROW_F32 && dtype != ARROW_F64 && dtype != ARROW_I32) return fail(ctx, ARROW_ERR_ARG, "unknown dtype %d", dtype);
     DenseBuf d;
     d.rows = rows;
     d.k = k;
@@ -3188,6 +3598,7 @@ int arrow_dense_fill(arrow_ctx *ctx, int buf, float value) {
     CHECK_CTX(ctx);
     DenseBuf *d = get_dense(ctx, buf);
     if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", buf);
+    REFUSE_I32(ctx, d, "arrow_dense_fill");
     const long long n = (long long)d->rows * d->k;
     if (n == 0) return ARROW_OK;
     if (value == 0.f) {
@@ -3532,6 +3943,7 @@ int arrow_ptrtable_upload(arrow_ctx *ctx, const int *bufs, int n_bufs, const int
         if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", bufs[b]);
         if (b == 0) k = d->k;
         else if (d->k != k) return fail(ctx, ARROW_ERR_ARG, "tiles of a pointer table must share the feature width");
+        REFUSE_I32(ctx, d, "arrow_ptrtable_upload");
         if (d->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "pointer tables are float32 only");
         bases[b] = (unsigned long long)d->p;
         rows_of[b] = d->rows;
@@ -3642,6 +4054,7 @@ int arrow_gather_rows(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int fla
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
     if (D->k != S->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch %d vs %d", D->k, S->k);
     if (D->dtype != S->dtype) return fail(ctx, ARROW_ERR_ARG, "dtype mismatch: destination %s, source %s", dtype_name(D->dtype), dtype_name(S->dtype));
+    REFUSE_I32(ctx, D, "arrow_gather_rows");
     if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "gather source and destination must not alias");
     if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
     if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
@@ -3714,6 +4127,7 @@ int arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int 
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
     if (D->k != S->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch %d vs %d", D->k, S->k);
     if (D->dtype != S->dtype) return fail(ctx, ARROW_ERR_ARG, "dtype mismatch: destination %s, source %s", dtype_name(D->dtype), dtype_name(S->dtype));
+    REFUSE_I32(ctx, D, "arrow_gather_rows_sr");
     if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "gather source and destination must not alias");
     if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
     if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
@@ -3722,12 +4136,94 @@ int arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int 
     return gather_rows_sr<SrMaxPlus>(ctx, D, S, m);
 }
 
+// ---- predecessors ---------------------------------------------------------------------------------
+int arrow_spmm_sr_witness(arrow_ctx *ctx, int csr, int x_buf, int row_labels, int val_out, int lab_out, int add_val,
+                          int add_lab, int add_map, int dist_buf, int semiring) {
+    CHECK_CTX(ctx);
+    if (semiring == ARROW_SR_PLUS_TIMES)
+        return fail(ctx, ARROW_ERR_UNSUPPORTED, "predecessors exist in the (min, +) / (max, +) semirings only");
+    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS)
+        return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
+    CHECK_POISON(ctx);
+    Csr *A = get_csr(ctx, csr);
+    DenseBuf *X = get_dense(ctx, x_buf);
+    DenseBuf *L = get_dense(ctx, lab_out);
+    DenseBuf *V = val_out >= 0 ? get_dense(ctx, val_out) : nullptr;
+    DenseBuf *D = dist_buf >= 0 ? get_dense(ctx, dist_buf) : nullptr;
+    if (!A) return fail(ctx, ARROW_ERR_HANDLE, "bad csr handle %d", csr);
+    if (!X || !L) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x=%d lab_out=%d)", x_buf, lab_out);
+    if (val_out >= 0 && !V) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (val_out=%d)", val_out);
+    if (dist_buf >= 0 && !D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (dist=%d)", dist_buf);
+    if (!V && !D) return fail(ctx, ARROW_ERR_ARG, "the pair epilogue (dist_buf < 0) needs a value tile");
+    if (X->dtype != A->dtype || (V && V->dtype != A->dtype) || (D && D->dtype != A->dtype))
+        return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, X is %s, val_out is %s, dist is %s", dtype_name(A->dtype),
+                    dtype_name(X->dtype), V ? dtype_name(V->dtype) : "-", D ? dtype_name(D->dtype) : "-");
+    if (L->dtype != ARROW_I32) return fail(ctx, ARROW_ERR_ARG, "lab_out is %s, labels are int32", dtype_name(L->dtype));
+    const int k = X->k;
+    if (L->k != k || (V && V->k != k) || (D && D->k != k))
+        return fail(ctx, ARROW_ERR_ARG, "X has %d feature columns, lab_out %d, val_out %d, dist %d", k, L->k, V ? V->k : -1, D ? D->k : -1);
+    if (X->rows < A->n_cols) return fail(ctx, ARROW_ERR_ARG, "X has %lld rows, block has %lld columns", (long long)X->rows, (long long)A->n_cols);
+    if (L->rows < A->n_rows || (V && V->rows < A->n_rows) || (D && D->rows < A->n_rows))
+        return fail(ctx, ARROW_ERR_ARG, "an output or dist tile has fewer rows than the block (%lld)", (long long)A->n_rows);
+    IdxMap *self = nullptr;
+    if (row_labels >= 0) {
+        self = get_map(ctx, row_labels);
+        if (!self) return fail(ctx, ARROW_ERR_HANDLE, "bad row label map %d", row_labels);
+        if (self->n < A->n_rows) return fail(ctx, ARROW_ERR_ARG, "row label map has %lld entries, block has %lld rows", (long long)self->n, (long long)A->n_rows);
+    }
+    DenseBuf *SV = nullptr, *SL = nullptr;
+    IdxMap *am = nullptr;
+    if (add_val >= 0 || add_lab >= 0 || add_map >= 0) {
+        SV = get_dense(ctx, add_val);
+        SL = get_dense(ctx, add_lab);
+        am = get_map(ctx, add_map);
+        if (!SV || !SL || !am) return fail(ctx, ARROW_ERR_HANDLE, "bad addend handles (val=%d lab=%d map=%d)", add_val, add_lab, add_map);
+        if (SV->dtype != A->dtype) return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, the addend is %s", dtype_name(A->dtype), dtype_name(SV->dtype));
+        if (SL->dtype != ARROW_I32) return fail(ctx, ARROW_ERR_ARG, "the addend's labels are %s, labels are int32", dtype_name(SL->dtype));
+        if (SV->k != k || SL->k != k) return fail(ctx, ARROW_ERR_ARG, "addend has %d / %d feature columns, expected %d", SV->k, SL->k, k);
+        if (am->n < A->n_rows) return fail(ctx, ARROW_ERR_ARG, "addend map has %lld entries, block has %lld rows", (long long)am->n, (long long)A->n_rows);
+        if (am->limit > SV->rows || am->limit > SL->rows)
+            return fail(ctx, ARROW_ERR_ARG, "addend map reaches row %lld, addend tiles have %lld / %lld rows", (long long)am->limit, (long long)SV->rows, (long long)SL->rows);
+    }
+    // the outputs alias nothing the launch reads, nor each other
+    const void *outs[2] = {V ? (const void *)V->p : nullptr, (const void *)L->p};
+    const void *ins[4] = {X->p, SV ? (const void *)SV->p : nullptr, SL ? (const void *)SL->p : nullptr, D ? (const void *)D->p : nullptr};
+    if (outs[0] == outs[1]) return fail(ctx, ARROW_ERR_ARG, "val_out and lab_out must not alias");
+    for (const void *o : outs)
+        for (const void *i : ins)
+            if (o != nullptr && o == i) return fail(ctx, ARROW_ERR_ARG, "an output tile aliases an input tile");
+    if (A->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "predecessors of the (min, +) / (max, +) semirings are float32 only");
+    if (A->n_rows == 0) return ARROW_OK;
+    WitArgs w;
+    memset(&w, 0, sizeof w);
+    SpmmArgs &a = w.t.a;
+    a.indptr = A->indptr;
+    a.indices = A->indices;
+    a.vals = A->vals;
+    a.X = X->p;
+    a.C = V ? V->p : nullptr;
+    a.n_rows = A->n_rows;
+    a.k = k;
+    a.k4 = k / 4;
+    a.long_threshold = A->long_threshold;
+    a.add_src = SV ? SV->p : nullptr;
+    a.add_map = am ? am->p : nullptr;
+    w.self = self ? self->p : nullptr;
+    w.lab_out = reinterpret_cast<int *>(L->p);
+    w.add_lab = SL ? reinterpret_cast<const int *>(SL->p) : nullptr;
+    w.dist = D ? D->p : nullptr;
+    if (semiring == ARROW_SR_MIN_PLUS) return spmm_wit<SrMinPlus>(ctx, A, w, true);
+    return spmm_wit<SrMaxPlus>(ctx, A, w, false);
+}
+
 int arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed) {
     CHECK_CTX(ctx);
     CHECK_POISON(ctx);
     DenseBuf *A = get_dense(ctx, a), *B = get_dense(ctx, b);
     if (!A || !B) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (a=%d b=%d)", a, b);
     if (!rows_changed) return fail(ctx, ARROW_ERR_ARG, "null rows_changed");
+    REFUSE_I32(ctx, A, "arrow_dense_count_diff");
+    REFUSE_I32(ctx, B, "arrow_dense_count_diff");
     if (A->rows != B->rows || A->k != B->k || A->dtype != B->dtype)
         return fail(ctx, ARROW_ERR_ARG, "tiles differ in shape or type: %lld x %d %s vs %lld x %d %s", (long long)A->rows, A->k,
                     dtype_name(A->dtype), (long long)B->rows, B->k, dtype_name(B->dtype));
@@ -3759,6 +4255,7 @@ int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, co
     if (!D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", dst_buf);
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
     if (!src_bufs || !row_bounds || n_src < 1 || n_src > MAX_SRC) return fail(ctx, ARROW_ERR_ARG, "need 1..%d sources", MAX_SRC);
+    REFUSE_I32(ctx, D, "arrow_gather_rows_multi");
     if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the multi-source gather is float32 only");
     if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
     MultiSrc ms;
@@ -3768,6 +4265,7 @@ int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, co
         DenseBuf *S = get_dense(ctx, src_bufs[s]);
         if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad source handle %d", src_bufs[s]);
         if (S->k != D->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in source %d", s);
+        REFUSE_I32(ctx, S, "arrow_gather_rows_multi");
         if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the multi-source gather is float32 only");
         if (row_bounds[s + 1] < row_bounds[s] || row_bounds[s + 1] - row_bounds[s] > S->rows)
             return fail(ctx, ARROW_ERR_ARG, "source %d owns %lld rows but its tile has %lld", s, (long long)(row_bounds[s + 1] - row_bounds[s]), (long long)S->rows);
@@ -3787,6 +4285,7 @@ int arrow_push_rows(arrow_ctx *ctx, const int *dst_bufs, const int64_t *item_bou
     IdxMap *m = get_map(ctx, map);
     if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", src_buf);
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
+    REFUSE_I32(ctx, S, "arrow_push_rows");
     if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_push_rows is float32 only");
     if (!dst_bufs || !item_bounds || n_dst < 1 || n_dst > MAX_SRC) return fail(ctx, ARROW_ERR_ARG, "need 1..%d destinations", MAX_SRC);
     if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
@@ -3802,6 +4301,7 @@ int arrow_push_rows(arrow_ctx *ctx, const int *dst_bufs, const int64_t *item_bou
         DenseBuf *D = get_dense(ctx, dst_bufs[d]);
         if (!D) return fail(ctx, ARROW_ERR_HANDLE, "bad destination handle %d", dst_bufs[d]);
         if (D->k != S->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in destination %d", d);
+        REFUSE_I32(ctx, D, "arrow_push_rows");
         if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_push_rows is float32 only");
         if (cnt > D->rows) return fail(ctx, ARROW_ERR_ARG, "destination %d receives %lld rows but its region has %lld", d, (long long)cnt, (long long)D->rows);
         if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "push source and destination must not alias");
@@ -3849,6 +4349,7 @@ int arrow_reduce_rows(arrow_ctx *ctx, int dst_buf, int out_table, const int *src
     if (!src_bufs || n_src < 1 || n_src > MAX_SRC || rows < 0) return fail(ctx, ARROW_ERR_ARG, "need 1..%d sources", MAX_SRC);
     DenseBuf *D = dst_buf >= 0 ? get_dense(ctx, dst_buf) : nullptr;
     if (dst_buf >= 0 && !D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", dst_buf);
+    REFUSE_I32(ctx, D, "arrow_reduce_rows");
     if (D && D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_reduce_rows is float32 only");
     PtrTable *OT = nullptr;
     if (out_table >= 0) {
@@ -3868,6 +4369,7 @@ int arrow_reduce_rows(arrow_ctx *ctx, int dst_buf, int out_table, const int *src
         if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad source handle %d", src_bufs[s2]);
         if (s2 == 0) k = S->k;
         if (S->k != k || (D && D->k != k) || (OT && OT->k != k)) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in source %d", s2);
+        REFUSE_I32(ctx, S, "arrow_reduce_rows");
         if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_reduce_rows is float32 only");
         if (S->rows < rows) return fail(ctx, ARROW_ERR_ARG, "source %d has %lld rows, %lld are reduced", s2, (long long)S->rows, (long long)rows);
         ms.p[s2] = S->p;

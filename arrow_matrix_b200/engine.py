@@ -26,6 +26,10 @@ where ⊗ is the float32 add and ⊕ is min / max.  The decomposition carries ov
 levels in any semiring): the forward exchange only moves rows, the backward aggregation becomes a ⊕, and the stale rows
 behind the sentinel are the same.  ``add_identity`` puts the ⊗ identity on level 0's diagonal, so that a step computes
 ``X ⊕ (A ⊗ X)``: the relaxation step of BFS and Bellman-Ford (``(I + A) X`` in ``plus_times``).
+
+``predecessors()`` returns, in the tropical semirings, the level-0 row each element's value came from (the parent array
+of a BFS tree, the predecessor of a shortest or critical path): one more pass of the fused step over (value, label)
+pairs, see DESIGN.md §4.
 """
 from __future__ import annotations
 
@@ -98,6 +102,8 @@ class ArrowEngine:
         self.perms, self.to_prev, self.to_next, self.sentinel = decomp.prepare_permutations(
             [p for _, p in decomposition], self.n_blocks, width)
         self.levels: List[_LevelState] = []
+        self._wit_labels: Optional[List[_lib.Dense]] = None     # predecessors(): int32 label tile per level (level 0: P)
+        self._wit_values = {}                                    # predecessors(): value tiles of levels without a cbuf
         fused_ok = True
         cmap_prev = None                      # level j-1 row -> level-0 row (host, int64, -1 invalid)
         for j, (B, _) in enumerate(decomposition):
@@ -355,6 +361,58 @@ class ArrowEngine:
                 return n
         return int(max_steps)
 
+    # -- predecessors (min_plus / max_plus) ----------------------------------------------------------------------
+    def predecessors(self, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Parents of the current level-0 features ``D`` (int32 [n x k], level-0 row order like ``result()``): ``P[v, s]``
+        is the level-0 row ``u`` of the witness of ``(v, s)`` -- the lexicographic ⊕ of the terms ``fl(a + D[u, s])`` the
+        fused step reduces into row ``v`` at any level, with ``u != v``, ties to the smallest ``u`` -- where ``D[v, s]``
+        is not the ⊕ identity and equals the witness value; ``-1`` elsewhere (sources, unreachable vertices).  At a fixed
+        point of the step with ``add_identity`` every vertex whose value came from an edge has a parent.  Synchronises.
+
+        One pass over the levels, deepest first, on the column-remapped level matrices of the fused step (built on the
+        first call and kept in exchange mode); value tiles are the levels' ``cbuf`` in fused mode (so ``result(j)`` for
+        ``j >= 1`` is overwritten there), label tiles are allocated on the first call.  Features, results of level 0,
+        the exchange-mode level tiles and the streaming slots are not touched: the next ``step()`` is the same.
+        Raises ``ValueError`` in ``plus_times`` and when a level reads rows behind the sentinel (``fused_ok`` is false:
+        such a row has no vertex identity)."""
+        if self.sr == _lib.SR_PLUS_TIMES:
+            raise ValueError("predecessors exist in the min_plus / max_plus semirings only, the engine runs plus_times")
+        if not self.fused_ok:
+            raise ValueError("predecessors need a level-0 row behind every non-zero, but a level reads rows behind the "
+                             "sentinel")
+        self.sync()
+        return self._predecessor_pass().d2h(out)
+
+    def _predecessor_pass(self) -> _lib.Dense:
+        """enqueue the launches of ``predecessors()`` (stream-ordered); returns the level-0 label tile holding P"""
+        st0 = self.levels[0]
+        x = st0.bufs[st0.xi]
+        if self._wit_labels is None:
+            self._wit_labels = [self.ctx.dense_alloc(st.rows, self.k, np.int32) for st in self.levels]
+        values = {}
+        for j in range(self.L - 1, 0, -1):
+            st = self.levels[j]
+            if st.csr_fused is None:                  # exchange mode: the remapped copy of the fused step, kept
+                st.csr_fused = st.csr.remap_columns(st.cmap_dev, st0.rows)
+            if st.cbuf is not None:
+                values[j] = st.cbuf
+            else:
+                if j not in self._wit_values:
+                    self._wit_values[j] = self.ctx.dense_alloc(st.rows, self.k)
+                values[j] = self._wit_values[j]
+            add = {}
+            if j + 1 < self.L:
+                nxt = self.levels[j + 1]
+                add = dict(add_values=values[j + 1], add_labels=self._wit_labels[j + 1], add_map=nxt.to_next_dev)
+            self.ctx.spmm_sr_witness(st.csr_fused, x, self._wit_labels[j], values[j], row_labels=st.cmap_dev,
+                                     semiring=self.sr, **add)
+        add = {}
+        if self.L > 1:
+            nxt = self.levels[1]
+            add = dict(add_values=values[1], add_labels=self._wit_labels[1], add_map=nxt.to_next_dev)
+        self.ctx.spmm_sr_witness(st0.csr, x, self._wit_labels[0], dist=x, semiring=self.sr, **add)
+        return self._wit_labels[0]
+
     # -- streaming iteration for host-resident features ------------------------------------------------------
     def stream_step(self, X_host: np.ndarray, out_host: np.ndarray):
         """Enqueue one full iteration on host data: upload ``X_host`` -> ``step()`` -> download level-0 result
@@ -452,4 +510,7 @@ class ArrowEngine:
         return b
 
     def close(self):
+        for b in (self._wit_labels or []) + list(self._wit_values.values()):
+            b.free()
+        self._wit_labels, self._wit_values = None, {}
         self.ctx.close()

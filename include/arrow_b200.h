@@ -14,7 +14,8 @@
  * arrow_last_error), no exceptions cross the boundary.  The caller owns host memory; the library
  * owns device memory (handles are small non-negative ints, valid for one context).  All work is
  * stream-ordered on the context's stream; arrow_sync() waits for it.  One host thread per context.
- * Dense tiles are row-major [rows x k] of fp32 or fp64; CSR is fp32 or fp64 values with int32 indices on the device.
+ * Dense tiles are row-major [rows x k] of fp32 or fp64 (or int32 labels); CSR is fp32 or fp64 values with int32 indices
+ * on the device.
  * The precision is fixed when a tile is allocated / a block uploaded (ARROW_F32 / ARROW_F64), and every operand of one
  * launch has the same precision.  fp64 covers the one-GPU product (arrow_spmm, arrow_spmm_add, arrow_gather_rows); the
  * multi-GPU entry points (two-part operand, pointer tables, push / reduce, multi-source gather) are fp32 only.
@@ -31,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 4
+#define ARROW_ABI_VERSION 5
 
 /* error codes */
 #define ARROW_OK              0
@@ -45,6 +46,9 @@ typedef struct arrow_ctx arrow_ctx;
 /* element types of dense tiles and CSR values */
 #define ARROW_F32             0
 #define ARROW_F64             1
+#define ARROW_I32             2   /* dense tiles only: labels / parents of arrow_spmm_sr_witness.  Allocation, free, h2d / d2h
+                                     (and the lane copies), copy and arrow_dense_dtype accept it; every arithmetic launch
+                                     refuses an int32 operand with ARROW_ERR_ARG */
 
 /* flags for arrow_spmm / arrow_gather_rows */
 #define ARROW_ACCUMULATE      1   /* C += ... instead of C = ...  (reference: `C_i += A_i0 @ X_0`,
@@ -134,11 +138,11 @@ int  arrow_map_d2h(arrow_ctx *ctx, int map, int32_t *host, int64_t n);
 
 /* ---- dense tiles (X_i / C_i / X_0 / C_0 of arrow_slim_mpi.py:354-394, concatenated) ----------- */
 int  arrow_dense_alloc(arrow_ctx *ctx, int64_t rows, int k, int *buf_out);      /* fp32, zero filled */
-int  arrow_dense_alloc_dtype(arrow_ctx *ctx, int64_t rows, int k, int dtype, int *buf_out);   /* ARROW_F32 / ARROW_F64 */
+int  arrow_dense_alloc_dtype(arrow_ctx *ctx, int64_t rows, int k, int dtype, int *buf_out);   /* ARROW_F32 / F64 / I32 */
 int  arrow_dense_dtype(arrow_ctx *ctx, int buf, int *dtype);
 int  arrow_dense_free(arrow_ctx *ctx, int buf);
 int  arrow_dense_fill(arrow_ctx *ctx, int buf, float value);                    /* converted to the tile's type */
-/* host rows are of the tile's element type (float or double) */
+/* host rows are of the tile's element type (float, double or int32_t) */
 int  arrow_dense_h2d(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, const void *host);
 int  arrow_dense_d2h(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, void *host);
 /* both tiles have the same element type, else ARROW_ERR_ARG */
@@ -215,6 +219,24 @@ int  arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int
 /* number of rows of two equally shaped tiles (same rows, k and element type) that differ in some element, compared by
  * value (-0 == +0, NaN != NaN); synchronises the context's current lane */
 int  arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed);
+
+/* ---- predecessors of the tropical semirings (one GPU, fp32) ------------------------------------------ */
+/* The product of arrow_spmm_sr over (value, label) pairs.  A candidate of row r is an entry p whose column c is valid
+ * (not a skipped -1) and differs from the row's own label self(r); its value is fl(A[r,p] + X[c]) and its label c.
+ * The witness of an element is the lexicographic ⊕ of its candidates: the better value wins (smaller for MIN_PLUS,
+ * larger for MAX_PLUS), equal values (-0 == +0) go to the smaller label; a NaN term never wins; no candidate gives
+ * (⊕ identity, -1).  The addend pair (add_val, add_lab)[add_map[r]] is ⊕-ed in where add_map[r] >= 0.  Exact: the
+ * result does not depend on the kernel, the grid or the order of the terms.
+ *   row_labels: map with self(r) per row (-1: none), or -1: self(r) = r
+ *   dist_buf < 0:  pair out, values to val_out (fp32), labels to lab_out (int32)
+ *   dist_buf >= 0: parents to lab_out: P[r] = label where D[r] (row r of dist_buf; it may be x_buf) is not the ⊕
+ *                  identity and the witness value equals it, else -1; values to val_out when val_out >= 0
+ *   add_val / add_lab / add_map: all three or none (-1)
+ * Every output has the block's rows and X's k; no output aliases an input or the other output.  ARROW_SR_PLUS_TIMES
+ * and fp64 operands: ARROW_ERR_UNSUPPORTED; mixed or wrong element types, bad shapes, aliasing, an unknown semiring
+ * code: ARROW_ERR_ARG. */
+int  arrow_spmm_sr_witness(arrow_ctx *ctx, int csr, int x_buf, int row_labels, int val_out, int lab_out, int add_val,
+                           int add_lab, int add_map, int dist_buf, int semiring);
 
 /* Multi-source gather over NVLink peer memory: `map` holds GLOBAL source rows; source s owns global
  * rows [row_bounds[s], row_bounds[s+1]) and src_bufs[s] is its (wrapped / IPC-imported) tile. */
