@@ -44,9 +44,9 @@ EXPORTS = [
     "arrow_host_alloc_numa", "arrow_bind_thread_to_device_numa", "arrow_preload_kernels",
     "arrow_csr_upload_f64", "arrow_dense_alloc_dtype", "arrow_dense_dtype",
     "arrow_spmm_sr", "arrow_gather_rows_sr", "arrow_dense_count_diff",
-    "arrow_spmm_sr_witness",
+    "arrow_spmm_sr_witness", "arrow_tile_rows", "arrow_tile_rows_rule",
 ]
-ABI_VERSION = 5          # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 6         # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -145,6 +145,8 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_gather_rows_sr": (c_int, [P, I, I, I, I]),
         "arrow_dense_count_diff": (c_int, [P, I, I, pI64]),
         "arrow_spmm_sr_witness": (c_int, [P, I, I, I, I, I, I, I, I, I, I]),
+        "arrow_tile_rows": (c_int, [P, I, I, pI]),
+        "arrow_tile_rows_rule": (c_int, [I, I, I64, I, I]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -252,10 +254,16 @@ class Context:
 
     OPT_L2_HINTS_PLAIN, OPT_L2_HINTS_FUSED, OPT_BIG_TILES, OPT_SPMM_CTAS_PER_SM, OPT_PREFETCH = 1, 2, 3, 4, 5
     OPT_ROWS_PER_GROUP, OPT_SPMM_SM_LIMIT, OPT_PUSH_CTAS, OPT_BARRIER_TIMEOUT_MS, OPT_SMEM_CARVEOUT = 6, 7, 8, 9, 10
-    OPT_FORCE_PREDICATED, OPT_TILE_KERNEL, OPT_PUSH_INTERLEAVE = 11, 12, 13
+    OPT_FORCE_PREDICATED, OPT_TILE_KERNEL, OPT_PUSH_INTERLEAVE, OPT_TILE_ROWS = 11, 12, 13, 14
 
     def set_option(self, option: int, value: int):
         self._check(self.lib.arrow_set_option(self._h, int(option), int(value)))
+
+    def tile_rows(self, k: int, dtype=np.float32) -> int:
+        """rows per CSR tile of this context's tile-kernel launches at feature width ``k`` (``arrow_tile_rows``)"""
+        rows = c_int()
+        self._check(self.lib.arrow_tile_rows(self._h, int(k), _DTYPE_CODE[element_type(dtype)], byref(rows)))
+        return rows.value
 
     # -- sparse -----------------------------------------------------------------------------
     def csr_upload(self, n_rows: int, n_cols: int, indptr: np.ndarray, indices: np.ndarray,

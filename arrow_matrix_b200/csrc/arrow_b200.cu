@@ -71,11 +71,10 @@ struct Csr {
     int *long_first = nullptr;        // device: first slot of each long row (n_long_rows+1)
     bool owns_long = false;
     int long_threshold = 0;
-    // row tiles for the CSR-streaming kernel: {row_begin, row_end, nnz_begin, nnz_end}
-    int4 *tiles = nullptr;
-    int n_tiles = 0;
-    int4 *tiles_big = nullptr;        // TILE_ROWS_BIG / TILE_NNZ_BIG variant for narrow feature tiles
-    int n_tiles_big = 0;
+    // row tiles for the CSR-streaming kernels: {row_begin, row_end, nnz_begin, nnz_end}, one list per TILE_LISTS entry
+    // (every list is empty or none is: each covers every row that is not long)
+    int4 *tiles[4] = {};
+    int n_tiles[4] = {};
     int parent = -1;                  // handle of the block whose indptr / values / tiles this one shares (remapped copy)
     int children = 0;                 // live remapped copies that share this block's arrays
     bool live = false;
@@ -110,6 +109,7 @@ struct arrow_ctx {
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     int sm_count = 132;
+    long long l2_bytes = 50LL << 20;  // cudaDeviceProp::l2CacheSize
     std::string err;
     std::vector<DenseBuf> dense;
     std::vector<Csr> csrs;
@@ -121,6 +121,7 @@ struct arrow_ctx {
     int l2_hints_plain = 3;           // arrow_set_option(ARROW_OPT_L2_HINTS_PLAIN)
     int l2_hints_fused = 0;           // arrow_set_option(ARROW_OPT_L2_HINTS_FUSED)
     int big_tiles = 1;                // arrow_set_option(ARROW_OPT_BIG_TILES): 128-row tiles when k <= 32
+    int tile_rows = 0;                // arrow_set_option(ARROW_OPT_TILE_ROWS): 0 = the L2 budget picks the tile list, else its rows
     int spmm_ctas_per_sm = 0;         // arrow_set_option(ARROW_OPT_SPMM_CTAS_PER_SM): 0 = as many as fit
     int prefetch_plain = 0;           // arrow_set_option(ARROW_OPT_PREFETCH): low nibble = plain launches, high nibble = fused launches;
     int prefetch_fused = 0;           //   0 none, 1 bulk L2 prefetch of the current tile's X rows, 2 of the next tile's (look-ahead)
@@ -232,8 +233,7 @@ void csr_release(Csr &c) {
         cudaFree(c.long_tasks);
         cudaFree(c.long_rows);
         cudaFree(c.long_first);
-        cudaFree(c.tiles);
-        cudaFree(c.tiles_big);
+        for (int4 *p : c.tiles) cudaFree(p);
     }
     c = Csr();
 }
@@ -666,10 +666,20 @@ __global__ void __launch_bounds__(TMA_WARPS * 32) k_spmm_tma(SpmmArgs a) {
 // mbarrier, one tile ahead of the math (two stages).  Warps then only issue the X gathers: a group of
 // G lanes owns a row, reads (col, val) from shared memory (broadcast) and VPL float4 of the X row.
 // ------------------------------------------------------------------------------------------------
-constexpr int TILE_ROWS = 64;       // small tiles keep the rows in flight (grid x TILE_ROWS) inside ~4 blocks => L2 hits
+constexpr int TILE_ROWS = 64;       // bounds of the tiles the TR = 64 kernel instances take
 constexpr int TILE_NNZ = 1024;
 constexpr int TILE_ROWS_BIG = 128;  // k <= 32: the panels are small, bigger tiles amortise the per-tile fixed cost
 constexpr int TILE_NNZ_BIG = 2048;
+// The row-tile lists every CSR carries (Csr::tiles[i]: <= rows, <= nnz entries).  The lists below TILE_LIST_SMALL fit the
+// TR = 64 instances' bounds, so they run on the same kernels; only the window of rows in flight changes (tile_list_for).
+struct TileListCaps { int rows, nnz; };
+constexpr TileListCaps TILE_LISTS[] = {{16, 256}, {32, 512}, {TILE_ROWS, TILE_NNZ}, {TILE_ROWS_BIG, TILE_NNZ_BIG}};
+constexpr int N_TILE_LISTS = 4;
+constexpr int TILE_LIST_SMALL = 2;  // the TILE_ROWS list
+constexpr int TILE_LIST_BIG = 3;    // the TILE_ROWS_BIG list (TR = 128 instances, k <= 32)
+constexpr int TILE_CTAS_PER_SM = 4; // __launch_bounds__(TILE_THREADS, 4) of every tile kernel: the resident CTAs per SM
+constexpr int TILE_L2_WINDOW_DIV = 4;   // the X rows of the window in flight may take 1/4 of the L2 (DESIGN section 3, lesson 2)
+static_assert(sizeof(Csr::tiles) / sizeof(Csr::tiles[0]) == N_TILE_LISTS, "one tile list per TILE_LISTS entry");
 constexpr int TILE_THREADS = 256;
 constexpr int TILE_STAGES = 2;      // CSR slices in shared memory: tile t (math), t+1 (in flight).  A third stage (tried in round 2 for a
                                     // look-ahead prefetch) cost more L1 than it bought: the L1 data array is the landing buffer of the gathers in flight
@@ -2003,6 +2013,27 @@ int launch_tiles_gv(arrow_ctx *ctx, const TileArgs &t, const TileLaunch &L) {
     }
 }
 
+// Which row-tile list a launch walks (an index into TILE_LISTS).  The CTAs share one atomic ticket, so the rows in flight
+// are about resident CTAs x rows per tile, and the X rows those rows gather from must stay in L2 until the last of their
+// ~10 gathers: at k = 128 fp32 on H100, 528 CTAs x 64 rows span 3-4 block-rows whose panels and the head panel take
+// about half of the 50 MB L2.  The rule counts the window's own X rows only (resident CTAs x rows x k x element size)
+// and lets them take 1 / TILE_L2_WINDOW_DIV of the L2, leaving the rest to the block overlap, the head panel and the CSR
+// and C streams; it picks the largest list that fits, never fewer than 16 rows.  The 128-row list needs a TR = 128
+// instance (big_ok: k <= 32 on the fp32 paths).
+int tile_list_rule(int k, int elem_bytes, long long l2_bytes, long long resident_ctas, bool big_ok) {
+    int i = big_ok ? TILE_LIST_BIG : TILE_LIST_SMALL;
+    while (i > 0 && resident_ctas * TILE_LISTS[i].rows * k * elem_bytes > l2_bytes / TILE_L2_WINDOW_DIV) --i;
+    return i;
+}
+
+int tile_list_for(const arrow_ctx *ctx, int k, int elem_bytes, bool big_ok) {
+    for (int i = 0; i < N_TILE_LISTS; ++i)                     // forced by ARROW_OPT_TILE_ROWS
+        if (TILE_LISTS[i].rows == ctx->tile_rows) return (i == TILE_LIST_BIG && !big_ok) ? TILE_LIST_SMALL : i;
+    const int per_sm = ctx->spmm_ctas_per_sm > 0 ? std::min(TILE_CTAS_PER_SM, ctx->spmm_ctas_per_sm) : TILE_CTAS_PER_SM;
+    const int sms = ctx->spmm_sm_limit > 0 ? std::min(ctx->sm_count, ctx->spmm_sm_limit) : ctx->sm_count;
+    return tile_list_rule(k, elem_bytes, ctx->l2_bytes, (long long)per_sm * sms, big_ok && ctx->big_tiles);
+}
+
 // (lanes per row, float4 per lane) for a k4 = k/4; vpl_req = 0 picks the default
 int launch_tiles(arrow_ctx *ctx, TileArgs &t, const Csr *A, const TileLaunch &L) {
     const int k4 = t.a.k4;
@@ -2014,8 +2045,10 @@ int launch_tiles(arrow_ctx *ctx, TileArgs &t, const Csr *A, const TileLaunch &L)
     if (lanes > 32) { vpl = (k4 + 31) / 32 <= 2 ? 2 : 4; lanes = (k4 + vpl - 1) / vpl; }
     int g = 1;
     while (g < lanes) g <<= 1;
-    const bool big = (k4 <= 8) && ctx->big_tiles && A->n_tiles_big > 0;     // k <= 32
-    if (big) { t.tiles = A->tiles_big; t.n_tiles = A->n_tiles_big; }
+    const int list = tile_list_for(ctx, t.a.k, 4, k4 <= 8);                  // k <= 32: TLB / TLP shapes exist
+    const bool big = list == TILE_LIST_BIG;
+    t.tiles = A->tiles[list];
+    t.n_tiles = A->n_tiles[list];
     // one row per lane group unless asked: on H100 at 10M rows pairs lose at k = 32 (1.75 vs 1.67 ms, scripts/kbench.py
     // variants 3 and 259)
     int rpg = L.rpg_req ? L.rpg_req : (ctx->rows_per_group ? ctx->rows_per_group : 1);
@@ -2123,11 +2156,12 @@ int spmm_f64(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool rowmap, bool 
         else LAUNCH_G64((k_spmm_generic_f64<false, false>));
 #undef LAUNCH_G64
         ctx->launches++;
-    } else if (A->n_tiles > 0) {
+    } else if (A->n_tiles[TILE_LIST_SMALL] > 0) {
         TileArgsF64 t;
         t.a = b;
-        t.tiles = A->tiles;
-        t.n_tiles = A->n_tiles;
+        const int list = tile_list_for(ctx, k, 8, false);              // one tile kernel size: TR = 64
+        t.tiles = A->tiles[list];
+        t.n_tiles = A->n_tiles[list];
         t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
         t.ticket = ctx->tile_ticket + 2 * lane;
         t.l2_hints = (rowmap || acc) ? ctx->l2_hints_fused : ctx->l2_hints_plain;
@@ -2527,8 +2561,10 @@ int launch_tiles_sr_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A, bool min_pl
     const int lanes = (k4 + vpl - 1) / vpl;           // <= 16: k4 <= 64
     int g = 1;
     while (g < lanes) g <<= 1;
-    const bool big = (k4 <= 8) && ctx->big_tiles && A->n_tiles_big > 0;     // k <= 32
-    if (big) { t.tiles = A->tiles_big; t.n_tiles = A->n_tiles_big; }
+    const int list = tile_list_for(ctx, t.a.k, 4, k4 <= 8);                  // k <= 32: SRB shapes exist
+    const bool big = list == TILE_LIST_BIG;
+    t.tiles = A->tiles[list];
+    t.n_tiles = A->n_tiles[list];
 #define TSR(GG, VV, TR, TN)                                                                              \
     return min_plus ? launch_tiles_sr_one<GG, VV, SrMinPlus, TR, TN>(ctx, t) : launch_tiles_sr_one<GG, VV, SrMaxPlus, TR, TN>(ctx, t)
 #define SRB(GG, VV) if (big && g == GG && vpl == VV) TSR(GG, VV, TILE_ROWS_BIG, TILE_NNZ_BIG)
@@ -2553,11 +2589,9 @@ int spmm_sr(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool min_plus) {
         const int grid = grid_for(ctx, (const void *)fn, 256, 0, ctas);
         fn<<<grid, 256, 0, stream>>>(a);
         ctx->launches++;
-    } else if (A->n_tiles > 0) {
+    } else if (A->n_tiles[TILE_LIST_SMALL] > 0) {
         TileArgs t;
         t.a = a;
-        t.tiles = A->tiles;
-        t.n_tiles = A->n_tiles;
         t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
         t.ticket = ctx->tile_ticket + 2 * lane;
         t.l2_hints = ctx->l2_hints_plain;
@@ -2967,8 +3001,10 @@ int launch_tiles_wit_shape(arrow_ctx *ctx, WitArgs &w, const Csr *A, bool min_pl
     const int lanes = (k4 + vpl - 1) / vpl;           // <= 32: k4 <= 64
     int g = 1;
     while (g < lanes) g <<= 1;
-    const bool big = (k4 <= 8) && ctx->big_tiles && A->n_tiles_big > 0;
-    if (big) { t.tiles = A->tiles_big; t.n_tiles = A->n_tiles_big; }
+    const int list = tile_list_for(ctx, t.a.k, 4, k4 <= 8);                  // k <= 32: WIB shapes exist
+    const bool big = list == TILE_LIST_BIG;
+    t.tiles = A->tiles[list];
+    t.n_tiles = A->n_tiles[list];
 #define TWI(GG, VV, TR, TN)                                                                              \
     return min_plus ? launch_tiles_wit_one<GG, VV, SrMinPlus, TR, TN>(ctx, w) : launch_tiles_wit_one<GG, VV, SrMaxPlus, TR, TN>(ctx, w)
 #define WIB(GG, VV) if (big && g == GG && vpl == VV) TWI(GG, VV, TILE_ROWS_BIG, TILE_NNZ_BIG)
@@ -2994,9 +3030,7 @@ int spmm_wit(arrow_ctx *ctx, const Csr *A, WitArgs &w, bool min_plus) {
         const int grid = grid_for(ctx, (const void *)fn, 256, 0, ctas);
         fn<<<grid, 256, 0, stream>>>(w);
         ctx->launches++;
-    } else if (A->n_tiles > 0) {
-        w.t.tiles = A->tiles;
-        w.t.n_tiles = A->n_tiles;
+    } else if (A->n_tiles[TILE_LIST_SMALL] > 0) {
         w.t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
         w.t.ticket = ctx->tile_ticket + 2 * lane;
         w.t.l2_hints = ctx->l2_hints_plain;
@@ -3072,6 +3106,7 @@ int arrow_ctx_create(int device, void *stream, arrow_ctx **out) {
         return fail(nullptr, ARROW_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
     }
     ctx->sm_count = prop.multiProcessorCount;
+    if (prop.l2CacheSize > 0) ctx->l2_bytes = prop.l2CacheSize;
     if (stream) {
         ctx->stream = (cudaStream_t)stream;
     } else {
@@ -3175,6 +3210,11 @@ int arrow_set_option(arrow_ctx *ctx, int option, int value) {
         case ARROW_OPT_L2_HINTS_PLAIN: ctx->l2_hints_plain = value & 3; return ARROW_OK;
         case ARROW_OPT_L2_HINTS_FUSED: ctx->l2_hints_fused = value & 3; return ARROW_OK;
         case ARROW_OPT_BIG_TILES: ctx->big_tiles = value ? 1 : 0; return ARROW_OK;
+        case ARROW_OPT_TILE_ROWS:
+            if (value != 0 && value != 16 && value != 32 && value != 64 && value != 128)
+                return fail(ctx, ARROW_ERR_ARG, "tile rows are 0 (automatic), 16, 32, 64 or 128, not %d", value);
+            ctx->tile_rows = value;
+            return ARROW_OK;
         case ARROW_OPT_SPMM_CTAS_PER_SM: ctx->spmm_ctas_per_sm = value < 0 ? 0 : value; return ARROW_OK;
         case ARROW_OPT_PREFETCH: ctx->prefetch_plain = value & 0xF; ctx->prefetch_fused = (value >> 4) & 0xF;
             if (ctx->prefetch_plain > 1 || ctx->prefetch_fused > 1) { ctx->prefetch_plain = ctx->prefetch_fused = 0; return fail(ctx, ARROW_ERR_ARG, "prefetch modes are 0..1 per nibble"); }
@@ -3189,6 +3229,19 @@ int arrow_set_option(arrow_ctx *ctx, int option, int value) {
         case ARROW_OPT_BARRIER_TIMEOUT_MS: ctx->barrier_timeout_ms = value < 1 ? 1 : value; return ARROW_OK;
         default: return fail(ctx, ARROW_ERR_ARG, "unknown option %d", option);
     }
+}
+
+int arrow_tile_rows_rule(int k, int elem_bytes, int64_t l2_bytes, int resident_ctas, int big_ok) {
+    if (k < 1 || (elem_bytes != 4 && elem_bytes != 8) || l2_bytes < 1 || resident_ctas < 1) return ARROW_ERR_ARG;
+    return TILE_LISTS[tile_list_rule(k, elem_bytes, l2_bytes, resident_ctas, big_ok != 0)].rows;
+}
+
+int arrow_tile_rows(arrow_ctx *ctx, int k, int dtype, int *rows) {
+    CHECK_CTX(ctx);
+    if (!rows || k < 1 || (dtype != ARROW_F32 && dtype != ARROW_F64)) return fail(ctx, ARROW_ERR_ARG, "bad tile-rows query");
+    const bool f64 = dtype == ARROW_F64;
+    *rows = TILE_LISTS[tile_list_for(ctx, k, f64 ? 8 : 4, !f64 && k <= 32)].rows;
+    return ARROW_OK;
 }
 
 // ---- sparse -------------------------------------------------------------------------------------
@@ -3223,7 +3276,7 @@ static int build_long_rows(arrow_ctx *ctx, Csr &c, const std::vector<int> &h_ind
                 if (h_indptr[e + 1] - h_indptr[r] > nnz_cap - 4 && e > r) break;
                 ++e;
             }
-            if (e == r) ++e;                                       // a single row always fits: thr <= TILE_NNZ - 8
+            if (e == r) ++e;                                       // a single row may pass nnz_cap but fits the kernels: thr <= TILE_NNZ - 8
             tiles.push_back(make_int4((int)r, (int)e, h_indptr[r], h_indptr[e]));
             r = e;
         }
@@ -3234,10 +3287,8 @@ static int build_long_rows(arrow_ctx *ctx, Csr &c, const std::vector<int> &h_ind
         }
         return ARROW_OK;
     };
-    {
-        int rc = build_tiles(TILE_ROWS, TILE_NNZ, &c.tiles, &c.n_tiles);
-        if (rc != ARROW_OK) return rc;
-        rc = build_tiles(TILE_ROWS_BIG, TILE_NNZ_BIG, &c.tiles_big, &c.n_tiles_big);
+    for (int i = 0; i < N_TILE_LISTS; ++i) {
+        const int rc = build_tiles(TILE_LISTS[i].rows, TILE_LISTS[i].nnz, &c.tiles[i], &c.n_tiles[i]);
         if (rc != ARROW_OK) return rc;
     }
     c.max_row_nnz = mx;
@@ -3857,11 +3908,9 @@ static int spmm_impl(arrow_ctx *ctx, const SpmmCall &q) {
 #undef LAUNCH_G
         ctx->launches++;
     } else if (variant == 3) {
-        if (A->n_tiles > 0) {
+        if (A->n_tiles[TILE_LIST_SMALL] > 0) {
             TileArgs t;
             t.a = a;
-            t.tiles = A->tiles;
-            t.n_tiles = A->n_tiles;
             t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
             t.ticket = ctx->tile_ticket + 2 * lane;
             t.l2_hints = (rm != nullptr || acc) ? ctx->l2_hints_fused : ctx->l2_hints_plain;

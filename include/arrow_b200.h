@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 5
+#define ARROW_ABI_VERSION 6
 
 /* error codes */
 #define ARROW_OK              0
@@ -79,7 +79,7 @@ int  arrow_set_tuning(arrow_ctx *ctx, int long_row_threshold, int long_row_segme
  * evict_first; PLAIN applies to C = A X launches, FUSED to launches with a row map or ARROW_ACCUMULATE. */
 #define ARROW_OPT_L2_HINTS_PLAIN 1
 #define ARROW_OPT_L2_HINTS_FUSED 2
-#define ARROW_OPT_BIG_TILES      3   /* 1 (default): 128-row / 2048-entry CSR tiles when k <= 32 */
+#define ARROW_OPT_BIG_TILES      3   /* 1 (default): 128-row / 2048-entry CSR tiles may be picked when k <= 32 (see ARROW_OPT_TILE_ROWS) */
 #define ARROW_OPT_PREFETCH        5   /* bulk L2 prefetch (cp.async.bulk.prefetch.L2, one request per X row) of a CSR tile's X rows
                                         before its math: bit 0 = plain launches, bit 4 = fused launches (row map / accumulate /
                                         gather-add / dual X / row pointers).  Measured as a loss;
@@ -97,7 +97,16 @@ int  arrow_set_tuning(arrow_ctx *ctx, int long_row_threshold, int long_row_segme
 #define ARROW_OPT_PUSH_INTERLEAVE 13   /* 1 (default): arrow_push_rows walks its destination blocks interleaved (every peer is written to at
                                         every instant); 0: block after block */
 #define ARROW_OPT_BARRIER_TIMEOUT_MS 9 /* arrow_peer_barrier gives up after this long (default 30000) and poisons the context */
+#define ARROW_OPT_TILE_ROWS      14   /* CSR row tiles the tile kernels walk: 0 (default) = picked per launch from the L2 size (arrow_tile_rows),
+                                         16 / 32 / 64 / 128 = that list (128 only where k <= 32 on float32, else 64).  Results are
+                                         bit-identical for every value: only the rows in flight change */
 int  arrow_set_option(arrow_ctx *ctx, int option, int value);
+/* Rows per CSR tile of the tile-kernel launches at feature width k and element type dtype (ARROW_F32 / ARROW_F64) under the
+ * context's options and device.  The automatic rule: the largest of 128 (float32, k <= 32, ARROW_OPT_BIG_TILES on) / 64 / 32 / 16
+ * rows for which resident CTAs x rows x k x element bytes <= L2 size / 4 (the X rows of the window in flight stay in L2), else 16.
+ * arrow_tile_rows_rule evaluates that rule for given values without a context or device (a negative value: bad arguments). */
+int  arrow_tile_rows(arrow_ctx *ctx, int k, int dtype, int *rows);
+int  arrow_tile_rows_rule(int k, int elem_bytes, int64_t l2_bytes, int resident_ctas, int big_ok);
 
 /* ---- sparse blocks (replaces _sp2cp, sp2cp.py:6-16: uploaded once, resident) ----------------- */
 /* indptr has n_rows+1 entries of indptr_bytes (4 or 8) each and may start at any base value
