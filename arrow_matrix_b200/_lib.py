@@ -19,12 +19,14 @@ LIB_PATH = os.path.join(_HERE, "libarrow_b200.so")
 ACCUMULATE = 1
 F32, F64 = 0, 1                       # ARROW_F32 / ARROW_F64: element type of dense tiles and CSR values
 I32 = 2                               # ARROW_I32: dense tiles of labels / parents (arrow_spmm_sr_witness)
+B1 = 3                                # ARROW_B1: bit tiles of the (or, and) semiring; host rows are b1_words(k) uint32 words
+BITS = "bits"                         # ``dense_alloc(..., dtype=BITS)``: a bit tile; its host rows are uint32 words
 _DTYPE_CODE = {np.dtype(np.float32): F32, np.dtype(np.float64): F64}
 _TILE_CODE = {**_DTYPE_CODE, np.dtype(np.int32): I32}
-_CODE_TILE = {c: dt for dt, c in _TILE_CODE.items()}
+_CODE_TILE = {**{c: dt for dt, c in _TILE_CODE.items()}, B1: BITS}
 VARIANT_AUTO, VARIANT_DIRECT, VARIANT_SHFL, VARIANT_TMA, VARIANT_TILES = -1, 0, 1, 2, 3
-SR_PLUS_TIMES, SR_MIN_PLUS, SR_MAX_PLUS = 0, 1, 2     # ARROW_SR_*: the semiring of arrow_spmm_sr / arrow_gather_rows_sr
-SEMIRINGS = {"plus_times": SR_PLUS_TIMES, "min_plus": SR_MIN_PLUS, "max_plus": SR_MAX_PLUS}
+SR_PLUS_TIMES, SR_MIN_PLUS, SR_MAX_PLUS, SR_OR_AND = 0, 1, 2, 3   # ARROW_SR_*: the semiring of arrow_spmm_sr / arrow_gather_rows_sr
+SEMIRINGS = {"plus_times": SR_PLUS_TIMES, "min_plus": SR_MIN_PLUS, "max_plus": SR_MAX_PLUS, "or_and": SR_OR_AND}
 IPC_HANDLE_BYTES = 80
 
 EXPORTS = [
@@ -44,9 +46,9 @@ EXPORTS = [
     "arrow_host_alloc_numa", "arrow_bind_thread_to_device_numa", "arrow_preload_kernels",
     "arrow_csr_upload_f64", "arrow_dense_alloc_dtype", "arrow_dense_dtype",
     "arrow_spmm_sr", "arrow_gather_rows_sr", "arrow_dense_count_diff",
-    "arrow_spmm_sr_witness", "arrow_tile_rows", "arrow_tile_rows_rule",
+    "arrow_spmm_sr_witness", "arrow_tile_rows", "arrow_tile_rows_rule", "arrow_bits_mark_new",
 ]
-ABI_VERSION = 6         # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 7         # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -147,6 +149,7 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_spmm_sr_witness": (c_int, [P, I, I, I, I, I, I, I, I, I, I]),
         "arrow_tile_rows": (c_int, [P, I, I, pI]),
         "arrow_tile_rows_rule": (c_int, [I, I, I64, I, I]),
+        "arrow_bits_mark_new": (c_int, [P, I, I, I, I, pI64]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -158,6 +161,33 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
 
 def _ptr(a: Optional[np.ndarray]) -> c_void_p:
     return c_void_p(None) if a is None else c_void_p(a.ctypes.data)
+
+
+def b1_words(k: int) -> int:
+    """uint32 words per row of a bit tile of ``k`` columns: one bit per column; one word for k <= 32, else padded to a
+    multiple of 4 words"""
+    return 1 if int(k) <= 32 else ((int(k) + 31) // 32 + 3) & ~3
+
+
+def pack_bits(X: np.ndarray) -> np.ndarray:
+    """bool (or any: non-zero is true) [n x k] -> uint32 [n x b1_words(k)]: column c is bit c % 32 of word c // 32,
+    padding bits are zero"""
+    X = np.asarray(X)
+    if X.ndim != 2:
+        raise ValueError(f"expected a 2-d array, got shape {X.shape}")
+    n, k = X.shape
+    by = np.packbits(X != 0, axis=1, bitorder="little")
+    out = np.zeros((n, b1_words(k) * 4), dtype=np.uint8)
+    out[:, :by.shape[1]] = by
+    return out.view("<u4").astype(np.uint32, copy=False)
+
+
+def unpack_bits(words: np.ndarray, k: int) -> np.ndarray:
+    """uint32 [n x w] words -> bool [n x k] (the inverse of ``pack_bits``; padding bits are ignored)"""
+    words = np.ascontiguousarray(words, dtype="<u4")
+    if words.ndim != 2 or words.shape[1] * 32 < k:
+        raise ValueError(f"{words.shape} words cannot hold {k} columns")
+    return np.unpackbits(words.view(np.uint8), axis=1, count=int(k), bitorder="little").astype(bool)
 
 
 def element_type(dtype) -> np.dtype:
@@ -304,7 +334,13 @@ class Context:
 
     # -- dense ------------------------------------------------------------------------------
     def dense_alloc(self, rows: int, k: int, dtype=np.float32) -> "Dense":
-        """a zero-filled tile of float32 / float64 features or of int32 labels (``arrow_spmm_sr_witness``)"""
+        """a zero-filled tile of float32 / float64 features, of int32 labels (``arrow_spmm_sr_witness``) or, with
+        ``dtype=BITS``, of ``k`` bit columns (``ARROW_B1``: host rows of ``b1_words(k)`` uint32 words; ``np.uint32``
+        itself is not a tile type)"""
+        if isinstance(dtype, str) and dtype == BITS:
+            h = c_int()
+            self._check(self.lib.arrow_dense_alloc_dtype(self._h, int(rows), int(k), B1, byref(h)))
+            return Dense(self, h.value, int(rows), int(k), owned=True, dtype=BITS)
         dtype = np.dtype(np.int32) if np.dtype(dtype) == np.int32 else element_type(dtype)
         h = c_int()
         if dtype == np.float32:
@@ -415,6 +451,13 @@ class Context:
         """dst[r] = dst[r] ⊕ src[m[r]] where m[r] >= 0 (``arrow_gather_rows_sr``)"""
         self._check(self.lib.arrow_gather_rows_sr(self._h, dst.h, src.h, m.h, int(semiring)))
 
+    def bits_mark_new(self, new: "Dense", old: "Dense", dist: "Dense", level: int) -> int:
+        """dist[r, c] = level where the bit (r, c) is set in ``new`` and clear in ``old`` (``arrow_bits_mark_new``); returns
+        the number of such bits; synchronises"""
+        n = c_int64()
+        self._check(self.lib.arrow_bits_mark_new(self._h, new.h, old.h, dist.h, int(level), byref(n)))
+        return int(n.value)
+
     def count_diff(self, a: "Dense", b: "Dense") -> int:
         """rows in which two equally shaped tiles differ in some element (-0 == +0, NaN != NaN); synchronises"""
         n = c_int64()
@@ -437,11 +480,11 @@ class Context:
     LANE_MAIN, LANE_H2D, LANE_D2H = 0, 1, 2
 
     def h2d_lane(self, lane: int, dst: "Dense", X: np.ndarray, row0: int = 0):
-        assert X.dtype == dst.dtype and X.flags.c_contiguous and X.shape[1] == dst.k
+        assert X.dtype == dst.dtype and X.flags.c_contiguous and X.shape[1] == dst.cols
         self._check(self.lib.arrow_dense_h2d_lane(self._h, lane, dst.h, int(row0), X.shape[0], _ptr(X)))
 
     def d2h_lane(self, lane: int, src: "Dense", out: np.ndarray, row0: int = 0):
-        assert out.dtype == src.dtype and out.flags.c_contiguous and out.shape[1] == src.k
+        assert out.dtype == src.dtype and out.flags.c_contiguous and out.shape[1] == src.cols
         self._check(self.lib.arrow_dense_d2h_lane(self._h, lane, src.h, int(row0), out.shape[0], _ptr(out)))
 
     def lane_wait(self, waiting_lane: int, signalling_lane: int):
@@ -549,10 +592,12 @@ class Dense(_Handle):
     def __init__(self, ctx, h, rows, k, owned, dtype=np.float32):
         super().__init__(ctx, h)
         self.rows, self.k, self.owned = rows, k, owned
-        self.dtype = np.dtype(dtype)
+        self.bits = isinstance(dtype, str) and dtype == BITS
+        self.dtype = np.dtype(np.uint32) if self.bits else np.dtype(dtype)       # host element type (words of a bit tile)
+        self.cols = b1_words(k) if self.bits else k                              # host elements per row
 
     def device_dtype(self) -> np.dtype:
-        """the element type the library holds for this tile (``arrow_dense_dtype``)"""
+        """the element type the library holds for this tile (``arrow_dense_dtype``; ``BITS`` for a bit tile)"""
         code = c_int()
         self.ctx._check(self.ctx.lib.arrow_dense_dtype(self.ctx._h, self.h, byref(code)))
         return _CODE_TILE[code.value]
@@ -560,16 +605,16 @@ class Dense(_Handle):
     def h2d(self, X: np.ndarray, row0: int = 0):
         """upload rows, converted to the tile's element type"""
         X = np.ascontiguousarray(X, dtype=self.dtype)
-        if X.ndim != 2 or X.shape[1] != self.k:
-            raise ValueError(f"expected [rows x {self.k}] {self.dtype}, got {X.shape}")
+        if X.ndim != 2 or X.shape[1] != self.cols:
+            raise ValueError(f"expected [rows x {self.cols}] {self.dtype}, got {X.shape}")
         self.ctx._check(self.ctx.lib.arrow_dense_h2d(self.ctx._h, self.h, int(row0), X.shape[0], _ptr(X)))
         self._keep = X                  # async copy: keep the host array alive until the next sync
 
     def d2h(self, out: Optional[np.ndarray] = None, row0: int = 0, rows: Optional[int] = None, sync: bool = True) -> np.ndarray:
         rows = self.rows - row0 if rows is None else rows
         if out is None:
-            out = np.empty((rows, self.k), dtype=self.dtype)
-        assert out.dtype == self.dtype and out.flags.c_contiguous and out.shape == (rows, self.k)
+            out = np.empty((rows, self.cols), dtype=self.dtype)
+        assert out.dtype == self.dtype and out.flags.c_contiguous and out.shape == (rows, self.cols)
         self.ctx._check(self.ctx.lib.arrow_dense_d2h(self.ctx._h, self.h, int(row0), int(rows), _ptr(out)))
         if sync:
             self.ctx.sync()

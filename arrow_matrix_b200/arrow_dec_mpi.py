@@ -76,8 +76,9 @@ class ArrowDecompositionMPI:
         """Same arguments as the reference (``:106-115``).  ``slim`` only selects the reference's rank
         layout; on a GPU both layouts are the same row-partitioned kernels, so it is accepted and ignored.
         Extensions (one GPU): ``semiring`` -- ``"plus_times"`` (the reference's product), ``"min_plus"`` or
-        ``"max_plus"`` (float32) -- and ``add_identity``, which makes a step compute ``X ⊕ (A ⊗ X)`` (see
-        ``engine.py``)."""
+        ``"max_plus"`` (float32), or ``"or_and"`` (bit features: ``set_features`` takes booleans, non-zero is true, and
+        ``result_tile()`` returns booleans; with ``add_identity`` a step is one hop of multi-source BFS, see
+        ``bfs_levels``) -- and ``add_identity``, which makes a step compute ``X ⊕ (A ⊗ X)`` (see ``engine.py``)."""
         assert not slim or block_diagonal
         assert np.sum(n_blocks) > 0
         def level_operator(owner, j):           # the reference hands out ArrowSlimMPI or ArrowMPI (``:166-197``)
@@ -166,6 +167,15 @@ class ArrowDecompositionMPI:
         if not isinstance(eng, ArrowEngine):
             raise ValueError("predecessors run on one GPU only")
         return eng.predecessors(out)
+
+    def bfs_levels(self, max_steps: int, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension (one GPU, ``or_and`` with ``add_identity``): hop levels of a multi-source BFS from the current
+        level-0 features, int32 in ``result_tile()`` row order, ``-1`` where never reached (see
+        ``ArrowEngine.bfs_levels``)."""
+        eng = self._require_engine()
+        if not isinstance(eng, ArrowEngine):
+            raise ValueError("bfs_levels runs on one GPU only")
+        return eng.bfs_levels(max_steps, out)
 
     def synchronize(self):
         self._require_engine().sync()

@@ -57,7 +57,11 @@ class ArrowSlimMPI(ArrowMatrix):
         assert X is not None
         if self._level != 0:
             raise ValueError("features enter at level 0; deeper levels receive them through the exchange")
-        self._engine.set_features(np.ascontiguousarray(X, dtype=_engine_dtype(self._engine)))
+        eng = self._engine
+        if getattr(eng, "bits", False):          # or_and: booleans, packed to bits by the engine (non-zero is true)
+            eng.set_features(np.asarray(X))
+        else:
+            eng.set_features(np.ascontiguousarray(X, dtype=_engine_dtype(eng)))
 
     def load_sparse_matrix_from_blocks(self, blocks) -> None:
         """``blocks`` is what ``ArrowDecompositionMPI.load_decomposition_new`` returned."""

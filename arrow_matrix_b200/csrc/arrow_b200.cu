@@ -214,15 +214,28 @@ IdxMap *get_map(arrow_ctx *ctx, int h) {
 inline int ceil_div_i64(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
 inline size_t dtype_size(int dtype) { return dtype == ARROW_F64 ? 8 : 4; }
-inline const char *dtype_name(int dtype) { return dtype == ARROW_F64 ? "float64" : (dtype == ARROW_I32 ? "int32" : "float32"); }
+inline const char *dtype_name(int dtype) {
+    return dtype == ARROW_F64 ? "float64" : (dtype == ARROW_I32 ? "int32" : (dtype == ARROW_B1 ? "bits" : "float32"));
+}
 // int32 tiles hold labels (arrow_spmm_sr_witness): only the allocation, copies and that launch accept them
 #define REFUSE_I32(ctx, d, what)                                                                                   \
     do {                                                                                                           \
         if ((d) != nullptr && (d)->dtype == ARROW_I32)                                                             \
             return fail((ctx), ARROW_ERR_ARG, "%s: int32 tiles hold labels, no arithmetic runs on them", (what));  \
     } while (0)
+// bit tiles run the (or, and) launches of one GPU only
+#define REFUSE_B1(ctx, d, what)                                                                                    \
+    do {                                                                                                           \
+        if ((d) != nullptr && (d)->dtype == ARROW_B1)                                                              \
+            return fail((ctx), ARROW_ERR_ARG, "%s: bit tiles run the (or, and) launches of one GPU only", (what)); \
+    } while (0)
+// uint32 words per row of a bit tile: one bit per column; a row of k <= 32 columns is one word (its own kernel instances,
+// 4-byte gathers: measured faster than a padded 16-byte row, DESIGN.md section 2), wider rows are padded to a multiple of
+// 4 words so that they are whole 16-byte vectors (the uint4 gathers of the bit kernels)
+inline int bit_row_words(int k) { return k <= 32 ? 1 : (((k + 31) / 32) + 3) & ~3; }
+inline size_t row_bytes(int dtype, int k) { return dtype == ARROW_B1 ? (size_t)bit_row_words(k) * 4 : (size_t)k * dtype_size(dtype); }
 // first byte of row `r` of a dense tile
-inline char *dense_row(const DenseBuf *d, int64_t r) { return (char *)d->p + (size_t)r * d->k * dtype_size(d->dtype); }
+inline char *dense_row(const DenseBuf *d, int64_t r) { return (char *)d->p + (size_t)r * row_bytes(d->dtype, d->k); }
 
 // frees whatever device arrays the block owns (cudaFree waits for the device, so no launch can still read them)
 void csr_release(Csr &c) {
@@ -520,6 +533,26 @@ __device__ __forceinline__ float4 ld_f4_hint(const float4 *ptr, uint64_t pol) { 
 __device__ __forceinline__ void st_f4_hint(float4 *ptr, const float4 &v, uint64_t pol) {
     asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(ptr), "f"(v.x), "f"(v.y), "f"(v.z),
                  "f"(v.w), "l"(pol)
+                 : "memory");
+}
+// the same three accesses on 16 bytes of bits (ARROW_B1 tiles), and on the 4 bytes of a one-word bit row further below
+__device__ __forceinline__ uint4 ldg_u4_hint(const uint4 *ptr, uint64_t pol) {
+    uint4 r;
+    asm("ld.global.nc.L2::cache_hint.v4.b32 {%0,%1,%2,%3}, [%4], %5;"
+        : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+        : "l"(ptr), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ uint4 ld_u4_hint(const uint4 *ptr, uint64_t pol) {
+    uint4 r;
+    asm("ld.global.L2::cache_hint.v4.b32 {%0,%1,%2,%3}, [%4], %5;"
+        : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+        : "l"(ptr), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ void st_u4_hint(uint4 *ptr, const uint4 &v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(ptr), "r"(v.x), "r"(v.y), "r"(v.z),
+                 "r"(v.w), "l"(pol)
                  : "memory");
 }
 __device__ __forceinline__ void bulk_g2s_hint(void *dst_smem, const void *src_gmem, uint32_t bytes, uint64_t *bar,
@@ -2672,6 +2705,441 @@ int gather_rows_sr(arrow_ctx *ctx, DenseBuf *D, const DenseBuf *S, const IdxMap 
 }
 
 // ------------------------------------------------------------------------------------------------
+// the boolean semiring (or, and) on bit tiles (ARROW_B1, one GPU): C[r] = (OR_p X[col_p]) | add[add_map[r]].  ⊗ is "the
+// entry exists", so the CSR values are never read (the CSR stage copy carries row pointers and column indices only); ⊕ is
+// OR.  A row of k columns is bit_row_words(k) uint32 words, a multiple of 4: the fp32 tile pipeline with k4 = words / 4
+// uint4 per row.  OR is exact, associative, commutative and idempotent: every kernel, grid and tile list gives the same bits.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void u4_or(uint4 &acc, const uint4 &x) {
+    acc.x |= x.x; acc.y |= x.y; acc.z |= x.z; acc.w |= x.w;
+}
+__device__ __forceinline__ uint4 u4_zero() { return make_uint4(0u, 0u, 0u, 0u); }
+__device__ __forceinline__ void u4_or(unsigned &acc, const unsigned &x) { acc |= x; }        // one-word rows
+template <class V> __device__ __forceinline__ V v_zero();
+template <> __device__ __forceinline__ uint4 v_zero<uint4>() { return make_uint4(0u, 0u, 0u, 0u); }
+template <> __device__ __forceinline__ unsigned v_zero<unsigned>() { return 0u; }
+__device__ __forceinline__ unsigned ldg_u4_hint(const unsigned *ptr, uint64_t pol) {
+    unsigned r;
+    asm("ld.global.nc.L2::cache_hint.b32 %0, [%1], %2;" : "=r"(r) : "l"(ptr), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ unsigned ld_u4_hint(const unsigned *ptr, uint64_t pol) {
+    unsigned r;
+    asm("ld.global.L2::cache_hint.b32 %0, [%1], %2;" : "=r"(r) : "l"(ptr), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ void st_u4_hint(unsigned *ptr, const unsigned &v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(ptr), "r"(v), "l"(pol) : "memory");
+}
+
+template <int TR, int TN>
+struct TileCfgBits {                                   // TileCfg without the values stream
+    static constexpr int PTR_WORDS = TileCfg<TR, TN>::PTR_WORDS;
+    static constexpr int NNZ_WORDS = TileCfg<TR, TN>::NNZ_WORDS;
+    static constexpr int STAGE_WORDS = PTR_WORDS + NNZ_WORDS;
+    static constexpr size_t SMEM_BYTES = (size_t)TILE_STAGES * STAGE_WORDS * 4 + 64;
+};
+
+// G lanes own a row, VPL vectors V each (uint4; one uint32 for the one-word rows of k <= 32).  Splitting a row's entries over S groups of G lanes (OR-reduced with shuffles) was
+// measured slower for every S > 1 (DESIGN.md section 3), so one lane group walks all of a row's entries.
+template <int G, int VPL, int TR, int TN, class V = uint4>
+__global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles_bits(TileArgs t) {
+    constexpr int TILE_PTR_WORDS = TileCfgBits<TR, TN>::PTR_WORDS;
+    constexpr int TILE_STAGE_WORDS = TileCfgBits<TR, TN>::STAGE_WORDS;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    int *stage_base = reinterpret_cast<int *>(smem_raw);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)TILE_STAGES * TILE_STAGE_WORDS * 4);
+    const SpmmArgs &a = t.a;
+    constexpr int RPW = 32 / G;
+    constexpr int UNROLL = (VPL == 2) ? 4 : 8;
+    constexpr int TAIL = UNROLL / 2;                              // predicated tail batches
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const bool EXACT = (t.a.k4 == G * VPL);                       // every lane owns valid columns
+    const int gc = lane % G;                                      // the lane's first V of the row
+    const int gi = lane / G;
+    const int k4 = a.k4;
+    const uint64_t pol_keep = (t.l2_hints & 1) ? l2_policy_evict_last() : l2_policy_evict_normal();
+    const uint64_t pol_stream = (t.l2_hints & 2) ? l2_policy_evict_first() : l2_policy_evict_normal();
+
+    if (threadIdx.x == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    auto issue_csr = [&](int tile, int st) {
+        const int4 d = __ldg(t.tiles + tile);
+        const int rb4 = d.x & ~3;
+        const int a0 = d.z & ~3;
+        const uint32_t ptr_bytes = (uint32_t)(((d.y - rb4 + 1) + 3) & ~3) * 4u;
+        const uint32_t nnz_bytes = (uint32_t)(((d.w - a0) + 3) & ~3) * 4u;
+        int *sp = stage_base + (size_t)st * TILE_STAGE_WORDS;
+        mbar_expect_tx(&bars[st], ptr_bytes + nnz_bytes);     // no values stream
+        bulk_g2s_hint(sp, a.indptr + rb4, ptr_bytes, &bars[st], pol_stream);
+        if (nnz_bytes) bulk_g2s_hint(sp + TILE_PTR_WORDS, a.indices + a0, nnz_bytes, &bars[st], pol_stream);
+    };
+
+    __shared__ int s_next[TILE_STAGES];
+    int tile = blockIdx.x;
+    if (tile < t.n_tiles && threadIdx.x == 0) issue_csr(tile, 0);
+    for (unsigned int n = 0; tile < t.n_tiles; ++n) {
+        const int st = (int)(n & 1u);
+        if (threadIdx.x == 0) {
+            const int next = atomicAdd(t.ticket, 1) + (int)gridDim.x;
+            s_next[st] = next;
+            if (next < t.n_tiles) issue_csr(next, st ^ 1);
+        }
+        const int4 d = __ldg(t.tiles + tile);
+        mbar_wait(&bars[st], (n >> 1) & 1u);
+        const int *sp = stage_base + (size_t)st * TILE_STAGE_WORDS;
+        const int *s_ptr = sp + (d.x - (d.x & ~3));
+        const int a0 = d.z & ~3;
+        const int *s_idx = sp + TILE_PTR_WORDS - a0;                    // index with global nnz offsets
+        const int n_rows_tile = d.y - d.x;
+
+        for (int lr = warp * RPW + gi; lr < n_rows_tile; lr += (TILE_THREADS / 32) * RPW) {
+            const int s = s_ptr[lr];
+            const int e = s_ptr[lr + 1];
+            if (e - s > a.long_threshold) continue;
+            const long long row = (long long)d.x + lr;
+            V acc[VPL];
+#pragma unroll
+            for (int i = 0; i < VPL; ++i) acc[i] = v_zero<V>();
+            if (a.add_map != nullptr) {
+                const int am = __ldg(a.add_map + row);
+                if (am >= 0) {
+                    const V *ar = reinterpret_cast<const V *>(a.add_src) + (long long)am * k4 + gc;
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i)
+                        if (gc + i * G < k4) acc[i] = ld_u4_hint(ar + i * G, pol_stream);
+                }
+            }
+            int p = s;
+            if (EXACT && !t.skip) {
+                // unpredicated batches: full UNROLL batches, then the remainder as 4 / 2 / 1
+                auto batch = [&](auto n_tag) {
+                    constexpr int N = decltype(n_tag)::value;
+                    V x[N][VPL];
+#pragma unroll
+                    for (int u = 0; u < N; ++u) {
+                        const V *xr = reinterpret_cast<const V *>(a.X) + (long long)s_idx[p + u] * k4 + gc;
+#pragma unroll
+                        for (int i = 0; i < VPL; ++i) x[u][i] = ldg_u4_hint(xr + i * G, pol_keep);
+                    }
+#pragma unroll
+                    for (int u = 0; u < N; ++u)
+#pragma unroll
+                        for (int i = 0; i < VPL; ++i) u4_or(acc[i], x[u][i]);
+                    p += N;
+                };
+                while (p + UNROLL <= e) batch(std::integral_constant<int, UNROLL>{});
+                if constexpr (UNROLL >= 8) { if (e - p >= 4) batch(std::integral_constant<int, 4>{}); }
+                if (e - p >= 2) batch(std::integral_constant<int, 2>{});
+                if (e - p >= 1) batch(std::integral_constant<int, 1>{});
+            }
+            // tail (and the general case): predicated batches; a skipped entry (column -1) or a slot past the row's end
+            // ORs zeros
+            for (; p < e; p += TAIL) {
+                V x[TAIL][VPL];
+#pragma unroll
+                for (int u = 0; u < TAIL; ++u) {
+                    const int c = (p + u < e) ? s_idx[p + u] : -1;
+                    const V *xr = reinterpret_cast<const V *>(a.X) + (long long)c * k4 + gc;   // c = -1: address arithmetic only
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i)
+                        x[u][i] = (c >= 0 && gc + i * G < k4) ? ldg_u4_hint(xr + i * G, pol_keep) : v_zero<V>();
+                }
+#pragma unroll
+                for (int u = 0; u < TAIL; ++u)
+#pragma unroll
+                    for (int i = 0; i < VPL; ++i) u4_or(acc[i], x[u][i]);
+            }
+            V *cr = reinterpret_cast<V *>(a.C) + row * k4 + gc;
+#pragma unroll
+            for (int i = 0; i < VPL; ++i)
+                if (gc + i * G < k4) st_u4_hint(cr + i * G, acc[i], pol_stream);
+        }
+        __syncthreads();            // stage `st` may be refilled by the next iteration's copy
+        tile = s_next[st];
+    }
+}
+
+// long rows: one CTA per segment ORs its entries' X rows into a scratch slot (warps over entries, lanes over words), then
+// one CTA per row ORs the slots and the addend (k_spmm_long_partial / k_spmm_long_reduce on words)
+__global__ void __launch_bounds__(256) k_spmm_long_partial_bits(LongArgs a) {
+    extern __shared__ unsigned int red_bits[];   // [warps][words]
+    const LongTask t = a.tasks[blockIdx.x];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    const int words = a.k;                        // a.k carries the row's words here
+    const unsigned int *X = reinterpret_cast<const unsigned int *>(a.X);
+    for (int c0 = 0; c0 < words; c0 += 128) {
+        unsigned int acc[4] = {0u, 0u, 0u, 0u};
+        for (int p = t.begin + warp; p < t.end; p += nwarps) {
+            const int c = __ldg(a.indices + p);
+            if (c < 0) continue;
+            const unsigned int *xr = X + (long long)c * words;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int w = c0 + lane + 32 * i;
+                if (w < words) acc[i] |= __ldg(xr + w);
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int w = c0 + lane + 32 * i;
+            if (w < words) red_bits[warp * words + w] = acc[i];
+        }
+    }
+    __syncthreads();
+    unsigned int *scratch = reinterpret_cast<unsigned int *>(a.scratch);
+    for (int w = threadIdx.x; w < words; w += blockDim.x) {
+        unsigned int r = 0u;
+        for (int q = 0; q < nwarps; ++q) r |= red_bits[q * words + w];
+        scratch[(long long)t.slot * words + w] = r;
+    }
+}
+
+__global__ void __launch_bounds__(128) k_spmm_long_reduce_bits(const int *__restrict__ long_rows,
+                                                               const int *__restrict__ long_first,
+                                                               const unsigned int *__restrict__ scratch,
+                                                               unsigned int *__restrict__ C, int words,
+                                                               const unsigned int *__restrict__ add_src,
+                                                               const int *__restrict__ add_map) {
+    const int r = long_rows[blockIdx.x];
+    unsigned int *crow = C + (long long)r * words;
+    const int am = (add_map != nullptr) ? add_map[r] : -1;
+    const int s0 = long_first[blockIdx.x], s1 = long_first[blockIdx.x + 1];
+    for (int w = threadIdx.x; w < words; w += blockDim.x) {
+        unsigned int acc = 0u;
+        for (int s = s0; s < s1; ++s) acc |= scratch[(long long)s * words + w];
+        if (am >= 0) acc |= add_src[(long long)am * words + w];
+        crow[w] = acc;
+    }
+}
+
+// dst[r] |= src[map[r]] (map[r] >= 0): the backward exchange of an (or, and) step; a lane group of G lanes per row,
+// whole uint4 of the padded rows
+template <int G>
+__global__ void __launch_bounds__(256) k_gather_rows_or(uint4 *__restrict__ dst, const uint4 *__restrict__ src,
+                                                        const int *__restrict__ map, long long n_rows, int vec_per_row) {
+    constexpr int RPW = 32 / G;
+    const int lane = threadIdx.x & 31;
+    const int gl = lane % G, gi = lane / G;
+    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
+    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    for (long long r = warp_id * RPW + gi; r < n_rows; r += warps_total * RPW) {
+        const int m = __ldg(map + r);
+        if (m < 0) continue;
+        const uint4 *sp = src + (long long)m * vec_per_row;
+        uint4 *dp = dst + r * vec_per_row;
+        for (int v = gl; v < vec_per_row; v += G) {
+            uint4 x = sp[v];
+            u4_or(x, dp[v]);
+            dp[v] = x;
+        }
+    }
+}
+
+// dst[r] |= src[map[r]] on one-word rows
+__global__ void __launch_bounds__(256) k_gather_rows_or_word(unsigned *__restrict__ dst, const unsigned *__restrict__ src,
+                                                             const int *__restrict__ map, long long n) {
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (long long)gridDim.x * blockDim.x) {
+        const int m = __ldg(map + r);
+        if (m >= 0) dst[r] |= src[m];
+    }
+}
+
+// bits of the k columns of word w of a row (the padding bits of the last word and of the padding words are outside)
+__device__ __forceinline__ unsigned int bit_col_mask(int w, int k) {
+    const int lo = w * 32;
+    if (lo >= k) return 0u;
+    return (k - lo >= 32) ? 0xffffffffu : ((1u << (k - lo)) - 1u);
+}
+
+// rows (warp per row) of two bit tiles that differ in one of the k columns
+__global__ void __launch_bounds__(256) k_count_diff_bits(const unsigned int *__restrict__ a, const unsigned int *__restrict__ b,
+                                                         long long rows, int k, int words, unsigned long long *__restrict__ count) {
+    __shared__ unsigned int s_count;
+    if (threadIdx.x == 0) s_count = 0u;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
+    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    for (long long r = warp_id; r < rows; r += warps_total) {
+        bool diff = false;
+        for (int w = lane; w * 32 < k; w += 32) diff |= ((a[r * words + w] ^ b[r * words + w]) & bit_col_mask(w, k)) != 0u;
+        if (__any_sync(0xffffffffu, diff) && lane == 0) atomicAdd(&s_count, 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && s_count) atomicAdd(count, (unsigned long long)s_count);
+}
+
+// dist[r, c] = level for every column c < k whose bit is set in `nw` and clear in `old`; counts those bits.  One thread
+// per (row, word).
+__global__ void __launch_bounds__(256) k_bits_mark_new(const unsigned int *__restrict__ nw, const unsigned int *__restrict__ old,
+                                                       int *__restrict__ dist, long long rows, int k, int words, int level,
+                                                       unsigned long long *__restrict__ count) {
+    const int used = (k + 31) / 32;
+    const long long total = rows * used;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    unsigned long long mine = 0;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const long long r = i / used;
+        const int w = (int)(i - r * used);
+        unsigned int fresh = nw[r * words + w] & ~old[r * words + w] & bit_col_mask(w, k);
+        mine += (unsigned long long)__popc(fresh);
+        int *drow = dist + r * k + w * 32;
+        while (fresh) {
+            const int c = __ffs(fresh) - 1;
+            drow[c] = level;
+            fresh &= fresh - 1u;
+        }
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, off);
+    if ((threadIdx.x & 31) == 0 && mine) atomicAdd(count, mine);
+}
+
+template <int G, int VPL, int TR, int TN, class V = uint4>
+int launch_tiles_bits_one(arrow_ctx *ctx, const TileArgs &t) {
+    constexpr size_t SMEM = TileCfgBits<TR, TN>::SMEM_BYTES;
+    auto fn = k_spmm_tiles_bits<G, VPL, TR, TN, V>;
+    static bool attr_set[64] = {};            /* function attributes are per device */
+    static int occ_dev[64] = {};
+    const int dv = ctx->device & 63;
+    if (!attr_set[dv]) {
+        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
+        attr_set[dv] = true;
+    }
+    const int occ = occ_dev[dv];
+    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
+    int sms = ctx->sm_count;
+    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
+    int grid = (int)std::min<long long>((long long)per_sm * sms, t.n_tiles);
+    cudaMemsetAsync(t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
+    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(t);
+    ctx->launches++;
+    return ARROW_OK;
+}
+
+// (lanes per row, uint4 per lane) from k4 = words / 4 as launch_tiles_sr_shape picks them from an fp32 row of `words`
+// columns, except that rows of more than 32 uint4 take 32 lanes of 2 (the VPL = 4 instances spill)
+int launch_tiles_bits_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A) {
+    if (t.a.k == 1) {                  // one-word rows (k <= 32): a lane per row, one uint32 gather per entry
+        t.a.k4 = 1;
+        const int list = tile_list_for(ctx, 1, 4, true);
+        t.tiles = A->tiles[list];
+        t.n_tiles = A->n_tiles[list];
+#define BIW(TR, TN) return launch_tiles_bits_one<1, 1, TR, TN, unsigned>(ctx, t)
+        if (list == TILE_LIST_BIG) BIW(TILE_ROWS_BIG, TILE_NNZ_BIG);
+        BIW(TILE_ROWS, TILE_NNZ);
+#undef BIW
+    }
+    const int k4 = t.a.k4;
+    const int vpl = k4 >= 8 ? 2 : 1;
+    const int lanes = (k4 + vpl - 1) / vpl;           // <= 32: k4 <= 64
+    int g = 1;
+    while (g < lanes) g <<= 1;
+    const int list = tile_list_for(ctx, 4 * k4, 4, k4 <= 8);                 // the row's bytes as an fp32 row
+    const bool big = list == TILE_LIST_BIG;
+    t.tiles = A->tiles[list];
+    t.n_tiles = A->n_tiles[list];
+#define TBI(GG, VV, TR, TN) return launch_tiles_bits_one<GG, VV, TR, TN>(ctx, t)
+#define BIB(GG, VV) if (big && g == GG && vpl == VV) TBI(GG, VV, TILE_ROWS_BIG, TILE_NNZ_BIG)
+#define BIS(GG, VV) if (g == GG && vpl == VV) TBI(GG, VV, TILE_ROWS, TILE_NNZ)
+    BIB(1, 1); BIB(2, 1); BIB(4, 1); BIB(8, 1); BIB(4, 2);
+    BIS(1, 1); BIS(2, 1); BIS(4, 1); BIS(8, 1); BIS(4, 2); BIS(8, 2); BIS(16, 2); BIS(32, 2);
+#undef BIS
+#undef BIB
+#undef TBI
+    return fail(ctx, ARROW_ERR_UNSUPPORTED, "no bit tile kernel for k4=%d vpl=%d", k4, vpl);
+}
+
+// the product of arrow_spmm_sr in (or, and); `a` carries the validated bit operands, a.k = the row's words
+int spmm_bits(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a) {
+    const int words = a.k;
+    const int lane = ctx->cur_lane;
+    cudaStream_t stream = cur_stream(ctx);
+    if (A->n_tiles[TILE_LIST_SMALL] > 0) {
+        TileArgs t;
+        t.a = a;
+        t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
+        t.ticket = ctx->tile_ticket + 2 * lane;
+        t.l2_hints = ctx->l2_hints_plain;
+        t.prefetch = 0;
+        const int rc = launch_tiles_bits_shape(ctx, t, A);
+        if (rc != ARROW_OK) return rc;
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+
+    if (A->n_long_tasks > 0) {
+        const size_t need = (size_t)A->n_long_tasks * words * 4;
+        if (need > ctx->long_scratch_bytes[lane]) {
+            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
+            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
+            ctx->long_scratch[lane] = nullptr;
+            ctx->long_scratch_bytes[lane] = 0;
+            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
+            ctx->long_scratch_bytes[lane] = need;
+        }
+        LongArgs la;
+        la.tasks = A->long_tasks;
+        la.indices = a.indices;
+        la.vals = nullptr;
+        la.X = a.X;
+        la.scratch = ctx->long_scratch[lane];
+        la.k = words;
+        la.X2 = nullptr;
+        la.x_split = 0;
+        const size_t smem = (size_t)8 * words * 4;             // <= 8 KB: words <= 256
+        k_spmm_long_partial_bits<<<A->n_long_tasks, 256, smem, stream>>>(la);
+        ctx->launches++;
+        k_spmm_long_reduce_bits<<<A->n_long_rows, 128, 0, stream>>>(
+            A->long_rows, A->long_first, reinterpret_cast<const unsigned int *>(la.scratch),
+            reinterpret_cast<unsigned int *>(a.C), words, reinterpret_cast<const unsigned int *>(a.add_src), a.add_map);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
+    return ARROW_OK;
+}
+
+constexpr int BITS_MAX_K = 8192;    // 256 words = 64 uint4 per row: the widest (G, VPL) = (32, 2) tile shape
+
+int gather_rows_or(arrow_ctx *ctx, DenseBuf *D, const DenseBuf *S, const IdxMap *m) {
+    const long long n_rows = m->n;
+    if (n_rows == 0) return ARROW_OK;
+    if (bit_row_words(D->k) == 1) {    // one-word rows: a thread per row
+        int grid = (int)std::max<long long>(1, std::min<long long>((n_rows + 255) / 256, (long long)ctx->sm_count * 8));
+        k_gather_rows_or_word<<<grid, 256, 0, cur_stream(ctx)>>>(reinterpret_cast<unsigned *>(D->p), reinterpret_cast<const unsigned *>(S->p), m->p, n_rows);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+        return ARROW_OK;
+    }
+    const int vpr = bit_row_words(D->k) / 4;
+    int g = 1;
+    while (g < vpr && g < 8) g <<= 1;                        // lanes per row
+    const int threads = 256;
+    const long long rows_per_cta = (threads / 32) * (32 / g);
+    int grid = (int)std::min<long long>((n_rows + rows_per_cta - 1) / rows_per_cta, (long long)ctx->sm_count * 8);
+    grid = std::max(grid, 1);
+    uint4 *dp = reinterpret_cast<uint4 *>(D->p);
+    const uint4 *sp = reinterpret_cast<const uint4 *>(S->p);
+    switch (g) {
+        case 1: k_gather_rows_or<1><<<grid, threads, 0, cur_stream(ctx)>>>(dp, sp, m->p, n_rows, vpr); break;
+        case 2: k_gather_rows_or<2><<<grid, threads, 0, cur_stream(ctx)>>>(dp, sp, m->p, n_rows, vpr); break;
+        case 4: k_gather_rows_or<4><<<grid, threads, 0, cur_stream(ctx)>>>(dp, sp, m->p, n_rows, vpr); break;
+        default: k_gather_rows_or<8><<<grid, threads, 0, cur_stream(ctx)>>>(dp, sp, m->p, n_rows, vpr); break;
+    }
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return ARROW_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // predecessors of the tropical semirings: the product of arrow_spmm_sr carried over (value, label) pairs.  A candidate
 // of row r is an entry p with a valid column c != self(r); its value is fl(A[r,p] + X[c]) and its label is c.  Pairs are
 // ⊕-reduced lexicographically: the better value wins (smaller for (min, +), larger for (max, +)), equal values (by value,
@@ -3600,12 +4068,13 @@ int arrow_map_d2h(arrow_ctx *ctx, int map, int32_t *host, int64_t n) {
 int arrow_dense_alloc_dtype(arrow_ctx *ctx, int64_t rows, int k, int dtype, int *buf_out) {
     CHECK_CTX(ctx);
     if (!buf_out || rows < 0 || k < 1) return fail(ctx, ARROW_ERR_ARG, "bad dense shape %lld x %d", (long long)rows, k);
-    if (dtype != ARROW_F32 && dtype != ARROW_F64 && dtype != ARROW_I32) return fail(ctx, ARROW_ERR_ARG, "unknown dtype %d", dtype);
+    if (dtype != ARROW_F32 && dtype != ARROW_F64 && dtype != ARROW_I32 && dtype != ARROW_B1)
+        return fail(ctx, ARROW_ERR_ARG, "unknown dtype %d", dtype);
     DenseBuf d;
     d.rows = rows;
     d.k = k;
     d.dtype = dtype;
-    const size_t bytes = std::max<size_t>((size_t)rows * (size_t)k * dtype_size(dtype), 16);
+    const size_t bytes = std::max<size_t>((size_t)rows * row_bytes(dtype, k), 16);
     cudaError_t e = cudaMalloc(&d.p, bytes);
     if (e != cudaSuccess) {
         cudaGetLastError();
@@ -3650,10 +4119,11 @@ int arrow_dense_fill(arrow_ctx *ctx, int buf, float value) {
     DenseBuf *d = get_dense(ctx, buf);
     if (!d) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", buf);
     REFUSE_I32(ctx, d, "arrow_dense_fill");
+    if (d->dtype == ARROW_B1 && value != 0.f) return fail(ctx, ARROW_ERR_ARG, "a bit tile is filled with 0 only");
     const long long n = (long long)d->rows * d->k;
     if (n == 0) return ARROW_OK;
     if (value == 0.f) {
-        CUDA_TRY(ctx, cudaMemsetAsync(d->p, 0, (size_t)n * dtype_size(d->dtype), ctx->stream));
+        CUDA_TRY(ctx, cudaMemsetAsync(d->p, 0, (size_t)d->rows * row_bytes(d->dtype, d->k), ctx->stream));
     } else if (d->dtype == ARROW_F64) {
         k_fill<double><<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(reinterpret_cast<double *>(d->p), (double)value, n);
         ctx->launches++;
@@ -3673,7 +4143,7 @@ int arrow_dense_h2d(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, const v
     if (!host || row0 < 0 || rows < 0 || row0 + rows > d->rows)
         return fail(ctx, ARROW_ERR_ARG, "h2d rows [%lld,%lld) outside tile of %lld rows", (long long)row0, (long long)(row0 + rows), (long long)d->rows);
     if (rows == 0) return ARROW_OK;
-    CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(d, row0), host, (size_t)rows * d->k * dtype_size(d->dtype), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(d, row0), host, (size_t)rows * row_bytes(d->dtype, d->k), cudaMemcpyHostToDevice, ctx->stream));
     return ARROW_OK;
 }
 
@@ -3684,7 +4154,7 @@ int arrow_dense_d2h(arrow_ctx *ctx, int buf, int64_t row0, int64_t rows, void *h
     if (!host || row0 < 0 || rows < 0 || row0 + rows > d->rows)
         return fail(ctx, ARROW_ERR_ARG, "d2h rows [%lld,%lld) outside tile of %lld rows", (long long)row0, (long long)(row0 + rows), (long long)d->rows);
     if (rows == 0) return ARROW_OK;
-    CUDA_TRY(ctx, cudaMemcpyAsync(host, dense_row(d, row0), (size_t)rows * d->k * dtype_size(d->dtype), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(host, dense_row(d, row0), (size_t)rows * row_bytes(d->dtype, d->k), cudaMemcpyDeviceToHost, ctx->stream));
     return ARROW_OK;
 }
 
@@ -3697,7 +4167,7 @@ int arrow_dense_copy(arrow_ctx *ctx, int dst, int64_t dst_row0, int src, int64_t
     if (rows < 0 || dst_row0 < 0 || src_row0 < 0 || dst_row0 + rows > a->rows || src_row0 + rows > b->rows)
         return fail(ctx, ARROW_ERR_ARG, "copy range outside tiles");
     if (rows == 0) return ARROW_OK;
-    CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(a, dst_row0), dense_row(b, src_row0), (size_t)rows * a->k * dtype_size(a->dtype),
+    CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(a, dst_row0), dense_row(b, src_row0), (size_t)rows * row_bytes(a->dtype, a->k),
                                   cudaMemcpyDeviceToDevice, cur_stream(ctx)));
     return ARROW_OK;
 }
@@ -3993,6 +4463,7 @@ int arrow_ptrtable_upload(arrow_ctx *ctx, const int *bufs, int n_bufs, const int
         if (b == 0) k = d->k;
         else if (d->k != k) return fail(ctx, ARROW_ERR_ARG, "tiles of a pointer table must share the feature width");
         REFUSE_I32(ctx, d, "arrow_ptrtable_upload");
+        REFUSE_B1(ctx, d, "arrow_ptrtable_upload");
         if (d->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "pointer tables are float32 only");
         bases[b] = (unsigned long long)d->p;
         rows_of[b] = d->rows;
@@ -4055,8 +4526,9 @@ static int gather_common(arrow_ctx *ctx, DenseBuf *D, const float *src, const Mu
     if (n_rows == 0) return ARROW_OK;
     const int k = D->k;
     const bool f64 = D->dtype == ARROW_F64;
-    const bool vec = f64 ? (k % 2 == 0) : (k % 4 == 0);        // 16-byte vectors: float4 / double2
-    const int vpr = vec ? (f64 ? k / 2 : k / 4) : k;
+    const bool bits = D->dtype == ARROW_B1;                  // whole rows of words, moved as float4 loads / stores (no arithmetic)
+    const bool vec = bits ? bit_row_words(k) % 4 == 0 : (f64 ? (k % 2 == 0) : (k % 4 == 0));        // 16-byte vectors: float4 / double2
+    const int vpr = bits ? (vec ? bit_row_words(k) / 4 : bit_row_words(k)) : (vec ? (f64 ? k / 2 : k / 4) : k);
     int g = 1;
     while (g < vpr && g < 32) g <<= 1;                       // lanes per row
     if (g > 8 && vpr <= 32) g = 8;                           // 8 lanes x 4 vectors cover k <= 128 in one pass
@@ -4104,6 +4576,8 @@ int arrow_gather_rows(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int fla
     if (D->k != S->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch %d vs %d", D->k, S->k);
     if (D->dtype != S->dtype) return fail(ctx, ARROW_ERR_ARG, "dtype mismatch: destination %s, source %s", dtype_name(D->dtype), dtype_name(S->dtype));
     REFUSE_I32(ctx, D, "arrow_gather_rows");
+    if (D->dtype == ARROW_B1 && (flags & ARROW_ACCUMULATE))
+        return fail(ctx, ARROW_ERR_ARG, "arrow_gather_rows: bits do not accumulate (arrow_gather_rows_sr with ARROW_SR_OR_AND ORs them)");
     if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "gather source and destination must not alias");
     if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
     if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
@@ -4119,7 +4593,7 @@ int arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, in
         if (add_buf < 0 && add_map < 0) return arrow_spmm(ctx, csr, x_buf, c_buf, -1, 0, ARROW_VARIANT_AUTO);
         return arrow_spmm_add(ctx, csr, x_buf, c_buf, add_buf, add_map, ARROW_VARIANT_AUTO);
     }
-    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS)
+    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS && semiring != ARROW_SR_OR_AND)
         return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
     CHECK_POISON(ctx);
     Csr *A = get_csr(ctx, csr);
@@ -4127,7 +4601,11 @@ int arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, in
     DenseBuf *C = get_dense(ctx, c_buf);
     if (!A) return fail(ctx, ARROW_ERR_HANDLE, "bad csr handle %d", csr);
     if (!X || !C) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x=%d c=%d)", x_buf, c_buf);
-    if (X->dtype != A->dtype || C->dtype != A->dtype)
+    // (or, and) reads the block's structure only: its operands are bit tiles whatever the block's value type
+    const int op_dtype = semiring == ARROW_SR_OR_AND ? ARROW_B1 : A->dtype;
+    if (semiring == ARROW_SR_OR_AND && (X->dtype != ARROW_B1 || C->dtype != ARROW_B1))
+        return fail(ctx, ARROW_ERR_ARG, "(or, and) runs on bit tiles: X is %s, C is %s", dtype_name(X->dtype), dtype_name(C->dtype));
+    if (X->dtype != op_dtype || C->dtype != op_dtype)
         return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, X is %s, C is %s", dtype_name(A->dtype),
                     dtype_name(X->dtype), dtype_name(C->dtype));
     if (X->k != C->k) return fail(ctx, ARROW_ERR_ARG, "X has %d feature columns, C has %d", X->k, C->k);
@@ -4142,12 +4620,25 @@ int arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, in
         IdxMap *am = get_map(ctx, add_map);
         if (!S || !am) return fail(ctx, ARROW_ERR_HANDLE, "bad addend handles (buf=%d map=%d)", add_buf, add_map);
         if (S->k != k) return fail(ctx, ARROW_ERR_ARG, "addend has %d feature columns, expected %d", S->k, k);
-        if (S->dtype != A->dtype) return fail(ctx, ARROW_ERR_ARG, "mixed precision: the block is %s, the addend is %s", dtype_name(A->dtype), dtype_name(S->dtype));
+        if (S->dtype != op_dtype) return fail(ctx, ARROW_ERR_ARG, "mixed precision: the operands are %s, the addend is %s", dtype_name(op_dtype), dtype_name(S->dtype));
         if (am->n < A->n_rows) return fail(ctx, ARROW_ERR_ARG, "addend map has %lld entries, block has %lld rows", (long long)am->n, (long long)A->n_rows);
         if (am->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "addend map reaches row %lld, addend tile has %lld rows", (long long)am->limit, (long long)S->rows);
         if (S->p == C->p) return fail(ctx, ARROW_ERR_ARG, "addend and C must not alias");
         a.add_src = S->p;
         a.add_map = am->p;
+    }
+    if (semiring == ARROW_SR_OR_AND) {
+        if (k > BITS_MAX_K) return fail(ctx, ARROW_ERR_UNSUPPORTED, "(or, and) covers k <= %d columns, X has %d", BITS_MAX_K, k);
+        if (A->n_rows == 0) return ARROW_OK;
+        a.indptr = A->indptr;
+        a.indices = A->indices;
+        a.X = X->p;
+        a.C = C->p;
+        a.n_rows = A->n_rows;
+        a.k = bit_row_words(k);                   // the bit kernels count in words
+        a.k4 = a.k / 4;
+        a.long_threshold = A->long_threshold;
+        return spmm_bits(ctx, A, a);
     }
     if (A->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the (min, +) / (max, +) semirings are float32 only");
     if (A->n_rows == 0) return ARROW_OK;
@@ -4167,7 +4658,7 @@ int arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, in
 int arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int semiring) {
     CHECK_CTX(ctx);
     if (semiring == ARROW_SR_PLUS_TIMES) return arrow_gather_rows(ctx, dst_buf, src_buf, map, ARROW_ACCUMULATE);
-    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS)
+    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS && semiring != ARROW_SR_OR_AND)
         return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
     CHECK_POISON(ctx);
     DenseBuf *D = get_dense(ctx, dst_buf), *S = get_dense(ctx, src_buf);
@@ -4180,6 +4671,9 @@ int arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int 
     if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "gather source and destination must not alias");
     if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
     if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
+    if ((semiring == ARROW_SR_OR_AND) != (D->dtype == ARROW_B1))
+        return fail(ctx, ARROW_ERR_ARG, "(or, and) runs on bit tiles and only there: semiring %d, tiles of %s", semiring, dtype_name(D->dtype));
+    if (semiring == ARROW_SR_OR_AND) return gather_rows_or(ctx, D, S, m);
     if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the (min, +) / (max, +) semirings are float32 only");
     if (semiring == ARROW_SR_MIN_PLUS) return gather_rows_sr<SrMinPlus>(ctx, D, S, m);
     return gather_rows_sr<SrMaxPlus>(ctx, D, S, m);
@@ -4284,7 +4778,10 @@ int arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed) 
     CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof(unsigned long long), stream));
     const int grid = (int)std::min<long long>((A->rows + 7) / 8, (long long)ctx->sm_count * 8);
     unsigned long long *c = reinterpret_cast<unsigned long long *>(cnt.p);
-    if (A->dtype == ARROW_F64)
+    if (A->dtype == ARROW_B1)
+        k_count_diff_bits<<<grid, 256, 0, stream>>>(reinterpret_cast<const unsigned int *>(A->p), reinterpret_cast<const unsigned int *>(B->p),
+                                                    A->rows, A->k, bit_row_words(A->k), c);
+    else if (A->dtype == ARROW_F64)
         k_count_diff<double><<<grid, 256, 0, stream>>>(reinterpret_cast<const double *>(A->p), reinterpret_cast<const double *>(B->p), A->rows, A->k, c);
     else
         k_count_diff<float><<<grid, 256, 0, stream>>>(A->p, B->p, A->rows, A->k, c);
@@ -4297,6 +4794,38 @@ int arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed) 
     return ARROW_OK;
 }
 
+int arrow_bits_mark_new(arrow_ctx *ctx, int new_buf, int old_buf, int dist_buf, int level, int64_t *n_new) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    DenseBuf *N = get_dense(ctx, new_buf), *O = get_dense(ctx, old_buf), *D = get_dense(ctx, dist_buf);
+    if (!N || !O || !D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (new=%d old=%d dist=%d)", new_buf, old_buf, dist_buf);
+    if (!n_new) return fail(ctx, ARROW_ERR_ARG, "null n_new");
+    if (N->dtype != ARROW_B1 || O->dtype != ARROW_B1 || D->dtype != ARROW_I32)
+        return fail(ctx, ARROW_ERR_ARG, "new / old are bit tiles and dist an int32 tile: got %s / %s / %s", dtype_name(N->dtype),
+                    dtype_name(O->dtype), dtype_name(D->dtype));
+    if (N->rows != O->rows || N->k != O->k || D->rows != N->rows || D->k != N->k)
+        return fail(ctx, ARROW_ERR_ARG, "tiles differ in shape: new %lld x %d, old %lld x %d, dist %lld x %d", (long long)N->rows, N->k,
+                    (long long)O->rows, O->k, (long long)D->rows, D->k);
+    *n_new = 0;
+    if (N->rows == 0) return ARROW_OK;
+    cudaStream_t stream = cur_stream(ctx);
+    DevTmp cnt;
+    CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof(unsigned long long)));
+    CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof(unsigned long long), stream));
+    const long long items = N->rows * (long long)((N->k + 31) / 32);
+    const int grid = (int)std::max<long long>(1, std::min<long long>((items + 255) / 256, (long long)ctx->sm_count * 8));
+    k_bits_mark_new<<<grid, 256, 0, stream>>>(reinterpret_cast<const unsigned int *>(N->p), reinterpret_cast<const unsigned int *>(O->p),
+                                              reinterpret_cast<int *>(D->p), N->rows, N->k, bit_row_words(N->k), level,
+                                              reinterpret_cast<unsigned long long *>(cnt.p));
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    unsigned long long h = 0;
+    CUDA_TRY(ctx, cudaMemcpyAsync(&h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+    *n_new = (int64_t)h;
+    return ARROW_OK;
+}
+
 int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, const int64_t *row_bounds, int n_src, int map, int flags) {
     CHECK_CTX(ctx);
     DenseBuf *D = get_dense(ctx, dst_buf);
@@ -4305,6 +4834,7 @@ int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, co
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
     if (!src_bufs || !row_bounds || n_src < 1 || n_src > MAX_SRC) return fail(ctx, ARROW_ERR_ARG, "need 1..%d sources", MAX_SRC);
     REFUSE_I32(ctx, D, "arrow_gather_rows_multi");
+    REFUSE_B1(ctx, D, "arrow_gather_rows_multi");
     if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the multi-source gather is float32 only");
     if (m->n > D->rows) return fail(ctx, ARROW_ERR_ARG, "map has %lld entries, destination has %lld rows", (long long)m->n, (long long)D->rows);
     MultiSrc ms;
@@ -4315,6 +4845,7 @@ int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, co
         if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad source handle %d", src_bufs[s]);
         if (S->k != D->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in source %d", s);
         REFUSE_I32(ctx, S, "arrow_gather_rows_multi");
+        REFUSE_B1(ctx, S, "arrow_gather_rows_multi");
         if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the multi-source gather is float32 only");
         if (row_bounds[s + 1] < row_bounds[s] || row_bounds[s + 1] - row_bounds[s] > S->rows)
             return fail(ctx, ARROW_ERR_ARG, "source %d owns %lld rows but its tile has %lld", s, (long long)(row_bounds[s + 1] - row_bounds[s]), (long long)S->rows);
@@ -4335,6 +4866,7 @@ int arrow_push_rows(arrow_ctx *ctx, const int *dst_bufs, const int64_t *item_bou
     if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", src_buf);
     if (!m) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
     REFUSE_I32(ctx, S, "arrow_push_rows");
+    REFUSE_B1(ctx, S, "arrow_push_rows");
     if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_push_rows is float32 only");
     if (!dst_bufs || !item_bounds || n_dst < 1 || n_dst > MAX_SRC) return fail(ctx, ARROW_ERR_ARG, "need 1..%d destinations", MAX_SRC);
     if (m->limit > S->rows) return fail(ctx, ARROW_ERR_ARG, "map reaches row %lld, source has %lld rows", (long long)m->limit, (long long)S->rows);
@@ -4351,6 +4883,7 @@ int arrow_push_rows(arrow_ctx *ctx, const int *dst_bufs, const int64_t *item_bou
         if (!D) return fail(ctx, ARROW_ERR_HANDLE, "bad destination handle %d", dst_bufs[d]);
         if (D->k != S->k) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in destination %d", d);
         REFUSE_I32(ctx, D, "arrow_push_rows");
+        REFUSE_B1(ctx, D, "arrow_push_rows");
         if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_push_rows is float32 only");
         if (cnt > D->rows) return fail(ctx, ARROW_ERR_ARG, "destination %d receives %lld rows but its region has %lld", d, (long long)cnt, (long long)D->rows);
         if (D->p == S->p) return fail(ctx, ARROW_ERR_ARG, "push source and destination must not alias");
@@ -4399,6 +4932,7 @@ int arrow_reduce_rows(arrow_ctx *ctx, int dst_buf, int out_table, const int *src
     DenseBuf *D = dst_buf >= 0 ? get_dense(ctx, dst_buf) : nullptr;
     if (dst_buf >= 0 && !D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %d", dst_buf);
     REFUSE_I32(ctx, D, "arrow_reduce_rows");
+    REFUSE_B1(ctx, D, "arrow_reduce_rows");
     if (D && D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_reduce_rows is float32 only");
     PtrTable *OT = nullptr;
     if (out_table >= 0) {
@@ -4419,6 +4953,7 @@ int arrow_reduce_rows(arrow_ctx *ctx, int dst_buf, int out_table, const int *src
         if (s2 == 0) k = S->k;
         if (S->k != k || (D && D->k != k) || (OT && OT->k != k)) return fail(ctx, ARROW_ERR_ARG, "feature width mismatch in source %d", s2);
         REFUSE_I32(ctx, S, "arrow_reduce_rows");
+        REFUSE_B1(ctx, S, "arrow_reduce_rows");
         if (S->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_reduce_rows is float32 only");
         if (S->rows < rows) return fail(ctx, ARROW_ERR_ARG, "source %d has %lld rows, %lld are reduced", s2, (long long)S->rows, (long long)rows);
         ms.p[s2] = S->p;
@@ -4539,7 +5074,7 @@ int arrow_dense_h2d_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_
     cudaStream_t st;
     int rc = lane_stream(ctx, lane, &st);
     if (rc != ARROW_OK) return rc;
-    if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(d, row0), host, (size_t)rows * d->k * dtype_size(d->dtype), cudaMemcpyHostToDevice, st));
+    if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(dense_row(d, row0), host, (size_t)rows * row_bytes(d->dtype, d->k), cudaMemcpyHostToDevice, st));
     return ARROW_OK;
 }
 
@@ -4551,7 +5086,7 @@ int arrow_dense_d2h_lane(arrow_ctx *ctx, int lane, int buf, int64_t row0, int64_
     cudaStream_t st;
     int rc = lane_stream(ctx, lane, &st);
     if (rc != ARROW_OK) return rc;
-    if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(host, dense_row(d, row0), (size_t)rows * d->k * dtype_size(d->dtype), cudaMemcpyDeviceToHost, st));
+    if (rows) CUDA_TRY(ctx, cudaMemcpyAsync(host, dense_row(d, row0), (size_t)rows * row_bytes(d->dtype, d->k), cudaMemcpyDeviceToHost, st));
     return ARROW_OK;
 }
 

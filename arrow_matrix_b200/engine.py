@@ -27,6 +27,11 @@ levels in any semiring): the forward exchange only moves rows, the backward aggr
 behind the sentinel are the same.  ``add_identity`` puts the ⊗ identity on level 0's diagonal, so that a step computes
 ``X ⊕ (A ⊗ X)``: the relaxation step of BFS and Bellman-Ford (``(I + A) X`` in ``plus_times``).
 
+``or_and`` is the boolean semiring on bit tiles (one bit per element, 32 per word): ⊗ is "the entry exists" and ⊕ is
+OR, so a step with ``add_identity`` is one hop of multi-source BFS / reachability.  Features go in as booleans (non-zero
+is true) and come out as booleans; ``bfs_levels()`` steps to the fixed point and records the hop at which every element
+was first reached.
+
 ``predecessors()`` returns, in the tropical semirings, the level-0 row each element's value came from (the parent array
 of a BFS tree, the predecessor of a shortest or critical path): one more pass of the fused step over (value, label)
 pairs, see DESIGN.md §4.
@@ -43,13 +48,14 @@ from . import decomp
 
 # the semiring's ⊕ identity (its "zero": what zero_rhs and fresh tiles hold) and ⊗ identity (what add_identity puts on
 # level 0's diagonal)
-_PLUS_ZERO = {_lib.SR_PLUS_TIMES: 0.0, _lib.SR_MIN_PLUS: float("inf"), _lib.SR_MAX_PLUS: float("-inf")}
-_TIMES_ONE = {_lib.SR_PLUS_TIMES: 1.0, _lib.SR_MIN_PLUS: 0.0, _lib.SR_MAX_PLUS: 0.0}
+_PLUS_ZERO = {_lib.SR_PLUS_TIMES: 0.0, _lib.SR_MIN_PLUS: float("inf"), _lib.SR_MAX_PLUS: float("-inf"), _lib.SR_OR_AND: 0.0}
+_TIMES_ONE = {_lib.SR_PLUS_TIMES: 1.0, _lib.SR_MIN_PLUS: 0.0, _lib.SR_MAX_PLUS: 0.0, _lib.SR_OR_AND: 1.0}
 
 
 def semiring_code(semiring: str, dtype, fused_style: str = "gather") -> int:
     """``_lib.SR_*`` of a semiring name; raises ``ValueError`` (before any CUDA work) for an unknown name and for the
-    combinations that do not exist: the tropical semirings are float32 and run the gather style of the fused step."""
+    combinations that do not exist: the tropical and boolean semirings need a float32 decomposition and run the gather
+    style of the fused step."""
     if semiring not in _lib.SEMIRINGS:
         raise ValueError(f"unknown semiring {semiring!r}: expected one of {', '.join(_lib.SEMIRINGS)}")
     code = _lib.SEMIRINGS[semiring]
@@ -104,6 +110,8 @@ class ArrowEngine:
         self.levels: List[_LevelState] = []
         self._wit_labels: Optional[List[_lib.Dense]] = None     # predecessors(): int32 label tile per level (level 0: P)
         self._wit_values = {}                                    # predecessors(): value tiles of levels without a cbuf
+        self._bfs_tiles: Optional[Tuple[_lib.Dense, ...]] = None   # bfs_levels(): (hop tile, all-zero and all-one bit tiles)
+        self.last_bfs_steps = 0                                  # steps the last bfs_levels() call took
         fused_ok = True
         cmap_prev = None                      # level j-1 row -> level-0 row (host, int64, -1 invalid)
         for j, (B, _) in enumerate(decomposition):
@@ -145,10 +153,15 @@ class ArrowEngine:
         self.ctx.sync()
 
     # -- buffers ---------------------------------------------------------------------------------
+    @property
+    def bits(self) -> bool:
+        """the tiles are bit tiles (``or_and``)"""
+        return getattr(self, "sr", _lib.SR_PLUS_TIMES) == _lib.SR_OR_AND
+
     def _alloc(self, rows: int) -> _lib.Dense:
-        """a tile holding the semiring's zero (the ⊕ identity)"""
-        b = self.ctx.dense_alloc(rows, self.k, self.dtype)
-        if self.sr != _lib.SR_PLUS_TIMES:
+        """a feature tile holding the semiring's zero (the ⊕ identity): the engine's element type, bits in ``or_and``"""
+        b = self.ctx.dense_alloc(rows, self.k, _lib.BITS if self.bits else self.dtype)
+        if _PLUS_ZERO[self.sr] != 0.0:
             b.fill(_PLUS_ZERO[self.sr])
         return b
 
@@ -194,13 +207,14 @@ class ArrowEngine:
 
     # -- features / results (level-0 row order, like the reference's per-rank tiles) -----------------
     def set_features(self, X: np.ndarray, sync: bool = True):
-        """Level-0 feature tiles, concatenated (``B.set_features`` on every level-0 rank)."""
+        """Level-0 feature tiles, concatenated (``B.set_features`` on every level-0 rank); in ``or_and`` non-zero is
+        true."""
         st = self.levels[0]
         if X.shape != (st.rows, self.k):
             raise ValueError(f"expected features of shape {(st.rows, self.k)}, got {X.shape}")
         if st.xi == st.ci:                      # X aliases C: keep the result tile intact, like a rebind
             st.xi = 1 - st.ci
-        st.bufs[st.xi].h2d(X)
+        st.bufs[st.xi].h2d(_lib.pack_bits(X) if self.bits else X)
         if sync:
             self.ctx.sync()
 
@@ -224,8 +238,18 @@ class ArrowEngine:
             raise RuntimeError("level tiles are not materialised in fused/scatter mode; use mode='exchange'")
         return st.bufs[st.ci]
 
+    def _host(self, tile: _lib.Dense, out: Optional[np.ndarray]) -> np.ndarray:
+        """a feature tile on the host: as it is, or unpacked to bool [rows x k] in ``or_and``"""
+        if not self.bits:
+            return tile.d2h(out)
+        got = _lib.unpack_bits(tile.d2h(), self.k)
+        if out is None:
+            return got
+        out[...] = got
+        return out
+
     def result(self, level: int = 0, out: Optional[np.ndarray] = None) -> np.ndarray:
-        return self.result_buffer(level).d2h(out)
+        return self._host(self.result_buffer(level), out)
 
     # -- small uniform API shared with the sharded engine (used by the reference-facing classes) ----------
     def local_rows_of(self, level: int) -> int:
@@ -243,7 +267,7 @@ class ArrowEngine:
         st = self.levels[level]
         if st.bufs[st.xi] is None:
             raise RuntimeError("level tiles are not materialised in fused mode; use mode='exchange'")
-        return st.bufs[st.xi].d2h(out)
+        return self._host(st.bufs[st.xi], out)
 
     def spmm_level(self, level: int):
         """One level's arrow product on its current features (``B.spmm()`` of that level)."""
@@ -258,7 +282,7 @@ class ArrowEngine:
         if self.mode == "exchange":
             return
         st0 = self.levels[0]
-        keep = [b.d2h() for b in st0.bufs]
+        keep = [b.d2h() for b in st0.bufs]                    # raw tiles (words in or_and)
         xi, ci = st0.xi, st0.ci
         self.set_mode("exchange")
         st0 = self.levels[0]
@@ -377,6 +401,8 @@ class ArrowEngine:
         such a row has no vertex identity)."""
         if self.sr == _lib.SR_PLUS_TIMES:
             raise ValueError("predecessors exist in the min_plus / max_plus semirings only, the engine runs plus_times")
+        if self.sr == _lib.SR_OR_AND:
+            raise ValueError("predecessors exist in the min_plus / max_plus semirings only, the engine runs or_and")
         if not self.fused_ok:
             raise ValueError("predecessors need a level-0 row behind every non-zero, but a level reads rows behind the "
                              "sentinel")
@@ -413,6 +439,39 @@ class ArrowEngine:
         self.ctx.spmm_sr_witness(st0.csr, x, self._wit_labels[0], dist=x, semiring=self.sr, **add)
         return self._wit_labels[0]
 
+    # -- multi-source BFS (or_and) ----------------------------------------------------------------------------------
+    def bfs_levels(self, max_steps: int, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Hop levels of a multi-source BFS from the current level-0 features (int32 [n x k], level-0 row order like
+        ``result()``): ``0`` where a feature bit is set now (the sources), ``h`` where the bit was first set by the
+        ``h``-th ``step()``, ``-1`` where it is never set.  Steps until a step sets no new bit, at most ``max_steps``
+        times; ``last_bfs_steps`` holds the number of steps taken.  After every step one device pass
+        (``arrow_bits_mark_new``) records the fresh bits and counts them: the level record and the fixed-point test at
+        once.  Needs ``or_and`` with ``add_identity`` (bits then only grow); raises ``ValueError`` before any CUDA work
+        otherwise.  The features end at the fixed point (``result()``); synchronises."""
+        if not self.bits:
+            raise ValueError(f"bfs_levels runs the or_and semiring, the engine runs {self.semiring}")
+        if not self.add_identity:
+            raise ValueError("bfs_levels needs add_identity=True: a step must keep the bits it already has")
+        self.sync()
+        st0 = self.levels[0]
+        if self._bfs_tiles is None:
+            ones = self._alloc(st0.rows)
+            ones.h2d(np.repeat(_lib.pack_bits(np.ones((1, self.k), bool)), st0.rows, axis=0))
+            self._bfs_tiles = (self.ctx.dense_alloc(st0.rows, self.k, np.int32), self._alloc(st0.rows), ones)
+        dist, zero, ones = self._bfs_tiles
+        self.ctx.bits_mark_new(st0.bufs[st0.xi], zero, dist, 0)
+        steps = 0
+        for level in range(1, int(max_steps) + 1):
+            xi = st0.xi
+            self.step()                          # reads bufs[xi], leaves the result in bufs[1 - xi]
+            steps = level
+            if self.ctx.bits_mark_new(st0.bufs[1 - xi], st0.bufs[xi], dist, level) == 0:
+                break
+        self.last_bfs_steps = steps
+        # every element reached in this call was written by it; the others (clear in the final bits) become -1
+        self.ctx.bits_mark_new(ones, st0.bufs[st0.xi], dist, -1)
+        return dist.d2h(out)
+
     # -- streaming iteration for host-resident features ------------------------------------------------------
     def stream_step(self, X_host: np.ndarray, out_host: np.ndarray):
         """Enqueue one full iteration on host data: upload ``X_host`` -> ``step()`` -> download level-0 result
@@ -420,6 +479,8 @@ class ArrowEngine:
         (side copy streams ordered with events, two device slots).  Both arrays must be pinned
         (``_lib.PinnedArray``) of the engine's dtype and must stay untouched until ``stream_drain()``; use at least two
         (X, out) pairs in rotation.  Results are identical to ``set_features(X); step(); result()``."""
+        if self.bits:
+            raise ValueError("stream_step moves float tiles; the or_and engine steps on device-resident bits only")
         st = self.levels[0]
         if X_host.shape != (st.rows, self.k) or out_host.shape != (st.rows, self.k):
             raise ValueError(f"expected host arrays of shape {(st.rows, self.k)}")
@@ -458,17 +519,24 @@ class ArrowEngine:
         """one ⊗ and one ⊕ per term, in every semiring"""
         return 2.0 * self.total_nnz * self.k
 
+    def _entry_and_row_bytes(self) -> Tuple[int, float]:
+        """bytes per non-zero (index + value; index only in or_and) and per feature row (k*e; the row's words in or_and)"""
+        if self.bits:
+            return 4, 4.0 * _lib.b1_words(self.k)
+        e = self.dtype.itemsize
+        return 4 + e, float(self.k * e)
+
     def algorithmic_bytes_per_step(self) -> float:
         """Per level nnz*(4+e) + (R+1)*4 + U*k*e + R*k*e (U = R = active rows, e = 4 or 8 bytes per element), plus the
         exchanges (forward 2 passes, backward 3 passes over the routed rows) -- the figure a fused implementation still
-        reports against."""
-        e = self.dtype.itemsize
+        reports against.  In ``or_and`` a non-zero is its 4-byte index and a row its words."""
+        nz, row = self._entry_and_row_bytes()
         total = 0.0
         for j, st in enumerate(self.levels):
-            total += st.nnz * (4 + e) + (st.rows + 1) * 4 + 2.0 * st.rows * self.k * e
+            total += st.nnz * nz + (st.rows + 1) * 4 + 2.0 * st.rows * row
             if j > 0:
                 m = int(np.count_nonzero(st.to_prev < self.levels[j - 1].rows))
-                total += 5.0 * m * self.k * e
+                total += 5.0 * m * row
         return total
 
     def _launch_level_as_in_step(self, j: int, src, dst):
@@ -486,7 +554,7 @@ class ArrowEngine:
         if j > 0 and self.mode == "fused":
             raise ValueError("levels > 0 are timed through step() in fused mode")
         src = st.bufs[st.xi]
-        scratch = self.ctx.dense_alloc(st.rows, self.k, self.dtype)
+        scratch = self._alloc(st.rows)
         for _ in range(warmup):
             self._launch_level_as_in_step(j, src, scratch)
         self.ctx.timer_start(5)
@@ -500,17 +568,18 @@ class ArrowEngine:
     def level_bytes(self, j: int) -> float:
         """algorithmic bytes of level ``j``'s launch: nnz*(4+e) + (R+1)*4 + R*k*e (X) + R*k*e (C) with e = 4 or 8 bytes
         per element, plus -- when the launch carries the epilogue gather-add -- one read of the routed rows of the deeper
-        level's tile (the other two passes of the reference's backward exchange do not exist in this launch)"""
-        e = self.dtype.itemsize
+        level's tile (the other two passes of the reference's backward exchange do not exist in this launch).  In
+        ``or_and`` a non-zero is its 4-byte index and a row its words."""
+        nz, row = self._entry_and_row_bytes()
         st = self.levels[j]
-        b = st.nnz * (4 + e) + (st.rows + 1) * 4 + 2.0 * st.rows * self.k * e
+        b = st.nnz * nz + (st.rows + 1) * 4 + 2.0 * st.rows * row
         if self.mode == "fused" and self.fused_style == "gather" and j + 1 < self.L:
             nxt = self.levels[j + 1]
-            b += float(np.count_nonzero(nxt.to_prev < st.rows)) * self.k * e
+            b += float(np.count_nonzero(nxt.to_prev < st.rows)) * row
         return b
 
     def close(self):
-        for b in (self._wit_labels or []) + list(self._wit_values.values()):
+        for b in (self._wit_labels or []) + list(self._wit_values.values()) + list(self._bfs_tiles or ()):
             b.free()
-        self._wit_labels, self._wit_values = None, {}
+        self._wit_labels, self._wit_values, self._bfs_tiles = None, {}, None
         self.ctx.close()

@@ -14,7 +14,7 @@
  * arrow_last_error), no exceptions cross the boundary.  The caller owns host memory; the library
  * owns device memory (handles are small non-negative ints, valid for one context).  All work is
  * stream-ordered on the context's stream; arrow_sync() waits for it.  One host thread per context.
- * Dense tiles are row-major [rows x k] of fp32 or fp64 (or int32 labels); CSR is fp32 or fp64 values with int32 indices
+ * Dense tiles are row-major [rows x k] of fp32 or fp64 (or int32 labels, or bits); CSR is fp32 or fp64 values with int32 indices
  * on the device.
  * The precision is fixed when a tile is allocated / a block uploaded (ARROW_F32 / ARROW_F64), and every operand of one
  * launch has the same precision.  fp64 covers the one-GPU product (arrow_spmm, arrow_spmm_add, arrow_gather_rows); the
@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 6
+#define ARROW_ABI_VERSION 7
 
 /* error codes */
 #define ARROW_OK              0
@@ -49,6 +49,12 @@ typedef struct arrow_ctx arrow_ctx;
 #define ARROW_I32             2   /* dense tiles only: labels / parents of arrow_spmm_sr_witness.  Allocation, free, h2d / d2h
                                      (and the lane copies), copy and arrow_dense_dtype accept it; every arithmetic launch
                                      refuses an int32 operand with ARROW_ERR_ARG */
+#define ARROW_B1              3   /* dense tiles only: bits, column c of a row is bit c % 32 of uint32 word c / 32; a row is
+                                     one word for k <= 32, else ((k + 31) / 32 rounded up to a multiple of 4) words (16-byte
+                                     vectors), and host rows of h2d / d2h have that layout.  Allocation zero-fills (padding bits stay 0 under every
+                                     launch), free, h2d / d2h (and the lane copies), copy, ptr, dtype and fill with 0 accept it;
+                                     the (or, and) launches below run on it; every other arithmetic or multi-GPU launch refuses a
+                                     bit operand with ARROW_ERR_ARG */
 
 /* flags for arrow_spmm / arrow_gather_rows */
 #define ARROW_ACCUMULATE      1   /* C += ... instead of C = ...  (reference: `C_i += A_i0 @ X_0`,
@@ -220,14 +226,22 @@ int  arrow_gather_rows(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int fl
 #define ARROW_SR_PLUS_TIMES 0
 #define ARROW_SR_MIN_PLUS   1
 #define ARROW_SR_MAX_PLUS   2
+#define ARROW_SR_OR_AND     3   /* the boolean semiring on ARROW_B1 tiles (k <= 8192, else ARROW_ERR_UNSUPPORTED): ⊗ is "the
+                                   entry exists" (the block's values, of either precision, are not read), ⊕ is OR.  Every
+                                   operand is a bit tile, else ARROW_ERR_ARG; a bit operand with another semiring: ARROW_ERR_ARG.
+                                   arrow_gather_rows without ARROW_ACCUMULATE moves bit rows (with it: ARROW_ERR_ARG) */
 /* C[r] = (⊕_p A[r,p] ⊗ X[col_p]) ⊕ add[add_map[r]]  (add_buf / add_map may be -1; rows with add_map[r] == -1 get the
  * product only; a row without entries, or whose entries are all skipped columns, gets the ⊕ identity) */
 int  arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, int add_map, int semiring);
 /* dst[r] = dst[r] ⊕ src[map[r]] for map[r] >= 0 (the backward exchange of a semiring step) */
 int  arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int semiring);
 /* number of rows of two equally shaped tiles (same rows, k and element type) that differ in some element, compared by
- * value (-0 == +0, NaN != NaN); synchronises the context's current lane */
+ * value (-0 == +0, NaN != NaN; bit tiles over their k columns); synchronises the context's current lane */
 int  arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed);
+/* BFS level record of the (or, and) step: dist[r, c] = level for every (r, c < k) whose bit is set in new_buf and clear in
+ * old_buf (bit tiles); every other element of dist_buf (ARROW_I32, same rows and k) is left alone.  *n_new = the number of
+ * such bits (0: the step reached its fixed point); synchronises the context's current lane. */
+int  arrow_bits_mark_new(arrow_ctx *ctx, int new_buf, int old_buf, int dist_buf, int level, int64_t *n_new);
 
 /* ---- predecessors of the tropical semirings (one GPU, fp32) ------------------------------------------ */
 /* The product of arrow_spmm_sr over (value, label) pairs.  A candidate of row r is an entry p whose column c is valid
