@@ -47,8 +47,10 @@ EXPORTS = [
     "arrow_csr_upload_f64", "arrow_dense_alloc_dtype", "arrow_dense_dtype",
     "arrow_spmm_sr", "arrow_gather_rows_sr", "arrow_dense_count_diff",
     "arrow_spmm_sr_witness", "arrow_tile_rows", "arrow_tile_rows_rule", "arrow_bits_mark_new",
+    "arrow_adj_build", "arrow_adj_free", "arrow_adj_info", "arrow_adj_d2h", "arrow_bits_mark_frontier",
+    "arrow_bits_push_frontier",
 ]
-ABI_VERSION = 7         # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 8        # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -150,6 +152,12 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_tile_rows": (c_int, [P, I, I, pI]),
         "arrow_tile_rows_rule": (c_int, [I, I, I64, I, I]),
         "arrow_bits_mark_new": (c_int, [P, I, I, I, I, pI64]),
+        "arrow_adj_build": (c_int, [P, I, pI, pI, I64, pI]),
+        "arrow_adj_free": (c_int, [P, I]),
+        "arrow_adj_info": (c_int, [P, I, pI64, pI64]),
+        "arrow_adj_d2h": (c_int, [P, I, P, P]),
+        "arrow_bits_mark_frontier": (c_int, [P, I, I, I, I, I, pI64, pI64, pI64]),
+        "arrow_bits_push_frontier": (c_int, [P, I, I, I]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -458,6 +466,30 @@ class Context:
         self._check(self.lib.arrow_bits_mark_new(self._h, new.h, old.h, dist.h, int(level), byref(n)))
         return int(n.value)
 
+    def adj_build(self, parts: Sequence[tuple], n_vertices: int) -> "Adjacency":
+        """The push adjacency of a BFS (``arrow_adj_build``): ``parts`` is a sequence of ``(Csr, RowMap or None)``; entry
+        (r, c) of a block gives the edge map(c) -> map(r) (None: the identity), edges with an end at -1 and u == v are
+        dropped.  Synchronises."""
+        n = len(parts)
+        csrs = (c_int * max(n, 1))(*[A.h for A, _ in parts])
+        maps = (c_int * max(n, 1))(*[m.h if m is not None else -1 for _, m in parts])
+        h = c_int()
+        self._check(self.lib.arrow_adj_build(self._h, n, csrs, maps, int(n_vertices), byref(h)))
+        return Adjacency(self, h.value)
+
+    def bits_mark_frontier(self, adj: "Adjacency", new: "Dense", old: "Dense", dist: "Dense", level: int):
+        """``bits_mark_new`` that also records in ``adj`` the rows with a fresh bit (``arrow_bits_mark_frontier``); returns
+        (fresh bits, frontier rows, frontier edges); synchronises"""
+        n, rows, edges = c_int64(), c_int64(), c_int64()
+        self._check(self.lib.arrow_bits_mark_frontier(self._h, adj.h, new.h, old.h, dist.h, int(level), byref(n),
+                                                      byref(rows), byref(edges)))
+        return int(n.value), int(rows.value), int(edges.value)
+
+    def bits_push_frontier(self, adj: "Adjacency", x: "Dense", out: "Dense"):
+        """out = x, then out[v] |= x[u] along the adjacency's edges of the recorded frontier rows u
+        (``arrow_bits_push_frontier``); ``x`` must be the tile of the last ``bits_mark_frontier`` on ``adj``"""
+        self._check(self.lib.arrow_bits_push_frontier(self._h, adj.h, x.h, out.h))
+
     def count_diff(self, a: "Dense", b: "Dense") -> int:
         """rows in which two equally shaped tiles differ in some element (-0 == +0, NaN != NaN); synchronises"""
         n = c_int64()
@@ -577,6 +609,26 @@ class RowMap(_Handle):
 
     def free(self):
         self._free("arrow_map_free")
+
+
+class Adjacency(_Handle):
+    """push adjacency of a BFS (``arrow_adj_build``): a CSR without values, row u listing the destinations v of u"""
+
+    def info(self):
+        n, m = c_int64(), c_int64()
+        self.ctx._check(self.ctx.lib.arrow_adj_info(self.ctx._h, self.h, byref(n), byref(m)))
+        return {"n_vertices": int(n.value), "n_edges": int(m.value)}
+
+    def d2h(self):
+        """(indptr, indices) as int32 host arrays"""
+        inf = self.info()
+        indptr = np.empty(inf["n_vertices"] + 1, np.int32)
+        indices = np.empty(inf["n_edges"], np.int32)
+        self.ctx._check(self.ctx.lib.arrow_adj_d2h(self.ctx._h, self.h, _ptr(indptr), _ptr(indices)))
+        return indptr, indices
+
+    def free(self):
+        self._free("arrow_adj_free")
 
 
 class PtrTable(_Handle):

@@ -24,6 +24,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <cub/device/device_radix_sort.cuh>
+
 #include <algorithm>
 #include <map>
 #include <mutex>
@@ -98,6 +100,19 @@ struct PtrTable {                     // one device pointer per row: where a SpM
     bool live = false;
 };
 
+struct Adj {                          // push adjacency of the (or, and) BFS (arrow_adj_build) and its frontier record
+    int64_t n = 0, m = 0;             // vertices (level-0 rows), edges
+    int *indptr = nullptr;            // device: n + 1 row pointers of the transposed matrix (row u: destinations v)
+    int *indices = nullptr;           // device: m destinations
+    int *front_rows = nullptr;        // device, n: rows of the last arrow_bits_mark_frontier, in list order
+    int *front_off = nullptr;         // device, n: first edge offset of each of them, increasing with the list position
+    int64_t n_front = 0, front_edges = 0;
+    int tag = -1;                     // dense handle whose fresh rows the record holds (-1: no record)
+    const void *tag_p = nullptr;      // and its storage and width (a freed and re-used handle does not match)
+    int tag_k = 0;
+    bool live = false;
+};
+
 thread_local std::string g_create_error;
 std::mutex g_numa_mu;                         // arrow_host_alloc_numa bookkeeping (pointer -> mapped length)
 std::map<void *, size_t> g_numa_allocs;
@@ -114,6 +129,7 @@ struct arrow_ctx {
     std::vector<DenseBuf> dense;
     std::vector<Csr> csrs;
     std::vector<IdxMap> maps;
+    std::vector<Adj> adjs;
     Timer timers[ARROW_MAX_TIMERS];
     int64_t launches = 0;
     int long_threshold = 512;
@@ -210,6 +226,10 @@ IdxMap *get_map(arrow_ctx *ctx, int h) {
     if (h < 0 || h >= (int)ctx->maps.size() || !ctx->maps[h].live) return nullptr;
     return &ctx->maps[h];
 }
+Adj *get_adj(arrow_ctx *ctx, int h) {
+    if (h < 0 || h >= (int)ctx->adjs.size() || !ctx->adjs[h].live) return nullptr;
+    return &ctx->adjs[h];
+}
 
 inline int ceil_div_i64(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
@@ -249,6 +269,14 @@ void csr_release(Csr &c) {
         for (int4 *p : c.tiles) cudaFree(p);
     }
     c = Csr();
+}
+
+void adj_release(Adj &a) {
+    cudaFree(a.indptr);
+    cudaFree(a.indices);
+    cudaFree(a.front_rows);
+    cudaFree(a.front_off);
+    a = Adj();
 }
 
 struct DevTmp {                       // scratch allocation released on every exit path
@@ -3140,6 +3168,200 @@ int gather_rows_or(arrow_ctx *ctx, DenseBuf *D, const DenseBuf *S, const IdxMap 
 }
 
 // ------------------------------------------------------------------------------------------------
+// direction-optimising BFS on bit tiles.  With add_identity a fused (or, and) step is X' = X | M X, M the level-0 x level-0
+// union of every level's entries (r, c) as edges cmap_j(c) -> cmap_j(r).  Inside a BFS, where X_h = X_{h-1} | M X_{h-1},
+// the next level is X_h | M F_h with F_h the rows holding a bit of X_h & ~X_{h-1}: a push of the frontier rows along the
+// transposed matrix (arrow_adj_build) gives the pull step's bits exactly, for the cost of the frontier's edges.
+// ------------------------------------------------------------------------------------------------
+struct AdjPart {
+    const int *__restrict__ indptr;
+    const int *__restrict__ indices;
+    const int *__restrict__ map;      // nullptr: the identity
+    long long nnz;
+    int n_rows;
+};
+
+// the largest i in [lo, hi] with a[i] <= e (a non-decreasing, a[lo] <= e): the row of entry e given row pointers, the
+// frontier row of edge slot e given first edge offsets (rows without entries share their offset with the next row)
+__device__ __forceinline__ int last_le(const int *__restrict__ a, int lo, int hi, long long e) {
+    while (lo < hi) {
+        const int mid = (int)(((long long)lo + hi + 1) >> 1);
+        if ((long long)__ldg(a + mid) <= e) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// edges of one block: entry (r, c) with c >= 0 gives u -> v = map(c) -> map(r); an end at -1 or u == v drops it.  Counts
+// them into *count; with `keys` also appends (u << 32) | v at a warp-aggregated cursor (the order is fixed by the sort).
+__global__ void __launch_bounds__(256) k_adj_edges(AdjPart p, unsigned long long *__restrict__ count,
+                                                   unsigned long long *__restrict__ keys) {
+    const int lane = threadIdx.x & 31;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long e0 = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31); e0 < p.nnz; e0 += stride) {
+        const long long e = e0 + lane;
+        bool ok = false;
+        unsigned long long key = 0;
+        if (e < p.nnz) {
+            const int c = __ldg(p.indices + e);
+            if (c >= 0) {
+                const int r = last_le(p.indptr, 0, p.n_rows - 1, e);
+                const int u = p.map ? __ldg(p.map + c) : c;
+                const int v = p.map ? __ldg(p.map + r) : r;
+                ok = u >= 0 && v >= 0 && u != v;
+                key = ((unsigned long long)(unsigned)u << 32) | (unsigned)v;
+            }
+        }
+        const unsigned ball = __ballot_sync(0xffffffffu, ok);
+        if (ball == 0u) continue;
+        unsigned long long base = 0;
+        if (lane == 0) base = atomicAdd(count, (unsigned long long)__popc(ball));
+        if (keys != nullptr) {
+            base = __shfl_sync(0xffffffffu, base, 0);
+            if (ok) keys[base + __popc(ball & ((1u << lane) - 1u))] = key;
+        }
+    }
+}
+
+// the CSR of the sorted keys: indices[e] = v of key e, indptr[u] = the first key of row u (lower bound of u << 32)
+__global__ void __launch_bounds__(256) k_adj_csr(const unsigned long long *__restrict__ keys, long long m, long long n,
+                                                 int *__restrict__ indptr, int *__restrict__ indices) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (long long e = t; e < m; e += stride) indices[e] = (int)(unsigned)keys[e];
+    for (long long u = t; u <= n; u += stride) {
+        const unsigned long long want = (unsigned long long)u << 32;
+        long long lo = 0, hi = m;
+        while (lo < hi) {
+            const long long mid = (lo + hi) >> 1;
+            if (keys[mid] < want) lo = mid + 1;
+            else hi = mid;
+        }
+        indptr[u] = (int)lo;
+    }
+}
+
+constexpr int MARK_THREADS = 256;
+
+// k_bits_mark_new's level record and bit count, a thread per row, plus the frontier record: the rows with a fresh bit in a
+// column < k, listed with their first edge offset in the push adjacency.  A CTA scans (1 << 32) + degree over its rows and
+// claims its slice of the list with one 64-bit atomicAdd on counts[1], so list positions (high half) and edge offsets (low
+// half) come from the same add and increase together; the edge sum stays below 2^31 and never carries into the rows.
+__global__ void __launch_bounds__(MARK_THREADS) k_bits_mark_frontier(const unsigned int *__restrict__ nw,
+                                                                     const unsigned int *__restrict__ old,
+                                                                     int *__restrict__ dist, long long rows, int k, int words,
+                                                                     int level, const int *__restrict__ adj_ptr,
+                                                                     int *__restrict__ front_rows, int *__restrict__ front_off,
+                                                                     unsigned long long *__restrict__ counts) {
+    constexpr int WARPS = MARK_THREADS / 32;
+    __shared__ unsigned long long s_warp[WARPS];
+    __shared__ unsigned long long s_base;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int used = (k + 31) / 32;
+    unsigned long long mine = 0;
+    for (long long r0 = (long long)blockIdx.x * MARK_THREADS; r0 < rows; r0 += (long long)gridDim.x * MARK_THREADS) {
+        const long long r = r0 + threadIdx.x;
+        unsigned long long claim = 0;
+        if (r < rows) {
+            bool any = false;
+            for (int w = 0; w < used; ++w) {
+                unsigned int fresh = nw[r * words + w] & ~old[r * words + w] & bit_col_mask(w, k);
+                any |= fresh != 0u;
+                mine += (unsigned long long)__popc(fresh);
+                int *drow = dist + r * k + w * 32;
+                while (fresh) {
+                    const int c = __ffs(fresh) - 1;
+                    drow[c] = level;
+                    fresh &= fresh - 1u;
+                }
+            }
+            if (any) claim = (1ull << 32) | (unsigned)(__ldg(adj_ptr + r + 1) - __ldg(adj_ptr + r));
+        }
+        unsigned long long incl = claim;                      // inclusive scan over the warp
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, incl, off);
+            if (lane >= off) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned long long total = 0;
+            for (int i = 0; i < WARPS; ++i) {
+                const unsigned long long t = s_warp[i];
+                s_warp[i] = total;
+                total += t;
+            }
+            s_base = total ? atomicAdd(counts + 1, total) : 0ull;
+        }
+        __syncthreads();
+        if (claim) {
+            const unsigned long long at = s_base + s_warp[warp] + incl - claim;
+            front_rows[at >> 32] = (int)r;
+            front_off[at >> 32] = (int)(unsigned)at;
+        }
+        __syncthreads();                                      // s_warp / s_base are rewritten by the next pass
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, off);
+    if (lane == 0 && mine) atomicAdd(counts, mine);
+}
+
+__device__ __forceinline__ void red_or_b32(unsigned *p, unsigned v) {
+    asm volatile("red.global.or.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void red_or_b64(unsigned long long *p, unsigned long long v) {
+    asm volatile("red.global.or.b64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+// out[vec] |= x, skipping zero words: one 32-bit OR for a one-word row, two 64-bit ORs for a 16-byte vector of a padded row
+__device__ __forceinline__ void push_or(unsigned *out, long long vec, unsigned x) {
+    if (x) red_or_b32(out + vec, x);
+}
+__device__ __forceinline__ void push_or(unsigned *out, long long vec, const uint4 &x) {
+    unsigned long long *p = reinterpret_cast<unsigned long long *>(out + 4 * vec);
+    if (x.x | x.y) red_or_b64(p, ((unsigned long long)x.y << 32) | x.x);
+    if (x.z | x.w) red_or_b64(p + 1, ((unsigned long long)x.w << 32) | x.z);
+}
+
+constexpr int PUSH_THREADS = 256, PUSH_ITEMS = 4;
+
+// out[v] |= x[u] along every edge u -> v of the recorded frontier rows.  An item is (edge slot e, vector q of the row's
+// first `vecs` vectors, those that hold columns < k); a CTA walks chunks of PUSH_THREADS * PUSH_ITEMS consecutive items, so
+// a hub row's edges spread over many CTAs.  The frontier rows of a chunk come from one binary search over the record's
+// edge offsets, each item's row from a search between them.
+template <class V>
+__global__ void __launch_bounds__(PUSH_THREADS) k_bits_push(const V *__restrict__ x, unsigned *__restrict__ out,
+                                                            const int *__restrict__ adj_ptr, const int *__restrict__ adj_idx,
+                                                            const int *__restrict__ front_rows,
+                                                            const int *__restrict__ front_off, int n_front, long long n_items,
+                                                            int vecs, int row_vecs) {
+    constexpr long long CHUNK = (long long)PUSH_THREADS * PUSH_ITEMS;
+    __shared__ int s_lo, s_hi;
+    for (long long c0 = (long long)blockIdx.x * CHUNK; c0 < n_items; c0 += (long long)gridDim.x * CHUNK) {
+        if (threadIdx.x == 0) {
+            const long long c1 = (c0 + CHUNK < n_items ? c0 + CHUNK : n_items) - 1;
+            s_lo = last_le(front_off, 0, n_front - 1, c0 / vecs);
+            s_hi = last_le(front_off, s_lo, n_front - 1, c1 / vecs);
+        }
+        __syncthreads();
+        const int lo = s_lo, hi = s_hi;
+#pragma unroll
+        for (int j = 0; j < PUSH_ITEMS; ++j) {
+            const long long i = c0 + j * PUSH_THREADS + threadIdx.x;
+            if (i < n_items) {
+                const long long e = i / vecs;
+                const int q = (int)(i - e * vecs);
+                const int p = last_le(front_off, lo, hi, e);
+                const int u = __ldg(front_rows + p);
+                const int v = __ldg(adj_idx + __ldg(adj_ptr + u) + (int)(e - __ldg(front_off + p)));
+                push_or(out, (long long)v * row_vecs + q, x[(long long)u * row_vecs + q]);
+            }
+        }
+        __syncthreads();                                      // s_lo / s_hi are rewritten by the next chunk
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // predecessors of the tropical semirings: the product of arrow_spmm_sr carried over (value, label) pairs.  A candidate
 // of row r is an entry p with a valid column c != self(r); its value is fl(A[r,p] + X[c]) and its label is c.  Pairs are
 // ⊕-reduced lexicographically: the better value wins (smaller for (min, +), larger for (max, +)), equal values (by value,
@@ -3616,6 +3838,8 @@ void arrow_ctx_destroy(arrow_ctx *ctx) {
         if (c.live) csr_release(c);
     for (auto &m : ctx->maps)
         if (m.live) cudaFree(m.p);
+    for (auto &a : ctx->adjs)
+        if (a.live) adj_release(a);
     for (auto &t : ctx->timers) {
         if (t.a) cudaEventDestroy(t.a);
         if (t.b) cudaEventDestroy(t.b);
@@ -4823,6 +5047,217 @@ int arrow_bits_mark_new(arrow_ctx *ctx, int new_buf, int old_buf, int dist_buf, 
     CUDA_TRY(ctx, cudaMemcpyAsync(&h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(stream));
     *n_new = (int64_t)h;
+    return ARROW_OK;
+}
+
+int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    if (!adj_out || n_parts < 0 || (n_parts > 0 && (!csrs || !maps)) || n_vertices < 0)
+        return fail(ctx, ARROW_ERR_ARG, "bad arguments (n_parts=%d, n_vertices=%lld)", n_parts, (long long)n_vertices);
+    if (n_vertices > 2147483646LL) return fail(ctx, ARROW_ERR_RANGE, "%lld vertices exceed the int32 device layout", (long long)n_vertices);
+    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_adj_build allocates and synchronises: not during graph capture");
+    std::vector<AdjPart> parts;
+    for (int i = 0; i < n_parts; ++i) {
+        const Csr *c = get_csr(ctx, csrs[i]);
+        if (!c) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad csr handle %d", i, csrs[i]);
+        const IdxMap *m = nullptr;
+        if (maps[i] != -1) {
+            m = get_map(ctx, maps[i]);
+            if (!m) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad map handle %d", i, maps[i]);
+            if (m->n < std::max(c->n_rows, c->n_cols))
+                return fail(ctx, ARROW_ERR_ARG, "part %d: the map has %lld entries, the block %lld rows and %lld columns", i,
+                            (long long)m->n, (long long)c->n_rows, (long long)c->n_cols);
+            if (m->limit > n_vertices)
+                return fail(ctx, ARROW_ERR_ARG, "part %d: the map reaches row %lld, there are %lld vertices", i,
+                            (long long)m->limit, (long long)n_vertices);
+        } else if (c->n_rows > n_vertices || c->n_cols > n_vertices) {
+            return fail(ctx, ARROW_ERR_ARG, "part %d: a %lld x %lld block with the identity map exceeds %lld vertices", i,
+                        (long long)c->n_rows, (long long)c->n_cols, (long long)n_vertices);
+        }
+        if (c->nnz > 0) parts.push_back(AdjPart{c->indptr, c->indices, m ? m->p : nullptr, (long long)c->nnz, (int)c->n_rows});
+    }
+    cudaStream_t s = ctx->stream;
+    auto edge_grid = [&](long long nnz) { return (int)std::min<long long>((nnz + 255) / 256, (long long)ctx->sm_count * 8); };
+    DevTmp cnt;
+    unsigned long long m = 0;
+    CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof(unsigned long long)));
+    unsigned long long *count = reinterpret_cast<unsigned long long *>(cnt.p);
+    CUDA_TRY(ctx, cudaMemsetAsync(count, 0, sizeof m, s));
+    for (const AdjPart &p : parts) {
+        k_adj_edges<<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
+        ctx->launches++;
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    CUDA_TRY(ctx, cudaMemcpyAsync(&m, count, sizeof m, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    if (m > 2147483647ULL) return fail(ctx, ARROW_ERR_RANGE, "%llu edges exceed the int32 device layout", m);
+
+    Adj a;
+    a.n = n_vertices;
+    a.m = (int64_t)m;
+    cudaError_t e = cudaMalloc(&a.indptr, (size_t)(n_vertices + 1) * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&a.indices, (size_t)std::max<unsigned long long>(m, 1) * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&a.front_rows, (size_t)std::max<int64_t>(n_vertices, 1) * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&a.front_off, (size_t)std::max<int64_t>(n_vertices, 1) * 4);
+    DevTmp keys, alt, temp;             // build scratch: 16 bytes per edge and the sort's temporary storage
+    const unsigned long long *sorted = nullptr;
+    if (e == cudaSuccess && m > 0) {
+        e = cudaMalloc(&keys.p, (size_t)m * 8);
+        if (e == cudaSuccess) e = cudaMalloc(&alt.p, (size_t)m * 8);
+        if (e == cudaSuccess) e = cudaMemsetAsync(count, 0, sizeof m, s);
+        if (e == cudaSuccess) {
+            for (const AdjPart &p : parts) {
+                k_adj_edges<<<edge_grid(p.nnz), 256, 0, s>>>(p, count, reinterpret_cast<unsigned long long *>(keys.p));
+                ctx->launches++;
+            }
+            e = cudaGetLastError();
+        }
+        int end_bit = 33;                                     // keys are (u << 32) | v with u < n_vertices
+        while (end_bit < 64 && (1LL << (end_bit - 32)) < n_vertices) ++end_bit;
+        cub::DoubleBuffer<unsigned long long> db(reinterpret_cast<unsigned long long *>(keys.p),
+                                                 reinterpret_cast<unsigned long long *>(alt.p));
+        size_t temp_bytes = 0;
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, db, (int)m, 0, end_bit, s);
+        if (e == cudaSuccess) e = cudaMalloc(&temp.p, std::max<size_t>(temp_bytes, 1));
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(temp.p, temp_bytes, db, (int)m, 0, end_bit, s);
+        sorted = db.Current();
+    }
+    if (e == cudaSuccess) {
+        const long long work = std::max<long long>((long long)m, n_vertices + 1);
+        k_adj_csr<<<edge_grid(work), 256, 0, s>>>(sorted, (long long)m, n_vertices, a.indptr, a.indices);
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        adj_release(a);
+        return fail(ctx, e == cudaErrorMemoryAllocation ? ARROW_ERR_NOMEM : ARROW_ERR_CUDA, "adjacency build failed: %s",
+                    cudaGetErrorString(e));
+    }
+    a.live = true;
+    const int h = new_slot(ctx->adjs);
+    ctx->adjs[h] = a;
+    *adj_out = h;
+    return ARROW_OK;
+}
+
+int arrow_adj_free(arrow_ctx *ctx, int adj) {
+    CHECK_CTX(ctx);
+    Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    adj_release(*a);
+    return ARROW_OK;
+}
+
+int arrow_adj_info(arrow_ctx *ctx, int adj, int64_t *n_vertices, int64_t *n_edges) {
+    CHECK_CTX(ctx);
+    const Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (n_vertices) *n_vertices = a->n;
+    if (n_edges) *n_edges = a->m;
+    return ARROW_OK;
+}
+
+int arrow_adj_d2h(arrow_ctx *ctx, int adj, int32_t *indptr, int32_t *indices) {
+    CHECK_CTX(ctx);
+    const Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (!indptr || (a->m > 0 && !indices)) return fail(ctx, ARROW_ERR_ARG, "null host buffer");
+    CUDA_TRY(ctx, cudaMemcpyAsync(indptr, a->indptr, (size_t)(a->n + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    if (a->m > 0) CUDA_TRY(ctx, cudaMemcpyAsync(indices, a->indices, (size_t)a->m * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    return ARROW_OK;
+}
+
+int arrow_bits_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int dist_buf, int level, int64_t *n_new,
+                             int64_t *frontier_rows, int64_t *frontier_edges) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    DenseBuf *N = get_dense(ctx, new_buf), *O = get_dense(ctx, old_buf), *D = get_dense(ctx, dist_buf);
+    if (!N || !O || !D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (new=%d old=%d dist=%d)", new_buf, old_buf, dist_buf);
+    if (!n_new || !frontier_rows || !frontier_edges) return fail(ctx, ARROW_ERR_ARG, "null output");
+    if (N->dtype != ARROW_B1 || O->dtype != ARROW_B1 || D->dtype != ARROW_I32)
+        return fail(ctx, ARROW_ERR_ARG, "new / old are bit tiles and dist an int32 tile: got %s / %s / %s", dtype_name(N->dtype),
+                    dtype_name(O->dtype), dtype_name(D->dtype));
+    if (N->rows != O->rows || N->k != O->k || D->rows != N->rows || D->k != N->k || N->rows != a->n)
+        return fail(ctx, ARROW_ERR_ARG, "tiles differ in shape: new %lld x %d, old %lld x %d, dist %lld x %d, adjacency %lld rows",
+                    (long long)N->rows, N->k, (long long)O->rows, O->k, (long long)D->rows, D->k, (long long)a->n);
+    *n_new = *frontier_rows = *frontier_edges = 0;
+    a->tag = -1;                                              // the record is rewritten below
+    cudaStream_t stream = cur_stream(ctx);
+    unsigned long long h[2] = {0, 0};                         // fresh bits, (frontier rows << 32) | frontier edges
+    if (N->rows > 0) {
+        DevTmp cnt;
+        CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof h));
+        CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof h, stream));
+        const int grid = (int)std::max<long long>(1, std::min<long long>((N->rows + MARK_THREADS - 1) / MARK_THREADS,
+                                                                         (long long)ctx->sm_count * 8));
+        k_bits_mark_frontier<<<grid, MARK_THREADS, 0, stream>>>(reinterpret_cast<const unsigned int *>(N->p),
+                                                                reinterpret_cast<const unsigned int *>(O->p),
+                                                                reinterpret_cast<int *>(D->p), N->rows, N->k, bit_row_words(N->k),
+                                                                level, a->indptr, a->front_rows, a->front_off,
+                                                                reinterpret_cast<unsigned long long *>(cnt.p));
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+        CUDA_TRY(ctx, cudaMemcpyAsync(h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+    }
+    a->n_front = (int64_t)(h[1] >> 32);
+    a->front_edges = (int64_t)(h[1] & 0xffffffffULL);
+    a->tag = new_buf;
+    a->tag_p = N->p;
+    a->tag_k = N->k;
+    *n_new = (int64_t)h[0];
+    *frontier_rows = a->n_front;
+    *frontier_edges = a->front_edges;
+    return ARROW_OK;
+}
+
+int arrow_bits_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    const Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    DenseBuf *X = get_dense(ctx, x_buf), *O = get_dense(ctx, out_buf);
+    if (!X || !O) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x=%d out=%d)", x_buf, out_buf);
+    if (X->dtype != ARROW_B1 || O->dtype != ARROW_B1)
+        return fail(ctx, ARROW_ERR_ARG, "x / out are bit tiles: got %s / %s", dtype_name(X->dtype), dtype_name(O->dtype));
+    if (a->tag < 0) return fail(ctx, ARROW_ERR_ARG, "no frontier record: run arrow_bits_mark_frontier on the adjacency first");
+    if (x_buf != a->tag || X->p != a->tag_p || X->k != a->tag_k)
+        return fail(ctx, ARROW_ERR_ARG, "x (tile %d) is not the tile of the last arrow_bits_mark_frontier (tile %d)", x_buf, a->tag);
+    if (x_buf == out_buf || X->p == O->p) return fail(ctx, ARROW_ERR_ARG, "out aliases x");
+    if (X->rows != a->n || O->rows != X->rows || O->k != X->k)
+        return fail(ctx, ARROW_ERR_ARG, "shape: x %lld x %d, out %lld x %d, adjacency %lld rows", (long long)X->rows, X->k,
+                    (long long)O->rows, O->k, (long long)a->n);
+    if (X->k > BITS_MAX_K) return fail(ctx, ARROW_ERR_UNSUPPORTED, "k=%d > %d", X->k, BITS_MAX_K);
+    cudaStream_t stream = cur_stream(ctx);
+    if (X->rows == 0) return ARROW_OK;
+    CUDA_TRY(ctx, cudaMemcpyAsync(O->p, X->p, (size_t)X->rows * row_bytes(ARROW_B1, X->k), cudaMemcpyDeviceToDevice, stream));
+    if (a->front_edges == 0) return ARROW_OK;
+    const int words = bit_row_words(X->k);
+    const int row_vecs = words == 1 ? 1 : words / 4;
+    const int vecs = words == 1 ? 1 : ((X->k + 31) / 32 + 3) / 4;         // the vectors that hold columns < k
+    const long long items = a->front_edges * vecs;
+    const long long chunks = (items + (long long)PUSH_THREADS * PUSH_ITEMS - 1) / ((long long)PUSH_THREADS * PUSH_ITEMS);
+    const int per_sm = ctx->spmm_ctas_per_sm > 0 ? std::min(ctx->spmm_ctas_per_sm, 8) : 8;
+    const int sms = ctx->spmm_sm_limit > 0 ? std::min(ctx->sm_count, ctx->spmm_sm_limit) : ctx->sm_count;
+    const int grid = (int)std::min<long long>(chunks, (long long)per_sm * sms);
+    unsigned *out = reinterpret_cast<unsigned *>(O->p);
+    if (words == 1)
+        k_bits_push<unsigned><<<grid, PUSH_THREADS, 0, stream>>>(reinterpret_cast<const unsigned *>(X->p), out, a->indptr,
+                                                                 a->indices, a->front_rows, a->front_off, (int)a->n_front,
+                                                                 items, vecs, row_vecs);
+    else
+        k_bits_push<uint4><<<grid, PUSH_THREADS, 0, stream>>>(reinterpret_cast<const uint4 *>(X->p), out, a->indptr,
+                                                              a->indices, a->front_rows, a->front_off, (int)a->n_front,
+                                                              items, vecs, row_vecs);
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
     return ARROW_OK;
 }
 

@@ -52,6 +52,18 @@ _PLUS_ZERO = {_lib.SR_PLUS_TIMES: 0.0, _lib.SR_MIN_PLUS: float("inf"), _lib.SR_M
 _TIMES_ONE = {_lib.SR_PLUS_TIMES: 1.0, _lib.SR_MIN_PLUS: 0.0, _lib.SR_MAX_PLUS: 0.0, _lib.SR_OR_AND: 1.0}
 
 
+# bfs_levels(): a level is a push when its frontier's edges times this are fewer than the non-zeros a pull step gathers.
+# Beamer et al. (SC 2012) use 14.  Per level on an H100 80 GB HBM3 at 700 W (scripts/bfs_direction_bench.py, DESIGN.md §8)
+# push and pull cross at total_nnz / frontier_edges of about 7.3 on G2 at k = 128 (pull 1.42 ms, push about 60 ps per edge
+# plus the tile copy) and about 4 at k = 16; on the 10**6-vertex BA graph at k = 128 the push was faster at every level.
+BFS_PUSH_ALPHA = 8
+
+
+def bfs_direction(frontier_edges: int, total_nnz: int, alpha: float = BFS_PUSH_ALPHA) -> str:
+    """``"push"`` when ``frontier_edges * alpha < total_nnz``, else ``"pull"``: the direction of the next BFS level"""
+    return "push" if frontier_edges * alpha < total_nnz else "pull"
+
+
 def semiring_code(semiring: str, dtype, fused_style: str = "gather") -> int:
     """``_lib.SR_*`` of a semiring name; raises ``ValueError`` (before any CUDA work) for an unknown name and for the
     combinations that do not exist: the tropical and boolean semirings need a float32 decomposition and run the gather
@@ -112,6 +124,9 @@ class ArrowEngine:
         self._wit_values = {}                                    # predecessors(): value tiles of levels without a cbuf
         self._bfs_tiles: Optional[Tuple[_lib.Dense, ...]] = None   # bfs_levels(): (hop tile, all-zero and all-one bit tiles)
         self.last_bfs_steps = 0                                  # steps the last bfs_levels() call took
+        self.last_bfs_directions: List[str] = []                 # "push" / "pull" per level of the last bfs_levels()
+        self._adj: Optional[_lib.Adjacency] = None               # bfs_levels(): the push adjacency, built on first use
+        self._push_limit: Optional[int] = None                   # None: bfs_direction() decides; else push iff edges < it
         fused_ok = True
         cmap_prev = None                      # level j-1 row -> level-0 row (host, int64, -1 invalid)
         for j, (B, _) in enumerate(decomposition):
@@ -443,11 +458,22 @@ class ArrowEngine:
     def bfs_levels(self, max_steps: int, out: Optional[np.ndarray] = None) -> np.ndarray:
         """Hop levels of a multi-source BFS from the current level-0 features (int32 [n x k], level-0 row order like
         ``result()``): ``0`` where a feature bit is set now (the sources), ``h`` where the bit was first set by the
-        ``h``-th ``step()``, ``-1`` where it is never set.  Steps until a step sets no new bit, at most ``max_steps``
-        times; ``last_bfs_steps`` holds the number of steps taken.  After every step one device pass
-        (``arrow_bits_mark_new``) records the fresh bits and counts them: the level record and the fixed-point test at
-        once.  Needs ``or_and`` with ``add_identity`` (bits then only grow); raises ``ValueError`` before any CUDA work
-        otherwise.  The features end at the fixed point (``result()``); synchronises."""
+        ``h``-th level, ``-1`` where it is never set.  Takes levels until one sets no new bit, at most ``max_steps``;
+        ``last_bfs_steps`` holds the number taken.  After every level one device pass records the fresh bits and counts
+        them: the level record and the fixed-point test at once.  Needs ``or_and`` with ``add_identity`` (bits then only
+        grow); raises ``ValueError`` before any CUDA work otherwise.  The features end at the fixed point (``result()``);
+        synchronises.
+
+        Direction-optimising (DESIGN.md §4): when ``fused_ok`` holds, a level is either a ``step()`` (pull) or a push of
+        the rows that gained a bit in the previous level along the transposed operator (built on the first call, kept
+        until ``close()``), whichever :func:`bfs_direction` picks from the frontier's edges; ``last_bfs_directions`` lists
+        the choice per level.  The levels, ``last_bfs_steps``, ``result()`` / ``features()`` of level 0 and the next
+        ``step()``'s level-0 result are bit-identical to a run of pull steps only.  After a push level the tiles of the
+        levels ``j >= 1`` (``result(j)``) are not that level's product; the next ``step()`` rewrites them."""
+        return self._bfs_run(max_steps).d2h(out)
+
+    def _bfs_run(self, max_steps: int) -> _lib.Dense:
+        """the device part of ``bfs_levels``: runs the levels and returns the int32 level tile, left on the device"""
         if not self.bits:
             raise ValueError(f"bfs_levels runs the or_and semiring, the engine runs {self.semiring}")
         if not self.add_identity:
@@ -459,18 +485,46 @@ class ArrowEngine:
             ones.h2d(np.repeat(_lib.pack_bits(np.ones((1, self.k), bool)), st0.rows, axis=0))
             self._bfs_tiles = (self.ctx.dense_alloc(st0.rows, self.k, np.int32), self._alloc(st0.rows), ones)
         dist, zero, ones = self._bfs_tiles
-        self.ctx.bits_mark_new(st0.bufs[st0.xi], zero, dist, 0)
-        steps = 0
+        # an exchange-mode step of one level has no backward exchange and leaves level 0's features where they are, so a
+        # push (which advances them like a fused step) would not match it: that engine pulls every level
+        adj = self._push_adjacency() if self.fused_ok and (self.mode == "fused" or self.L > 1) else None
+        limit = self._push_limit
+
+        def mark(new, old, level):
+            """(fresh bits, push next): the level record, and the direction of the next level"""
+            if adj is None:
+                return self.ctx.bits_mark_new(new, old, dist, level), False
+            n_new, _, edges = self.ctx.bits_mark_frontier(adj, new, old, dist, level)
+            push = edges < limit if limit is not None else bfs_direction(edges, self.total_nnz) == "push"
+            return n_new, push
+
+        _, push = mark(st0.bufs[st0.xi], zero, 0)
+        steps, directions = 0, []
         for level in range(1, int(max_steps) + 1):
             xi = st0.xi
-            self.step()                          # reads bufs[xi], leaves the result in bufs[1 - xi]
+            if push:                             # X_h | M F_h, F_h the rows marked by the previous pass
+                self.ctx.bits_push_frontier(adj, st0.bufs[xi], st0.bufs[1 - xi])
+                st0.xi = st0.ci = 1 - xi
+            else:
+                self.step()                      # reads bufs[xi], leaves the result in bufs[1 - xi]
+            directions.append("push" if push else "pull")
             steps = level
-            if self.ctx.bits_mark_new(st0.bufs[1 - xi], st0.bufs[xi], dist, level) == 0:
+            n_new, push = mark(st0.bufs[1 - xi], st0.bufs[xi], level)
+            if n_new == 0:
                 break
         self.last_bfs_steps = steps
+        self.last_bfs_directions = directions
         # every element reached in this call was written by it; the others (clear in the final bits) become -1
         self.ctx.bits_mark_new(ones, st0.bufs[st0.xi], dist, -1)
-        return dist.d2h(out)
+        return dist
+
+    def _push_adjacency(self) -> _lib.Adjacency:
+        """the transposed operator of the fused step with the identity (built on the first call): every level's own block
+        with its level-j -> level-0 row map (level 0: the identity)"""
+        if self._adj is None:
+            parts = [(st.csr, st.cmap_dev) for st in self.levels]
+            self._adj = self.ctx.adj_build(parts, self.levels[0].rows)
+        return self._adj
 
     # -- streaming iteration for host-resident features ------------------------------------------------------
     def stream_step(self, X_host: np.ndarray, out_host: np.ndarray):
@@ -581,5 +635,7 @@ class ArrowEngine:
     def close(self):
         for b in (self._wit_labels or []) + list(self._wit_values.values()) + list(self._bfs_tiles or ()):
             b.free()
-        self._wit_labels, self._wit_values, self._bfs_tiles = None, {}, None
+        if self._adj is not None:
+            self._adj.free()
+        self._wit_labels, self._wit_values, self._bfs_tiles, self._adj = None, {}, None, None
         self.ctx.close()

@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 7
+#define ARROW_ABI_VERSION 8
 
 /* error codes */
 #define ARROW_OK              0
@@ -242,6 +242,33 @@ int  arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed)
  * old_buf (bit tiles); every other element of dist_buf (ARROW_I32, same rows and k) is left alone.  *n_new = the number of
  * such bits (0: the step reached its fixed point); synchronises the context's current lane. */
 int  arrow_bits_mark_new(arrow_ctx *ctx, int new_buf, int old_buf, int dist_buf, int level, int64_t *n_new);
+
+/* ---- direction-optimising BFS (one GPU, (or, and) on bit tiles) ------------------------------------------------------ */
+/* Push adjacency: a boolean n_vertices x n_vertices matrix M stored transposed, as CSR without values (row u lists every
+ * v with an edge u -> v in ascending order, duplicates kept), built on the device from n_parts blocks.  Entry (r, c) of
+ * block csrs[i] with c >= 0 gives the edge m_i(c) -> m_i(r), m_i the row map maps[i] (-1: the identity); edges with an
+ * end at -1 and edges with u == v are dropped.  With level 0's block and identity, and each level j >= 1's block with its
+ * level-j -> level-0 row map, M is the operator of the fused (or, and) step with the identity: X' = X | M X.  Temporary
+ * device memory of 16 bytes per edge is freed before the call returns; the adjacency keeps 4 (n + 1) + 4 m bytes and a
+ * frontier record of 8 n bytes.  ARROW_ERR_ARG: a map shorter than its block's rows or columns, a map or an identity
+ * block that reaches past n_vertices; ARROW_ERR_RANGE: 2^31 edges or more; ARROW_ERR_UNSUPPORTED: during graph capture.
+ * Synchronises. */
+int  arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out);
+int  arrow_adj_free(arrow_ctx *ctx, int adj);
+int  arrow_adj_info(arrow_ctx *ctx, int adj, int64_t *n_vertices, int64_t *n_edges);
+/* indptr: n_vertices + 1 entries, indices: n_edges entries */
+int  arrow_adj_d2h(arrow_ctx *ctx, int adj, int32_t *indptr, int32_t *indices);
+/* arrow_bits_mark_new (the same dist and *n_new; new_buf has the adjacency's rows), and in the same pass the frontier
+ * record of `adj`: the rows with a bit set in new_buf and clear in old_buf in one of the k columns, tagged with new_buf.
+ * *frontier_rows is their number, *frontier_edges the sum of their rows' lengths in the adjacency.  Synchronises. */
+int  arrow_bits_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int dist_buf, int level, int64_t *n_new,
+                              int64_t *frontier_rows, int64_t *frontier_edges);
+/* out = x, then out[v] |= x[u] for every recorded frontier row u and every v of adj row u (non-returning ORs; zero words
+ * are skipped).  x must be the tile of the last arrow_bits_mark_frontier on `adj`.  When X_h = X_{h-1} | M X_{h-1} and the
+ * record holds the rows of X_h & ~X_{h-1}, out = X_h | M X_h: the pull step's bits for the frontier's edges.  out may be
+ * X_{h-1}'s tile (x alone is read).  ARROW_ERR_ARG: non-bit tiles, no record, x not the recorded tile, out == x, rows
+ * other than the adjacency's, out of another shape or k; ARROW_ERR_UNSUPPORTED: k > 8192. */
+int  arrow_bits_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf);
 
 /* ---- predecessors of the tropical semirings (one GPU, fp32) ------------------------------------------ */
 /* The product of arrow_spmm_sr over (value, label) pairs.  A candidate of row r is an entry p whose column c is valid
