@@ -1289,8 +1289,14 @@ __global__ void __launch_bounds__(256) k_spmm_generic(SpmmArgs a) {
 
 // ------------------------------------------------------------------------------------------------
 // long rows (hubs of the arrow head): one CTA per segment of `segment` non-zeros, partial sums to
-// scratch, then an in-order reduction per row -- deterministic, no atomics.
+// scratch, then an in-order reduction per row -- deterministic, no atomics.  The partial kernels
+// reduce each 128-column chunk through a fixed [8 warps][128] shared array before the next chunk,
+// so their shared memory does not grow with k (a [warps][k] array passes the H100's 227 KB per
+// block at k > 7264 in fp32).  Per element the order is the same at every k: each warp's chain in
+// entry order, then warps 0..7.
 // ------------------------------------------------------------------------------------------------
+constexpr int LONG_WARPS = 8;        // 256 threads per partial CTA
+constexpr int LONG_CHUNK = 128;      // columns per chunk: 32 lanes x 4
 struct LongArgs {
     const LongTask *__restrict__ tasks;
     const int *__restrict__ indices;
@@ -1303,12 +1309,12 @@ struct LongArgs {
 };
 
 __global__ void __launch_bounds__(256) k_spmm_long_partial(LongArgs a) {
-    extern __shared__ float red[];    // [warps][k]
+    __shared__ float red[LONG_WARPS][LONG_CHUNK];
     const LongTask t = a.tasks[blockIdx.x];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-    for (int c0 = 0; c0 < a.k; c0 += 128) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int c0 = 0; c0 < a.k; c0 += LONG_CHUNK) {
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int p = t.begin + warp; p < t.end; p += nwarps) {
+        for (int p = t.begin + warp; p < t.end; p += LONG_WARPS) {
             const int c = __ldg(a.indices + p);
             const float v = __ldg(a.vals + p);
             if (c < 0) continue;
@@ -1320,16 +1326,15 @@ __global__ void __launch_bounds__(256) k_spmm_long_partial(LongArgs a) {
             }
         }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int col = c0 + lane + 32 * i;
-            if (col < a.k) red[warp * a.k + col] = acc[i];
+        for (int i = 0; i < 4; ++i) red[warp][lane + 32 * i] = acc[i];
+        __syncthreads();
+        const int col = c0 + threadIdx.x;
+        if (threadIdx.x < LONG_CHUNK && col < a.k) {
+            float sum = 0.f;
+            for (int w = 0; w < LONG_WARPS; ++w) sum += red[w][threadIdx.x];
+            a.scratch[(long long)t.slot * a.k + col] = sum;
         }
-    }
-    __syncthreads();
-    for (int col = threadIdx.x; col < a.k; col += blockDim.x) {
-        float sum = 0.f;
-        for (int w = 0; w < nwarps; ++w) sum += red[w * a.k + col];
-        a.scratch[(long long)t.slot * a.k + col] = sum;
+        __syncthreads();
     }
 }
 
@@ -1623,12 +1628,12 @@ struct LongArgsF64 {
 };
 
 __global__ void __launch_bounds__(256) k_spmm_long_partial_f64(LongArgsF64 a) {
-    extern __shared__ double red_f64[];   // [warps][k]
+    __shared__ double red_f64[LONG_WARPS][LONG_CHUNK];
     const LongTask t = a.tasks[blockIdx.x];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-    for (int c0 = 0; c0 < a.k; c0 += 128) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int c0 = 0; c0 < a.k; c0 += LONG_CHUNK) {
         double acc[4] = {0.0, 0.0, 0.0, 0.0};
-        for (int p = t.begin + warp; p < t.end; p += nwarps) {
+        for (int p = t.begin + warp; p < t.end; p += LONG_WARPS) {
             const int c = __ldg(a.indices + p);
             const double v = __ldg(a.vals + p);
             if (c < 0) continue;
@@ -1640,16 +1645,15 @@ __global__ void __launch_bounds__(256) k_spmm_long_partial_f64(LongArgsF64 a) {
             }
         }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int col = c0 + lane + 32 * i;
-            if (col < a.k) red_f64[warp * a.k + col] = acc[i];
+        for (int i = 0; i < 4; ++i) red_f64[warp][lane + 32 * i] = acc[i];
+        __syncthreads();
+        const int col = c0 + threadIdx.x;
+        if (threadIdx.x < LONG_CHUNK && col < a.k) {
+            double sum = 0.0;
+            for (int w = 0; w < LONG_WARPS; ++w) sum += red_f64[w][threadIdx.x];
+            a.scratch[(long long)t.slot * a.k + col] = sum;
         }
-    }
-    __syncthreads();
-    for (int col = threadIdx.x; col < a.k; col += blockDim.x) {
-        double sum = 0.0;
-        for (int w = 0; w < nwarps; ++w) sum += red_f64[w * a.k + col];
-        a.scratch[(long long)t.slot * a.k + col] = sum;
+        __syncthreads();
     }
 }
 
@@ -2250,10 +2254,7 @@ int spmm_f64(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool rowmap, bool 
         la.X = b.X;
         la.scratch = scr;
         la.k = k;
-        const size_t smem = (size_t)8 * k * sizeof(double);
-        if (smem > 48 * 1024)
-            CUDA_TRY(ctx, cudaFuncSetAttribute(k_spmm_long_partial_f64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_spmm_long_partial_f64<<<A->n_long_tasks, 256, smem, stream>>>(la);
+        k_spmm_long_partial_f64<<<A->n_long_tasks, 256, 0, stream>>>(la);
         ctx->launches++;
         if (rowmap && acc) k_spmm_long_reduce_f64<true, true><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
         else if (rowmap) k_spmm_long_reduce_f64<true, false><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
@@ -2494,12 +2495,12 @@ __global__ void __launch_bounds__(256) k_spmm_generic_sr(SpmmArgs a) {
 // the addend (k_spmm_long_partial / k_spmm_long_reduce)
 template <class SR>
 __global__ void __launch_bounds__(256) k_spmm_long_partial_sr(LongArgs a) {
-    extern __shared__ float red_sr[];   // [warps][k]
+    __shared__ float red_sr[LONG_WARPS][LONG_CHUNK];
     const LongTask t = a.tasks[blockIdx.x];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-    for (int c0 = 0; c0 < a.k; c0 += 128) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int c0 = 0; c0 < a.k; c0 += LONG_CHUNK) {
         float acc[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
-        for (int p = t.begin + warp; p < t.end; p += nwarps) {
+        for (int p = t.begin + warp; p < t.end; p += LONG_WARPS) {
             const int c = __ldg(a.indices + p);
             const float v = __ldg(a.vals + p);
             if (c < 0) continue;
@@ -2511,16 +2512,15 @@ __global__ void __launch_bounds__(256) k_spmm_long_partial_sr(LongArgs a) {
             }
         }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int col = c0 + lane + 32 * i;
-            if (col < a.k) red_sr[warp * a.k + col] = acc[i];
+        for (int i = 0; i < 4; ++i) red_sr[warp][lane + 32 * i] = acc[i];
+        __syncthreads();
+        const int col = c0 + threadIdx.x;
+        if (threadIdx.x < LONG_CHUNK && col < a.k) {
+            float r = SR::zero();
+            for (int w = 0; w < LONG_WARPS; ++w) r = SR::plus(r, red_sr[w][threadIdx.x]);
+            a.scratch[(long long)t.slot * a.k + col] = r;
         }
-    }
-    __syncthreads();
-    for (int col = threadIdx.x; col < a.k; col += blockDim.x) {
-        float r = SR::zero();
-        for (int w = 0; w < nwarps; ++w) r = SR::plus(r, red_sr[w * a.k + col]);
-        a.scratch[(long long)t.slot * a.k + col] = r;
+        __syncthreads();
     }
 }
 
@@ -2682,10 +2682,7 @@ int spmm_sr(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool min_plus) {
         la.k = k;
         la.X2 = nullptr;
         la.x_split = 0;
-        const size_t smem = (size_t)8 * k * 4;
-        if (smem > 48 * 1024)
-            CUDA_TRY(ctx, cudaFuncSetAttribute(k_spmm_long_partial_sr<SR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_spmm_long_partial_sr<SR><<<A->n_long_tasks, 256, smem, stream>>>(la);
+        k_spmm_long_partial_sr<SR><<<A->n_long_tasks, 256, 0, stream>>>(la);
         ctx->launches++;
         k_spmm_long_reduce_sr<SR><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, la.scratch, a.C, k,
                                                                        a.add_src, a.add_map);
@@ -3603,15 +3600,15 @@ __global__ void __launch_bounds__(256) k_spmm_generic_wit(WitArgs w) {
 template <class SR>
 __global__ void __launch_bounds__(256) k_spmm_long_partial_wit(LongArgs a, const int *__restrict__ self,
                                                                int *__restrict__ lab_scratch) {
-    extern __shared__ float red_wv[];   // [warps][k] values, then [warps][k] labels
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-    int *red_wl = reinterpret_cast<int *>(red_wv + nwarps * a.k);
+    __shared__ float red_wv[LONG_WARPS][LONG_CHUNK];
+    __shared__ int red_wl[LONG_WARPS][LONG_CHUNK];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const LongTask t = a.tasks[blockIdx.x];
     const int own = (self != nullptr) ? self[t.row] : t.row;
-    for (int c0 = 0; c0 < a.k; c0 += 128) {
+    for (int c0 = 0; c0 < a.k; c0 += LONG_CHUNK) {
         float av[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
         int al[4] = {-1, -1, -1, -1};
-        for (int p = t.begin + warp; p < t.end; p += nwarps) {
+        for (int p = t.begin + warp; p < t.end; p += LONG_WARPS) {
             const int c = __ldg(a.indices + p);
             const float v = __ldg(a.vals + p);
             if (c < 0 || c == own) continue;
@@ -3623,18 +3620,17 @@ __global__ void __launch_bounds__(256) k_spmm_long_partial_wit(LongArgs a, const
             }
         }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int col = c0 + lane + 32 * i;
-            if (col < a.k) { red_wv[warp * a.k + col] = av[i]; red_wl[warp * a.k + col] = al[i]; }
+        for (int i = 0; i < 4; ++i) { red_wv[warp][lane + 32 * i] = av[i]; red_wl[warp][lane + 32 * i] = al[i]; }
+        __syncthreads();
+        const int col = c0 + threadIdx.x;
+        if (threadIdx.x < LONG_CHUNK && col < a.k) {
+            float v = SR::zero();
+            int l = -1;
+            for (int w = 0; w < LONG_WARPS; ++w) wit_plus<SR>(v, l, red_wv[w][threadIdx.x], red_wl[w][threadIdx.x]);
+            a.scratch[(long long)t.slot * a.k + col] = v;
+            lab_scratch[(long long)t.slot * a.k + col] = l;
         }
-    }
-    __syncthreads();
-    for (int col = threadIdx.x; col < a.k; col += blockDim.x) {
-        float v = SR::zero();
-        int l = -1;
-        for (int w = 0; w < nwarps; ++w) wit_plus<SR>(v, l, red_wv[w * a.k + col], red_wl[w * a.k + col]);
-        a.scratch[(long long)t.slot * a.k + col] = v;
-        lab_scratch[(long long)t.slot * a.k + col] = l;
+        __syncthreads();
     }
 }
 
@@ -3752,10 +3748,7 @@ int spmm_wit(arrow_ctx *ctx, const Csr *A, WitArgs &w, bool min_plus) {
         la.X2 = nullptr;
         la.x_split = 0;
         int *lab_scratch = reinterpret_cast<int *>(ctx->long_scratch[lane] + slots);
-        const size_t smem = (size_t)8 * k * 8;
-        if (smem > 48 * 1024)
-            CUDA_TRY(ctx, cudaFuncSetAttribute(k_spmm_long_partial_wit<SR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_spmm_long_partial_wit<SR><<<A->n_long_tasks, 256, smem, stream>>>(la, w.self, lab_scratch);
+        k_spmm_long_partial_wit<SR><<<A->n_long_tasks, 256, 0, stream>>>(la, w.self, lab_scratch);
         ctx->launches++;
         k_spmm_long_reduce_wit<SR><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, la.scratch,
                                                                         lab_scratch, w);
@@ -4654,10 +4647,7 @@ static int spmm_impl(arrow_ctx *ctx, const SpmmCall &q) {
         la.k = k;
         la.X2 = a.X2;
         la.x_split = a.x_split;
-        const size_t smem = (size_t)8 * k * 4;
-        if (smem > 48 * 1024)
-            CUDA_TRY(ctx, cudaFuncSetAttribute(k_spmm_long_partial, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_spmm_long_partial<<<A->n_long_tasks, 256, smem, stream>>>(la);
+        k_spmm_long_partial<<<A->n_long_tasks, 256, 0, stream>>>(la);
         ctx->launches++;
         const int *rmp = rm ? rm->p : nullptr;
         float *cp = C ? C->p : nullptr;

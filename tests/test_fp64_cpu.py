@@ -1,4 +1,7 @@
-"""CPU tests of float64 decompositions: loading and precision of the values, refusals, and the byte accounting."""
+"""CPU tests of float64 decompositions: loading and precision of the values, refusals, the byte accounting, and the
+float64 tile shapes the GPU sweep reaches."""
+import re
+
 import numpy as np
 import pytest
 from scipy import sparse
@@ -7,6 +10,8 @@ from arrow_matrix_b200 import _lib, decomp, graphio, synth
 from arrow_matrix_b200.arrow_dec_mpi import ArrowDecompositionMPI
 from arrow_matrix_b200.comm import SelfComm
 from arrow_matrix_b200.engine import ArrowEngine, _LevelState
+from tests import tile_dispatch as td
+from tests.test_gpu_fp64 import KS as GPU_SWEEP_KS
 
 W = 8
 
@@ -129,3 +134,39 @@ def test_byte_accounting_uses_the_element_size():
         routed = float(np.count_nonzero(nxt.to_prev < st.rows)) if mode == "fused" else 0.0
         assert f32.level_bytes(0) == st.nnz * 8 + (st.rows + 1) * 4 + 2.0 * st.rows * k * 4 + routed * k * 4
         assert f64.level_bytes(0) == st.nnz * 12 + (st.rows + 1) * 4 + 2.0 * st.rows * k * 8 + routed * k * 8
+
+
+def f64_tile_shape(k: int):
+    """(G, VPL) of the float64 tile kernel a launch with ``k`` columns runs (``launch_tiles_f64``): lanes per row and
+    double2 per lane from k2 = k / 2"""
+    assert k % 2 == 0 and 2 <= k <= 256
+    k2 = k // 2
+    vpl = 4 if k2 >= 32 else (2 if k2 >= 8 else 1)
+    lanes = -(-k2 // vpl)
+    g = 1
+    while g < lanes:
+        g <<= 1
+    return g, vpl
+
+
+def source_f64_shapes(path: str) -> set:
+    """the TF(G, VPL) lines of ``launch_tiles_f64`` in the CUDA source"""
+    with open(path) as f:
+        src = f.read()
+    body = src[src.index("int launch_tiles_f64(arrow_ctx *ctx"):]
+    body = body[:body.index("#undef TF")]
+    return {(int(m.group(1)), int(m.group(2))) for m in re.finditer(r"(?<![A-Z])TF\((\d+),\s*(\d+)\);", body)}
+
+
+def test_float64_tile_shapes_are_all_reached_by_the_gpu_sweep():
+    in_source = source_f64_shapes(td.SOURCE)
+    reached = {f64_tile_shape(k) for k in GPU_SWEEP_KS if k % 2 == 0 and k <= 256}
+    assert len(in_source) == 10 and reached == in_source, \
+        f"unreached: {in_source - reached}, not in the source: {reached - in_source}"
+
+
+def test_float64_tile_shape_restatement():
+    """the widths either side of every shape boundary"""
+    assert [f64_tile_shape(k) for k in (2, 4, 6, 8, 10, 16, 18, 32, 34, 62, 64, 66, 128, 130, 256)] == [
+        (1, 1), (2, 1), (4, 1), (4, 1), (8, 1), (4, 2), (8, 2), (8, 2), (16, 2), (16, 2), (8, 4), (16, 4), (16, 4),
+        (32, 4), (32, 4)]

@@ -22,7 +22,9 @@ from tests.test_gpu_kernels import assert_close
 
 pytestmark = pytest.mark.gpu
 
-KS = [1, 2, 3, 4, 6, 8, 10, 16, 30, 32, 64, 126, 128, 256, 258, 512]
+# every float64 tile shape (tests/test_fp64_cpu.py pins them to launch_tiles_f64), the generic kernel (k odd or > 256)
+# and both sides of its boundary; 34 and 62 run TF(16, 2), at 62 with the last lane's second double2 as padding
+KS = [1, 2, 3, 4, 6, 8, 10, 16, 30, 32, 34, 62, 64, 126, 128, 256, 258, 512]
 GRIDS = {"1 CTA": (1, 1), "default": (0, 0)}          # (SPMM_SM_LIMIT, SPMM_CTAS_PER_SM)
 ERR_ARG, ERR_UNSUPPORTED = -2, -6
 
@@ -60,9 +62,10 @@ def _ragged_block(rng):
 class Problem:
     """one float64 block and the operands of every epilogue at one k"""
 
-    def __init__(self, ctx, A, k, seed):
+    def __init__(self, ctx, A, k, seed, threshold=td.LONG_THRESHOLD, segment=td.LONG_SEGMENT):
         rng = np.random.default_rng(seed)
         self.ctx, self.A, self.k = ctx, A, k
+        self.threshold, self.segment = threshold, segment          # the long-row tuning the block was uploaded under
         n, nc = A.shape
         self.n = n
         used = np.unique(A.indices)
@@ -97,15 +100,16 @@ class Problem:
         before = self.Cold if acc else self.Cnan
         self.dC.h2d(before)
         rowmap = self.rm if epi in ("rowmap", "rowmap_acc", "skip") else None
+        tuning = dict(threshold=self.threshold, segment=self.segment)
         if epi == "add":
             ctx.spmm_add(self.dA, self.dX, self.dC, self.dadd, self.dam)
-            e = sb.reference(P, before, add=self.addh, add_map=self.amap, label=f"k={self.k} {epi}")
+            e = sb.reference(P, before, add=self.addh, add_map=self.amap, label=f"k={self.k} {epi}", **tuning)
         elif epi == "skip":
             ctx.spmm(self.dAs, self.dXs, self.dC, rowmap=self.dm, accumulate=True)
-            e = sb.reference(self.Ps, before, rowmap=rowmap, accumulate=True, label=f"k={self.k} {epi}")
+            e = sb.reference(self.Ps, before, rowmap=rowmap, accumulate=True, label=f"k={self.k} {epi}", **tuning)
         else:
             ctx.spmm(self.dA, self.dX, self.dC, rowmap=self.dm if rowmap is not None else None, accumulate=acc)
-            e = sb.reference(P, before, rowmap=rowmap, accumulate=acc, label=f"k={self.k} {epi}")
+            e = sb.reference(P, before, rowmap=rowmap, accumulate=acc, label=f"k={self.k} {epi}", **tuning)
         return self.dC.d2h(), e
 
     def free(self):

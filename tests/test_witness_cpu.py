@@ -1,6 +1,9 @@
 """CPU tests of the predecessor pass: the host restatement (tests/witness_ref.py) equals a brute-force scan, and at fixed
 points of the step its parents form shortest-path trees (min_plus, Dijkstra lengths, BFS levels) and critical-path
-chains (max_plus on a DAG, a topological DP); the refusals happen before any CUDA work."""
+chains (max_plus on a DAG, a topological DP); the refusals happen before any CUDA work; the GPU sweep reaches every
+witness tile shape."""
+import re
+
 import numpy as np
 import pytest
 from scipy import sparse
@@ -12,6 +15,7 @@ from arrow_matrix_b200.comm import SelfComm
 from arrow_matrix_b200.decomposition import arrow_decomposition, reconstruct
 from arrow_matrix_b200.engine import ArrowEngine
 from tests import semiring_ref as sr
+from tests import tile_dispatch as td
 from tests import witness_ref as wr
 
 
@@ -230,3 +234,37 @@ def test_restatement_refuses_rows_behind_the_sentinel():
     assert not lv.fused_ok()
     with pytest.raises(AssertionError, match="sentinel"):
         wr.predecessors(dec, w, np.zeros((lv.rows[0], 2), np.float32), "min_plus", levels=lv)
+
+
+def wit_tile_shape(k: int, big_tiles: bool = True):
+    """(G, VPL, big tiles) of the witness tile kernel a launch with ``k`` columns runs (``launch_tiles_wit_shape``): one
+    float4 per lane up to 32 lanes, then two; the big tiles where launch_tiles would pick them (k <= 32)"""
+    assert k % 4 == 0 and 4 <= k <= 256
+    k4 = k // 4
+    vpl = 2 if k4 > 32 else 1
+    lanes = -(-k4 // vpl)
+    g = 1
+    while g < lanes:
+        g <<= 1
+    return g, vpl, bool(big_tiles) and k4 <= 8
+
+
+def source_wit_shapes(path: str) -> set:
+    """the WIB / WIS (G, VPL) lines of ``launch_tiles_wit_shape`` in the CUDA source"""
+    with open(path) as f:
+        src = f.read()
+    body = src[src.index("int launch_tiles_wit_shape(arrow_ctx *ctx"):]
+    body = body[:body.index("#undef WIS")]
+    found = set()
+    for macro, big in (("WIB", True), ("WIS", False)):
+        for m in re.finditer(rf"(?<![A-Z]){macro}\((\d+),\s*(\d+)\);", body):
+            found.add((int(m.group(1)), int(m.group(2)), big))
+    return found
+
+
+def test_witness_tile_shapes_are_all_reached_by_the_gpu_sweep():
+    """tests/test_gpu_witness.py runs sr.SWEEP_KS with the big tiles on and off"""
+    in_source = source_wit_shapes(td.SOURCE)
+    reached = {wit_tile_shape(k, big) for k in sr.SWEEP_KS if k % 4 == 0 and k <= 256 for big in (True, False)}
+    assert len(in_source) == 11 and reached == in_source, \
+        f"unreached: {in_source - reached}, not in the source: {reached - in_source}"
