@@ -48,9 +48,10 @@ EXPORTS = [
     "arrow_spmm_sr", "arrow_gather_rows_sr", "arrow_dense_count_diff",
     "arrow_spmm_sr_witness", "arrow_tile_rows", "arrow_tile_rows_rule", "arrow_bits_mark_new",
     "arrow_adj_build", "arrow_adj_free", "arrow_adj_info", "arrow_adj_d2h", "arrow_bits_mark_frontier",
-    "arrow_bits_push_frontier",
+    "arrow_bits_push_frontier", "arrow_adj_build_weighted", "arrow_adj_values_d2h", "arrow_sr_mark_frontier",
+    "arrow_sr_push_frontier",
 ]
-ABI_VERSION = 8        # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 9        # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -158,6 +159,10 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_adj_d2h": (c_int, [P, I, P, P]),
         "arrow_bits_mark_frontier": (c_int, [P, I, I, I, I, I, pI64, pI64, pI64]),
         "arrow_bits_push_frontier": (c_int, [P, I, I, I]),
+        "arrow_adj_build_weighted": (c_int, [P, I, pI, pI, I64, pI]),
+        "arrow_adj_values_d2h": (c_int, [P, I, P]),
+        "arrow_sr_mark_frontier": (c_int, [P, I, I, I, pI64, pI64, pI64]),
+        "arrow_sr_push_frontier": (c_int, [P, I, I, I, I]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -466,15 +471,17 @@ class Context:
         self._check(self.lib.arrow_bits_mark_new(self._h, new.h, old.h, dist.h, int(level), byref(n)))
         return int(n.value)
 
-    def adj_build(self, parts: Sequence[tuple], n_vertices: int) -> "Adjacency":
+    def adj_build(self, parts: Sequence[tuple], n_vertices: int, weighted: bool = False) -> "Adjacency":
         """The push adjacency of a BFS (``arrow_adj_build``): ``parts`` is a sequence of ``(Csr, RowMap or None)``; entry
         (r, c) of a block gives the edge map(c) -> map(r) (None: the identity), edges with an end at -1 and u == v are
-        dropped.  Synchronises."""
+        dropped.  ``weighted`` (``arrow_adj_build_weighted``): every edge carries its entry's fp32 value and the edges
+        u == v are kept -- the adjacency of the min-plus / max-plus push.  Synchronises."""
         n = len(parts)
         csrs = (c_int * max(n, 1))(*[A.h for A, _ in parts])
         maps = (c_int * max(n, 1))(*[m.h if m is not None else -1 for _, m in parts])
         h = c_int()
-        self._check(self.lib.arrow_adj_build(self._h, n, csrs, maps, int(n_vertices), byref(h)))
+        build = self.lib.arrow_adj_build_weighted if weighted else self.lib.arrow_adj_build
+        self._check(build(self._h, n, csrs, maps, int(n_vertices), byref(h)))
         return Adjacency(self, h.value)
 
     def bits_mark_frontier(self, adj: "Adjacency", new: "Dense", old: "Dense", dist: "Dense", level: int):
@@ -489,6 +496,19 @@ class Context:
         """out = x, then out[v] |= x[u] along the adjacency's edges of the recorded frontier rows u
         (``arrow_bits_push_frontier``); ``x`` must be the tile of the last ``bits_mark_frontier`` on ``adj``"""
         self._check(self.lib.arrow_bits_push_frontier(self._h, adj.h, x.h, out.h))
+
+    def sr_mark_frontier(self, adj: "Adjacency", new: "Dense", old: "Dense"):
+        """(rows changed by value -- ``count_diff``'s figure --, frontier rows, frontier edges) of two fp32 tiles; records
+        in ``adj`` the rows that differ in bits (``arrow_sr_mark_frontier``); synchronises"""
+        n, rows, edges = c_int64(), c_int64(), c_int64()
+        self._check(self.lib.arrow_sr_mark_frontier(self._h, adj.h, new.h, old.h, byref(n), byref(rows), byref(edges)))
+        return int(n.value), int(rows.value), int(edges.value)
+
+    def sr_push_frontier(self, adj: "Adjacency", x: "Dense", out: "Dense", semiring: int):
+        """out = canon(x), then out[v] ⊕= fl(a + x[u]) along the weighted adjacency's edges of the recorded frontier rows u
+        (``arrow_sr_push_frontier``, ``semiring`` SR_MIN_PLUS or SR_MAX_PLUS); ``x`` must be the tile of the last
+        ``sr_mark_frontier`` on ``adj``"""
+        self._check(self.lib.arrow_sr_push_frontier(self._h, adj.h, x.h, out.h, int(semiring)))
 
     def count_diff(self, a: "Dense", b: "Dense") -> int:
         """rows in which two equally shaped tiles differ in some element (-0 == +0, NaN != NaN); synchronises"""
@@ -612,7 +632,8 @@ class RowMap(_Handle):
 
 
 class Adjacency(_Handle):
-    """push adjacency of a BFS (``arrow_adj_build``): a CSR without values, row u listing the destinations v of u"""
+    """push adjacency (``arrow_adj_build``): a CSR, row u listing the destinations v of u; without values, or with the
+    edges' fp32 weights (``arrow_adj_build_weighted``)"""
 
     def info(self):
         n, m = c_int64(), c_int64()
@@ -626,6 +647,12 @@ class Adjacency(_Handle):
         indices = np.empty(inf["n_edges"], np.int32)
         self.ctx._check(self.ctx.lib.arrow_adj_d2h(self.ctx._h, self.h, _ptr(indptr), _ptr(indices)))
         return indptr, indices
+
+    def values_d2h(self):
+        """the weights as a float32 host array, in the order of ``d2h()``'s indices (weighted adjacency only)"""
+        values = np.empty(self.info()["n_edges"], np.float32)
+        self.ctx._check(self.ctx.lib.arrow_adj_values_d2h(self.ctx._h, self.h, _ptr(values)))
+        return values
 
     def free(self):
         self._free("arrow_adj_free")

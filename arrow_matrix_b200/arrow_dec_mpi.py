@@ -177,6 +177,15 @@ class ArrowDecompositionMPI:
             raise ValueError("bfs_levels runs on one GPU only")
         return eng.bfs_levels(max_steps, out)
 
+    def iterate_to_fixed_point(self, max_steps: int) -> int:
+        """Extension (one GPU): ``step()`` until a step changes no level-0 row, at most ``max_steps`` times; returns the
+        number of steps taken.  Direction-optimising in ``min_plus`` / ``max_plus`` with ``add_identity`` (multi-source
+        shortest and critical paths; see ``ArrowEngine.iterate_to_fixed_point``)."""
+        eng = self._require_engine()
+        if not isinstance(eng, ArrowEngine):
+            raise ValueError("iterate_to_fixed_point runs on one GPU only")
+        return eng.iterate_to_fixed_point(max_steps)
+
     def synchronize(self):
         self._require_engine().sync()
 

@@ -100,10 +100,12 @@ struct PtrTable {                     // one device pointer per row: where a SpM
     bool live = false;
 };
 
-struct Adj {                          // push adjacency of the (or, and) BFS (arrow_adj_build) and its frontier record
+struct Adj {                          // push adjacency (arrow_adj_build / arrow_adj_build_weighted) and its frontier record
     int64_t n = 0, m = 0;             // vertices (level-0 rows), edges
     int *indptr = nullptr;            // device: n + 1 row pointers of the transposed matrix (row u: destinations v)
     int *indices = nullptr;           // device: m destinations
+    float *values = nullptr;          // device: m fp32 weights, beside indices (weighted adjacency only)
+    bool weighted = false;
     int *front_rows = nullptr;        // device, n: rows of the last arrow_bits_mark_frontier, in list order
     int *front_off = nullptr;         // device, n: first edge offset of each of them, increasing with the list position
     int64_t n_front = 0, front_edges = 0;
@@ -274,6 +276,7 @@ void csr_release(Csr &c) {
 void adj_release(Adj &a) {
     cudaFree(a.indptr);
     cudaFree(a.indices);
+    cudaFree(a.values);
     cudaFree(a.front_rows);
     cudaFree(a.front_off);
     a = Adj();
@@ -3189,10 +3192,14 @@ __device__ __forceinline__ int last_le(const int *__restrict__ a, int lo, int hi
     return lo;
 }
 
-// edges of one block: entry (r, c) with c >= 0 gives u -> v = map(c) -> map(r); an end at -1 or u == v drops it.  Counts
-// them into *count; with `keys` also appends (u << 32) | v at a warp-aggregated cursor (the order is fixed by the sort).
+// edges of one block: entry (r, c) with c >= 0 gives u -> v = map(c) -> map(r); an end at -1 drops it, and so does u == v
+// unless W (the weighted adjacency keeps self-loops: a negative one changes a min-plus step).  Counts them into *count;
+// with `keys` also appends (u << 32) | v at a warp-aggregated cursor (the order is fixed by the sort), and with W the
+// entry's value w_in[e] at the same slot of w_out.
+template <bool W>
 __global__ void __launch_bounds__(256) k_adj_edges(AdjPart p, unsigned long long *__restrict__ count,
-                                                   unsigned long long *__restrict__ keys) {
+                                                   unsigned long long *__restrict__ keys,
+                                                   const float *__restrict__ w_in = nullptr, float *__restrict__ w_out = nullptr) {
     const int lane = threadIdx.x & 31;
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long e0 = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31); e0 < p.nnz; e0 += stride) {
@@ -3205,7 +3212,7 @@ __global__ void __launch_bounds__(256) k_adj_edges(AdjPart p, unsigned long long
                 const int r = last_le(p.indptr, 0, p.n_rows - 1, e);
                 const int u = p.map ? __ldg(p.map + c) : c;
                 const int v = p.map ? __ldg(p.map + r) : r;
-                ok = u >= 0 && v >= 0 && u != v;
+                ok = u >= 0 && v >= 0 && (W || u != v);
                 key = ((unsigned long long)(unsigned)u << 32) | (unsigned)v;
             }
         }
@@ -3215,7 +3222,11 @@ __global__ void __launch_bounds__(256) k_adj_edges(AdjPart p, unsigned long long
         if (lane == 0) base = atomicAdd(count, (unsigned long long)__popc(ball));
         if (keys != nullptr) {
             base = __shfl_sync(0xffffffffu, base, 0);
-            if (ok) keys[base + __popc(ball & ((1u << lane) - 1u))] = key;
+            if (ok) {
+                const unsigned long long at = base + __popc(ball & ((1u << lane) - 1u));
+                keys[at] = key;
+                if (W) w_out[at] = __ldg(w_in + e);
+            }
         }
     }
 }
@@ -3352,6 +3363,159 @@ __global__ void __launch_bounds__(PUSH_THREADS) k_bits_push(const V *__restrict_
                 const int u = __ldg(front_rows + p);
                 const int v = __ldg(adj_idx + __ldg(adj_ptr + u) + (int)(e - __ldg(front_off + p)));
                 push_or(out, (long long)v * row_vecs + q, x[(long long)u * row_vecs + q]);
+            }
+        }
+        __syncthreads();                                      // s_lo / s_hi are rewritten by the next chunk
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// direction-optimising shortest and critical paths on fp32 tiles (min-plus, max-plus).  With add_identity a fused step is
+// F(X)[v] = ⊕ over in-edges (u, a) of v of fl(a + X[u]), NaN terms dropped, the in-edges being the identity diagonal and
+// every level's entries through its row map.  Inside a fixed-point loop, X_h = F(X_{h-1}) <= X_{h-1}; a row whose bits did
+// not change contributes terms X_h already holds, so F(X_h)[v] = canon(X_h[v]) ⊕ (⊕ over the frontier rows u -> v of
+// fl(a + X_h[u])), canon(x) = fl(0 + x) with NaN as the ⊕ identity: the push of the frontier along the weighted transposed
+// operator (arrow_adj_build_weighted) gives the pull step's bits, provided no weight is -0 (fl(-0 + -0) = -0 breaks the
+// bit order of the argument).
+// ------------------------------------------------------------------------------------------------
+
+// k_count_diff's figure (rows that differ by value: -0 == +0, NaN != NaN) and the frontier record of the rows that differ
+// in bits, each with its first edge offset in the push adjacency.  A warp takes its 32 rows of a pass one at a time (lanes
+// over the columns) and lane i keeps the claim of the i-th; a CTA claims its slice of the list with one 64-bit atomicAdd
+// on counts[1], packed like k_bits_mark_frontier's.
+__global__ void __launch_bounds__(MARK_THREADS) k_sr_mark_frontier(const float *__restrict__ nw, const float *__restrict__ old,
+                                                                   long long rows, int k, const int *__restrict__ adj_ptr,
+                                                                   int *__restrict__ front_rows, int *__restrict__ front_off,
+                                                                   unsigned long long *__restrict__ counts) {
+    constexpr int WARPS = MARK_THREADS / 32;
+    __shared__ unsigned long long s_warp[WARPS];
+    __shared__ unsigned long long s_base;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned long long changed = 0;                           // rows that differ by value (lane 0 counts them)
+    for (long long r0 = (long long)blockIdx.x * MARK_THREADS; r0 < rows; r0 += (long long)gridDim.x * MARK_THREADS) {
+        const long long w0 = r0 + (long long)warp * 32;
+        unsigned long long claim = 0;
+        for (int i = 0; i < 32 && w0 + i < rows; ++i) {
+            const float *a = nw + (w0 + i) * k, *b = old + (w0 + i) * k;
+            bool by_value = false, by_bits = false;
+            for (int c = lane; c < k; c += 32) {
+                const float x = a[c], y = b[c];
+                by_value |= x != y;
+                by_bits |= __float_as_uint(x) != __float_as_uint(y);
+            }
+            by_value = __any_sync(0xffffffffu, by_value);
+            by_bits = __any_sync(0xffffffffu, by_bits);
+            changed += (lane == 0 && by_value);
+            if (lane == i && by_bits)
+                claim = (1ull << 32) | (unsigned)(__ldg(adj_ptr + w0 + i + 1) - __ldg(adj_ptr + w0 + i));
+        }
+        unsigned long long incl = claim;                      // inclusive scan over the warp
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, incl, off);
+            if (lane >= off) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned long long total = 0;
+            for (int i = 0; i < WARPS; ++i) {
+                const unsigned long long t = s_warp[i];
+                s_warp[i] = total;
+                total += t;
+            }
+            s_base = total ? atomicAdd(counts + 1, total) : 0ull;
+        }
+        __syncthreads();
+        if (claim) {
+            const unsigned long long at = s_base + s_warp[warp] + incl - claim;
+            front_rows[at >> 32] = (int)(w0 + lane);
+            front_off[at >> 32] = (int)(unsigned)at;
+        }
+        __syncthreads();                                      // s_warp / s_base are rewritten by the next pass
+    }
+    if (changed) atomicAdd(counts, changed);
+}
+
+// canon(x) = fl(0 + x) ⊕ the identity: what the identity diagonal contributes to a pull step (NaN -> identity, -0 -> +0)
+template <class SR>
+__device__ __forceinline__ float sr_canon(float x) {
+    return SR::plus(SR::zero(), SR::times(0.0f, x));
+}
+template <class SR>
+__global__ void __launch_bounds__(256) k_sr_canon(const float4 *__restrict__ x, float4 *__restrict__ out, long long n4,
+                                                  const float *__restrict__ xs, float *__restrict__ outs, long long n) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (long long i = t; i < n4; i += stride) {
+        const float4 v = x[i];
+        out[i] = make_float4(sr_canon<SR>(v.x), sr_canon<SR>(v.y), sr_canon<SR>(v.z), sr_canon<SR>(v.w));
+    }
+    for (long long i = 4 * n4 + t; i < n; i += stride) outs[i] = sr_canon<SR>(xs[i]);
+}
+
+// a non-returning float min / max from integer reductions: a float with the sign bit clear orders like its bits as s32, one
+// with the sign bit set in reverse of its bits as u32, and every sign-set bit pattern is above every sign-clear one as
+// u32 and below it as s32.  t is never NaN, and the target never holds NaN or -0 (canon).
+__device__ __forceinline__ void red_fold(SrMinPlus, float *p, float t) {
+    if (__float_as_int(t) >= 0) asm volatile("red.global.min.s32 [%0], %1;" ::"l"(p), "r"(__float_as_int(t)) : "memory");
+    else asm volatile("red.global.max.u32 [%0], %1;" ::"l"(p), "r"(__float_as_uint(t)) : "memory");
+}
+__device__ __forceinline__ void red_fold(SrMaxPlus, float *p, float t) {
+    if (__float_as_int(t) >= 0) asm volatile("red.global.max.s32 [%0], %1;" ::"l"(p), "r"(__float_as_int(t)) : "memory");
+    else asm volatile("red.global.min.u32 [%0], %1;" ::"l"(p), "r"(__float_as_uint(t)) : "memory");
+}
+__device__ __forceinline__ bool improves(SrMinPlus, float t, float c) { return t < c; }   // false for a NaN t
+__device__ __forceinline__ bool improves(SrMaxPlus, float t, float c) { return t > c; }
+
+// fold t = fl(a + xu) into *o when it improves on canon(xv), xv the read-only x[v] (failed relaxations cost no atomic)
+template <class SR>
+__device__ __forceinline__ void sr_relax(float *o, float a, float xu, float xv) {
+    const float t = SR::times(a, xu);
+    if (improves(SR(), t, sr_canon<SR>(xv))) red_fold(SR(), o, t);
+}
+template <class SR>
+__device__ __forceinline__ void sr_relax(float *o, float a, const float4 &xu, const float4 &xv) {
+    sr_relax<SR>(o, a, xu.x, xv.x);
+    sr_relax<SR>(o + 1, a, xu.y, xv.y);
+    sr_relax<SR>(o + 2, a, xu.z, xv.z);
+    sr_relax<SR>(o + 3, a, xu.w, xv.w);
+}
+
+// out[v] ⊕= fl(a + x[u]) along every edge (u -> v, a) of the recorded frontier rows.  An item is (edge slot e, vector q of
+// the row's `vecs` float4 groups, or columns when k % 4 != 0); CTAs walk chunks like k_bits_push, so a hub row's edges
+// spread over many CTAs.
+template <class SR, class V>
+__global__ void __launch_bounds__(PUSH_THREADS) k_sr_push(const V *__restrict__ x, float *__restrict__ out,
+                                                          const int *__restrict__ adj_ptr, const int *__restrict__ adj_idx,
+                                                          const float *__restrict__ adj_val,
+                                                          const int *__restrict__ front_rows,
+                                                          const int *__restrict__ front_off, int n_front, long long n_items,
+                                                          int vecs) {
+    constexpr long long CHUNK = (long long)PUSH_THREADS * PUSH_ITEMS;
+    constexpr int PER = (int)(sizeof(V) / sizeof(float));
+    __shared__ int s_lo, s_hi;
+    for (long long c0 = (long long)blockIdx.x * CHUNK; c0 < n_items; c0 += (long long)gridDim.x * CHUNK) {
+        if (threadIdx.x == 0) {
+            const long long c1 = (c0 + CHUNK < n_items ? c0 + CHUNK : n_items) - 1;
+            s_lo = last_le(front_off, 0, n_front - 1, c0 / vecs);
+            s_hi = last_le(front_off, s_lo, n_front - 1, c1 / vecs);
+        }
+        __syncthreads();
+        const int lo = s_lo, hi = s_hi;
+#pragma unroll
+        for (int j = 0; j < PUSH_ITEMS; ++j) {
+            const long long i = c0 + j * PUSH_THREADS + threadIdx.x;
+            if (i < n_items) {
+                const long long e = i / vecs;
+                const int q = (int)(i - e * vecs);
+                const int p = last_le(front_off, lo, hi, e);
+                const int u = __ldg(front_rows + p);
+                const int slot = __ldg(adj_ptr + u) + (int)(e - __ldg(front_off + p));
+                const int v = __ldg(adj_idx + slot);
+                const float a = __ldg(adj_val + slot);
+                const long long vq = (long long)v * vecs + q;
+                sr_relax<SR>(out + vq * PER, a, x[(long long)u * vecs + q], x[vq]);
             }
         }
         __syncthreads();                                      // s_lo / s_hi are rewritten by the next chunk
@@ -5040,17 +5204,24 @@ int arrow_bits_mark_new(arrow_ctx *ctx, int new_buf, int old_buf, int dist_buf, 
     return ARROW_OK;
 }
 
-int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out) {
-    CHECK_CTX(ctx);
-    CHECK_POISON(ctx);
+namespace {
+// arrow_adj_build (weighted false) and arrow_adj_build_weighted: one validation, one edge pass, one sort
+int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, bool weighted, int *adj_out) {
+    const char *fn = weighted ? "arrow_adj_build_weighted" : "arrow_adj_build";
     if (!adj_out || n_parts < 0 || (n_parts > 0 && (!csrs || !maps)) || n_vertices < 0)
         return fail(ctx, ARROW_ERR_ARG, "bad arguments (n_parts=%d, n_vertices=%lld)", n_parts, (long long)n_vertices);
     if (n_vertices > 2147483646LL) return fail(ctx, ARROW_ERR_RANGE, "%lld vertices exceed the int32 device layout", (long long)n_vertices);
-    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_adj_build allocates and synchronises: not during graph capture");
+    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "%s allocates and synchronises: not during graph capture", fn);
     std::vector<AdjPart> parts;
+    std::vector<const float *> weights;                       // the entries' values of each part (weighted only)
     for (int i = 0; i < n_parts; ++i) {
         const Csr *c = get_csr(ctx, csrs[i]);
         if (!c) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad csr handle %d", i, csrs[i]);
+        if (weighted && c->dtype != ARROW_F32)
+            return fail(ctx, ARROW_ERR_UNSUPPORTED, "part %d: %s carries fp32 weights, the block is %s", i, fn,
+                        dtype_name(c->dtype));
+        if (weighted && c->nnz > 0 && !c->vals)
+            return fail(ctx, ARROW_ERR_ARG, "part %d: the block has no values to carry as weights", i);
         const IdxMap *m = nullptr;
         if (maps[i] != -1) {
             m = get_map(ctx, maps[i]);
@@ -5065,7 +5236,10 @@ int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *map
             return fail(ctx, ARROW_ERR_ARG, "part %d: a %lld x %lld block with the identity map exceeds %lld vertices", i,
                         (long long)c->n_rows, (long long)c->n_cols, (long long)n_vertices);
         }
-        if (c->nnz > 0) parts.push_back(AdjPart{c->indptr, c->indices, m ? m->p : nullptr, (long long)c->nnz, (int)c->n_rows});
+        if (c->nnz > 0) {
+            parts.push_back(AdjPart{c->indptr, c->indices, m ? m->p : nullptr, (long long)c->nnz, (int)c->n_rows});
+            weights.push_back(c->vals);
+        }
     }
     cudaStream_t s = ctx->stream;
     auto edge_grid = [&](long long nnz) { return (int)std::min<long long>((nnz + 255) / 256, (long long)ctx->sm_count * 8); };
@@ -5075,7 +5249,8 @@ int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *map
     unsigned long long *count = reinterpret_cast<unsigned long long *>(cnt.p);
     CUDA_TRY(ctx, cudaMemsetAsync(count, 0, sizeof m, s));
     for (const AdjPart &p : parts) {
-        k_adj_edges<<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
+        if (weighted) k_adj_edges<true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
+        else k_adj_edges<false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
         ctx->launches++;
     }
     CUDA_TRY(ctx, cudaGetLastError());
@@ -5086,19 +5261,29 @@ int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *map
     Adj a;
     a.n = n_vertices;
     a.m = (int64_t)m;
+    a.weighted = weighted;
     cudaError_t e = cudaMalloc(&a.indptr, (size_t)(n_vertices + 1) * 4);
     if (e == cudaSuccess) e = cudaMalloc(&a.indices, (size_t)std::max<unsigned long long>(m, 1) * 4);
+    if (e == cudaSuccess && weighted) e = cudaMalloc(&a.values, (size_t)std::max<unsigned long long>(m, 1) * 4);
     if (e == cudaSuccess) e = cudaMalloc(&a.front_rows, (size_t)std::max<int64_t>(n_vertices, 1) * 4);
     if (e == cudaSuccess) e = cudaMalloc(&a.front_off, (size_t)std::max<int64_t>(n_vertices, 1) * 4);
-    DevTmp keys, alt, temp;             // build scratch: 16 bytes per edge and the sort's temporary storage
+    // build scratch: 16 bytes per edge (24 weighted) and the sort's temporary storage
+    DevTmp keys, alt, wk, walt, temp;
     const unsigned long long *sorted = nullptr;
     if (e == cudaSuccess && m > 0) {
         e = cudaMalloc(&keys.p, (size_t)m * 8);
         if (e == cudaSuccess) e = cudaMalloc(&alt.p, (size_t)m * 8);
+        if (e == cudaSuccess && weighted) e = cudaMalloc(&wk.p, (size_t)m * 4);
+        if (e == cudaSuccess && weighted) e = cudaMalloc(&walt.p, (size_t)m * 4);
         if (e == cudaSuccess) e = cudaMemsetAsync(count, 0, sizeof m, s);
         if (e == cudaSuccess) {
-            for (const AdjPart &p : parts) {
-                k_adj_edges<<<edge_grid(p.nnz), 256, 0, s>>>(p, count, reinterpret_cast<unsigned long long *>(keys.p));
+            unsigned long long *kp = reinterpret_cast<unsigned long long *>(keys.p);
+            for (size_t i = 0; i < parts.size(); ++i) {
+                const AdjPart &p = parts[i];
+                if (weighted)
+                    k_adj_edges<true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp, weights[i], reinterpret_cast<float *>(wk.p));
+                else
+                    k_adj_edges<false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp);
                 ctx->launches++;
             }
             e = cudaGetLastError();
@@ -5107,10 +5292,18 @@ int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *map
         while (end_bit < 64 && (1LL << (end_bit - 32)) < n_vertices) ++end_bit;
         cub::DoubleBuffer<unsigned long long> db(reinterpret_cast<unsigned long long *>(keys.p),
                                                  reinterpret_cast<unsigned long long *>(alt.p));
+        cub::DoubleBuffer<float> dw(reinterpret_cast<float *>(wk.p), reinterpret_cast<float *>(walt.p));
         size_t temp_bytes = 0;
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, db, (int)m, 0, end_bit, s);
-        if (e == cudaSuccess) e = cudaMalloc(&temp.p, std::max<size_t>(temp_bytes, 1));
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(temp.p, temp_bytes, db, (int)m, 0, end_bit, s);
+        if (weighted) {                                       // duplicates of (u, v) may leave in any order
+            if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, db, dw, (int)m, 0, end_bit, s);
+            if (e == cudaSuccess) e = cudaMalloc(&temp.p, std::max<size_t>(temp_bytes, 1));
+            if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(temp.p, temp_bytes, db, dw, (int)m, 0, end_bit, s);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(a.values, dw.Current(), (size_t)m * 4, cudaMemcpyDeviceToDevice, s);
+        } else {
+            if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, db, (int)m, 0, end_bit, s);
+            if (e == cudaSuccess) e = cudaMalloc(&temp.p, std::max<size_t>(temp_bytes, 1));
+            if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(temp.p, temp_bytes, db, (int)m, 0, end_bit, s);
+        }
         sorted = db.Current();
     }
     if (e == cudaSuccess) {
@@ -5130,6 +5323,31 @@ int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *map
     const int h = new_slot(ctx->adjs);
     ctx->adjs[h] = a;
     *adj_out = h;
+    return ARROW_OK;
+}
+}  // namespace
+
+int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, false, adj_out);
+}
+
+int arrow_adj_build_weighted(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices,
+                             int *adj_out) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, true, adj_out);
+}
+
+int arrow_adj_values_d2h(arrow_ctx *ctx, int adj, float *values) {
+    CHECK_CTX(ctx);
+    const Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (!a->weighted) return fail(ctx, ARROW_ERR_ARG, "the adjacency carries no weights (built by arrow_adj_build)");
+    if (a->m > 0 && !values) return fail(ctx, ARROW_ERR_ARG, "null host buffer");
+    if (a->m > 0) CUDA_TRY(ctx, cudaMemcpyAsync(values, a->values, (size_t)a->m * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     return ARROW_OK;
 }
 
@@ -5246,6 +5464,103 @@ int arrow_bits_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf) {
         k_bits_push<uint4><<<grid, PUSH_THREADS, 0, stream>>>(reinterpret_cast<const uint4 *>(X->p), out, a->indptr,
                                                               a->indices, a->front_rows, a->front_off, (int)a->n_front,
                                                               items, vecs, row_vecs);
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return ARROW_OK;
+}
+
+int arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int64_t *rows_changed, int64_t *frontier_rows,
+                           int64_t *frontier_edges) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    DenseBuf *N = get_dense(ctx, new_buf), *O = get_dense(ctx, old_buf);
+    if (!N || !O) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (new=%d old=%d)", new_buf, old_buf);
+    if (!rows_changed || !frontier_rows || !frontier_edges) return fail(ctx, ARROW_ERR_ARG, "null output");
+    if (N->dtype != ARROW_F32 || O->dtype != ARROW_F32)
+        return fail(ctx, ARROW_ERR_ARG, "new / old are fp32 tiles: got %s / %s", dtype_name(N->dtype), dtype_name(O->dtype));
+    if (N->rows != O->rows || N->k != O->k || N->rows != a->n)
+        return fail(ctx, ARROW_ERR_ARG, "tiles differ in shape: new %lld x %d, old %lld x %d, adjacency %lld rows",
+                    (long long)N->rows, N->k, (long long)O->rows, O->k, (long long)a->n);
+    *rows_changed = *frontier_rows = *frontier_edges = 0;
+    a->tag = -1;                                              // the record is rewritten below
+    cudaStream_t stream = cur_stream(ctx);
+    unsigned long long h[2] = {0, 0};                         // rows changed, (frontier rows << 32) | frontier edges
+    if (N->rows > 0 && N->k > 0) {
+        DevTmp cnt;
+        CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof h));
+        CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof h, stream));
+        const int grid = (int)std::min<long long>((N->rows + MARK_THREADS - 1) / MARK_THREADS, (long long)ctx->sm_count * 8);
+        k_sr_mark_frontier<<<grid, MARK_THREADS, 0, stream>>>(N->p, O->p, N->rows, N->k, a->indptr, a->front_rows,
+                                                              a->front_off, reinterpret_cast<unsigned long long *>(cnt.p));
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+        CUDA_TRY(ctx, cudaMemcpyAsync(h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+    }
+    a->n_front = (int64_t)(h[1] >> 32);
+    a->front_edges = (int64_t)(h[1] & 0xffffffffULL);
+    a->tag = new_buf;
+    a->tag_p = N->p;
+    a->tag_k = N->k;
+    *rows_changed = (int64_t)h[0];
+    *frontier_rows = a->n_front;
+    *frontier_edges = a->front_edges;
+    return ARROW_OK;
+}
+
+int arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int semiring) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    if (semiring == ARROW_SR_PLUS_TIMES || semiring == ARROW_SR_OR_AND)
+        return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_sr_push_frontier runs min-plus and max-plus, not semiring %d", semiring);
+    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS) return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
+    const Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    DenseBuf *X = get_dense(ctx, x_buf), *O = get_dense(ctx, out_buf);
+    if (!X || !O) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x=%d out=%d)", x_buf, out_buf);
+    if (X->dtype != ARROW_F32 || O->dtype != ARROW_F32)
+        return fail(ctx, ARROW_ERR_ARG, "x / out are fp32 tiles: got %s / %s", dtype_name(X->dtype), dtype_name(O->dtype));
+    if (!a->weighted) return fail(ctx, ARROW_ERR_ARG, "the adjacency carries no weights: build it with arrow_adj_build_weighted");
+    if (a->tag < 0) return fail(ctx, ARROW_ERR_ARG, "no frontier record: run arrow_sr_mark_frontier on the adjacency first");
+    if (x_buf != a->tag || X->p != a->tag_p || X->k != a->tag_k)
+        return fail(ctx, ARROW_ERR_ARG, "x (tile %d) is not the tile of the last arrow_sr_mark_frontier (tile %d)", x_buf, a->tag);
+    if (x_buf == out_buf || X->p == O->p) return fail(ctx, ARROW_ERR_ARG, "out aliases x");
+    if (X->rows != a->n || O->rows != X->rows || O->k != X->k)
+        return fail(ctx, ARROW_ERR_ARG, "shape: x %lld x %d, out %lld x %d, adjacency %lld rows", (long long)X->rows, X->k,
+                    (long long)O->rows, O->k, (long long)a->n);
+    cudaStream_t stream = cur_stream(ctx);
+    const long long n = (long long)X->rows * X->k;
+    if (n == 0) return ARROW_OK;
+    const bool mn = semiring == ARROW_SR_MIN_PLUS;
+    {                                                         // out = canon(x), float4 groups and a scalar tail
+        const bool aligned = (((uintptr_t)X->p | (uintptr_t)O->p) & 15) == 0;     // a wrapped tile with k % 4 != 0 may not be
+        const long long n4 = aligned ? n / 4 : 0;
+        const int grid = (int)std::max<long long>(1, std::min<long long>((n4 + 255) / 256, (long long)ctx->sm_count * 8));
+        const float4 *x4 = reinterpret_cast<const float4 *>(X->p);
+        float4 *o4 = reinterpret_cast<float4 *>(O->p);
+        if (mn) k_sr_canon<SrMinPlus><<<grid, 256, 0, stream>>>(x4, o4, n4, X->p, O->p, n);
+        else k_sr_canon<SrMaxPlus><<<grid, 256, 0, stream>>>(x4, o4, n4, X->p, O->p, n);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
+    if (a->front_edges == 0) return ARROW_OK;
+    const bool v4 = X->k % 4 == 0;
+    const int vecs = v4 ? X->k / 4 : X->k;
+    const long long items = a->front_edges * vecs;
+    const long long chunks = (items + (long long)PUSH_THREADS * PUSH_ITEMS - 1) / ((long long)PUSH_THREADS * PUSH_ITEMS);
+    const int per_sm = ctx->spmm_ctas_per_sm > 0 ? std::min(ctx->spmm_ctas_per_sm, 8) : 8;
+    const int sms = ctx->spmm_sm_limit > 0 ? std::min(ctx->sm_count, ctx->spmm_sm_limit) : ctx->sm_count;
+    const int grid = (int)std::min<long long>(chunks, (long long)per_sm * sms);
+    const float4 *x4 = reinterpret_cast<const float4 *>(X->p);
+#define SRP(SR, V, XP) k_sr_push<SR, V><<<grid, PUSH_THREADS, 0, stream>>>(XP, O->p, a->indptr, a->indices, a->values, \
+                                                                       a->front_rows, a->front_off, (int)a->n_front, items, vecs)
+    if (mn && v4) SRP(SrMinPlus, float4, x4);
+    else if (mn) SRP(SrMinPlus, float, X->p);
+    else if (v4) SRP(SrMaxPlus, float4, x4);
+    else SRP(SrMaxPlus, float, X->p);
+#undef SRP
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     return ARROW_OK;

@@ -64,6 +64,15 @@ def bfs_direction(frontier_edges: int, total_nnz: int, alpha: float = BFS_PUSH_A
     return "push" if frontier_edges * alpha < total_nnz else "pull"
 
 
+# iterate_to_fixed_point() in min_plus / max_plus: a level is a push when its frontier's edges times this are fewer than
+# the non-zeros a pull step gathers (bfs_direction with this alpha).  A tropical push moves k fp32 values per edge and
+# compares each, so it costs more per edge than the bit push.  Per level on an H100 80 GB HBM3 at 700 W
+# (scripts/sssp_direction_bench.py, DESIGN.md §8) push and pull cross at total_nnz / frontier_edges of about 9-10 on G2 at
+# k = 128 (pull 10.8 ms, push 3.6 ms plus about 0.4 ns per edge), 7-9 at k = 16 and about 2 on the 10**6-vertex BA graph at
+# k = 32.
+SR_PUSH_ALPHA = 9
+
+
 def semiring_code(semiring: str, dtype, fused_style: str = "gather") -> int:
     """``_lib.SR_*`` of a semiring name; raises ``ValueError`` (before any CUDA work) for an unknown name and for the
     combinations that do not exist: the tropical and boolean semirings need a float32 decomposition and run the gather
@@ -127,6 +136,9 @@ class ArrowEngine:
         self.last_bfs_directions: List[str] = []                 # "push" / "pull" per level of the last bfs_levels()
         self._adj: Optional[_lib.Adjacency] = None               # bfs_levels(): the push adjacency, built on first use
         self._push_limit: Optional[int] = None                   # None: bfs_direction() decides; else push iff edges < it
+        self.last_fixed_point_directions: List[str] = []         # "push" / "pull" per step of iterate_to_fixed_point()
+        self._sr_adj: Optional[_lib.Adjacency] = None            # iterate_to_fixed_point(): weighted push adjacency
+        self._neg_zero_weight = False                            # a -0 entry in some level: the tropical push is not exact
         fused_ok = True
         cmap_prev = None                      # level j-1 row -> level-0 row (host, int64, -1 invalid)
         for j, (B, _) in enumerate(decomposition):
@@ -138,6 +150,8 @@ class ArrowEngine:
             if j == 0 and self.add_identity:
                 ip, idx, dat = decomp.with_diagonal(ip, idx, dat, st.rows, _TIMES_ONE[self.sr], self.dtype)
             st.nnz = int(ip[-1])
+            if self.sr in (_lib.SR_MIN_PLUS, _lib.SR_MAX_PLUS) and np.any((dat == 0) & np.signbit(dat)):
+                self._neg_zero_weight = True
             st.csr = self.ctx.csr_upload(st.rows, st.rows, ip, idx, dat, dtype=self.dtype)
             if j > 0:
                 tp = self.to_prev[j][: st.rows]
@@ -393,12 +407,68 @@ class ArrowEngine:
 
     def iterate_to_fixed_point(self, max_steps: int) -> int:
         """``step()`` until a step changes no level-0 row (BFS levels, shortest paths, reachability), at most
-        ``max_steps`` times; returns the number of steps taken (the last one changed nothing unless it hit the limit)."""
+        ``max_steps`` times; returns the number of steps taken (the last one changed nothing unless it hit the limit).
+
+        Direction-optimising in ``min_plus`` / ``max_plus`` with ``add_identity`` when ``fused_ok`` holds (DESIGN.md §4):
+        a level is either a ``step()`` (pull) or a push of the rows whose bits changed in the previous level along the
+        weighted transposed operator (built on the first call, kept until ``close()``), whichever :func:`bfs_direction`
+        picks with ``SR_PUSH_ALPHA`` from the frontier's edges; ``last_fixed_point_directions`` lists the choice per
+        level.  The step count and, after every level, the level-0 features (so ``result()``, ``features()``,
+        ``count_changed()``, ``predecessors()`` and the next ``step()``) are bit-identical to pull steps only.  After a
+        push level the tiles of the levels ``j >= 1`` (``result(j)``) are not that level's product; the next ``step()``
+        rewrites them.  Every other engine, and one with a -0 weight, pulls every level."""
+        adj = self._sr_push_adjacency() if self._sr_push_ok() and int(max_steps) >= 1 else None
+        if adj is None:
+            for n in range(1, int(max_steps) + 1):
+                self.step()
+                if self.count_changed() == 0:
+                    self.last_fixed_point_directions = ["pull"] * n
+                    return n
+            self.last_fixed_point_directions = ["pull"] * max(int(max_steps), 0)
+            return int(max_steps)
+        st0 = self.levels[0]
+        limit = self._push_limit
+
+        def mark(new, old):
+            """(rows changed, push next): the stop test, and the direction of the next level"""
+            changed, _, edges = self.ctx.sr_mark_frontier(adj, new, old)
+            push = edges < limit if limit is not None else bfs_direction(edges, self.total_nnz, SR_PUSH_ALPHA) == "push"
+            return changed, push
+
+        # X_{-1} is the ⊕ identity: the first frontier is every row holding something else.  The tile that the first level
+        # writes holds it meanwhile.
+        xi = st0.xi
+        st0.bufs[1 - xi].fill(_PLUS_ZERO[self.sr])
+        _, push = mark(st0.bufs[xi], st0.bufs[1 - xi])
+        directions = []
         for n in range(1, int(max_steps) + 1):
-            self.step()
-            if self.count_changed() == 0:
+            xi = st0.xi
+            if push:                             # canon(X_h) ⊕ the frontier rows' relaxations
+                self.ctx.sr_push_frontier(adj, st0.bufs[xi], st0.bufs[1 - xi], self.sr)
+                st0.xi = st0.ci = 1 - xi
+            else:
+                self.step()                      # reads bufs[xi], leaves the result in bufs[1 - xi]
+            directions.append("push" if push else "pull")
+            changed, push = mark(st0.bufs[1 - xi], st0.bufs[xi])
+            if changed == 0:
+                self.last_fixed_point_directions = directions
                 return n
+        self.last_fixed_point_directions = directions
         return int(max_steps)
+
+    def _sr_push_ok(self) -> bool:
+        """iterate_to_fixed_point() may push: a tropical engine with the identity, every non-zero behind a level-0 row, no
+        -0 weight, and a step that advances level 0's features (an exchange-mode step of one level does not)"""
+        return (self.sr in (_lib.SR_MIN_PLUS, _lib.SR_MAX_PLUS) and self.add_identity and self.fused_ok
+                and not self._neg_zero_weight and (self.mode == "fused" or self.L > 1))
+
+    def _sr_push_adjacency(self) -> _lib.Adjacency:
+        """the weighted transposed operator of the fused step with the identity (built on the first call): every level's
+        own block with its level-j -> level-0 row map (level 0: the identity, its diagonal included)"""
+        if self._sr_adj is None:
+            parts = [(st.csr, st.cmap_dev) for st in self.levels]
+            self._sr_adj = self.ctx.adj_build(parts, self.levels[0].rows, weighted=True)
+        return self._sr_adj
 
     # -- predecessors (min_plus / max_plus) ----------------------------------------------------------------------
     def predecessors(self, out: Optional[np.ndarray] = None) -> np.ndarray:
@@ -635,7 +705,8 @@ class ArrowEngine:
     def close(self):
         for b in (self._wit_labels or []) + list(self._wit_values.values()) + list(self._bfs_tiles or ()):
             b.free()
-        if self._adj is not None:
-            self._adj.free()
-        self._wit_labels, self._wit_values, self._bfs_tiles, self._adj = None, {}, None, None
+        for a in (self._adj, self._sr_adj):
+            if a is not None:
+                a.free()
+        self._wit_labels, self._wit_values, self._bfs_tiles, self._adj, self._sr_adj = None, {}, None, None, None
         self.ctx.close()

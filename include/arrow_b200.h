@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 8
+#define ARROW_ABI_VERSION 9
 
 /* error codes */
 #define ARROW_OK              0
@@ -269,6 +269,31 @@ int  arrow_bits_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf,
  * X_{h-1}'s tile (x alone is read).  ARROW_ERR_ARG: non-bit tiles, no record, x not the recorded tile, out == x, rows
  * other than the adjacency's, out of another shape or k; ARROW_ERR_UNSUPPORTED: k > 8192. */
 int  arrow_bits_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf);
+
+/* ---- direction-optimising shortest and critical paths (one GPU, min-plus / max-plus on fp32 tiles) ---------------------- */
+/* The push adjacency of arrow_adj_build carrying each edge's fp32 weight (the entry's value), with the edges u == v kept
+ * (a negative self-loop changes a min-plus step); edges with an end at -1 are still dropped.  Duplicates of (u, v) come
+ * out in any order.  Temporary device memory of 24 bytes per edge is freed before the call returns; the adjacency keeps
+ * 4 (n + 1) + 8 m bytes and the frontier record of 8 n bytes.  Refusals: those of arrow_adj_build, and
+ * ARROW_ERR_UNSUPPORTED for a fp64 block.  Synchronises. */
+int  arrow_adj_build_weighted(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices,
+                              int *adj_out);
+/* values: n_edges weights, in the order of arrow_adj_d2h's indices; ARROW_ERR_ARG on an adjacency without weights */
+int  arrow_adj_values_d2h(arrow_ctx *ctx, int adj, float *values);
+/* One pass over two fp32 tiles of the adjacency's rows: *rows_changed counts the rows that differ by value (-0 == +0,
+ * NaN != NaN: arrow_dense_count_diff's figure), and the frontier record of `adj`, tagged with new_buf, lists the rows that
+ * differ in bits.  *frontier_rows is their number, *frontier_edges the sum of their rows' lengths.  Synchronises. */
+int  arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int64_t *rows_changed, int64_t *frontier_rows,
+                            int64_t *frontier_edges);
+/* out = canon(x) (fl(0 + x), NaN -> the ⊕ identity: what the identity diagonal contributes to a step), then for every
+ * recorded frontier row u and edge u -> v of weight a, t = fl(a + x[u, s]) is folded into out[v, s] with a non-returning
+ * min (MIN_PLUS) or max (MAX_PLUS) where it improves on canon(x[v, s]); NaN terms are skipped.  x must be the tile of the
+ * last arrow_sr_mark_frontier on `adj`.  When X_h is the step of X_{h-1} (with the identity), X_h <= X_{h-1} in the
+ * semiring's order, the record holds the rows where they differ and no weight is -0, out is the step of X_h bit for bit.
+ * ARROW_ERR_ARG: non-fp32 tiles, an adjacency without weights, no record, x not the recorded tile, out aliasing x, rows
+ * other than the adjacency's, out of another shape or k, an unknown semiring code; ARROW_ERR_UNSUPPORTED: PLUS_TIMES,
+ * OR_AND. */
+int  arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int semiring);
 
 /* ---- predecessors of the tropical semirings (one GPU, fp32) ------------------------------------------ */
 /* The product of arrow_spmm_sr over (value, label) pairs.  A candidate of row r is an entry p whose column c is valid
