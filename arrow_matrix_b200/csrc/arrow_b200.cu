@@ -233,8 +233,6 @@ Adj *get_adj(arrow_ctx *ctx, int h) {
     return &ctx->adjs[h];
 }
 
-inline int ceil_div_i64(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
-
 inline size_t dtype_size(int dtype) { return dtype == ARROW_F64 ? 8 : 4; }
 inline const char *dtype_name(int dtype) {
     return dtype == ARROW_F64 ? "float64" : (dtype == ARROW_I32 ? "int32" : (dtype == ARROW_B1 ? "bits" : "float32"));
@@ -327,10 +325,14 @@ struct SpmmArgs {
     float *const *__restrict__ out_ptr;  // optional destination pointer per row (nullptr entry = row dropped); overrides C / rowmap
 };
 
-// row `c` of the (possibly two-part) X operand
-__device__ __forceinline__ const float *x_row_ptr(const SpmmArgs &a, int c) {
-    if (a.X2 != nullptr && c >= a.x_split) return a.X2 + (long long)(c - a.x_split) * a.k;
-    return a.X + (long long)c * a.k;
+// row `c` of the X operand of SpmmArgs / LongArgs, whose X pointers carry elements of type T.  Only float operands come
+// in two parts (the C ABI refuses X2 for float64); for the others the test is compiled out, which lets ptxas unroll the
+// entry loops of the row-parallel kernels.
+template <class T, class Args>
+__device__ __forceinline__ const T *x_row_ptr(const Args &a, int c) {
+    if (std::is_same<T, float>::value && a.X2 != nullptr && c >= a.x_split)
+        return reinterpret_cast<const T *>(a.X2) + (long long)(c - a.x_split) * a.k;
+    return reinterpret_cast<const T *>(a.X) + (long long)c * a.k;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1241,10 +1243,31 @@ __global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles(TileArgs t) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// generic k (not a multiple of 4): warp per row, lanes over columns, scalar accesses.
+// Row-parallel kernels over a semiring: the generic kernel (k not a vector width; warp per row, lanes over columns,
+// scalar accesses) and the long-row pair (hubs of the arrow head: one CTA per segment of `segment` non-zeros writes a
+// partial to scratch, then one CTA per row reduces the partials in order -- deterministic, no atomics).  A semiring type
+// gives the element T, zero() (the ⊕ identity), plus(a, b) = a ⊕ b, mac(acc, v, x) = acc ⊕ (v ⊗ x) and kValues (false:
+// the CSR carries no values and `vals` is not read).  SpmmArgs / LongArgs carry T elements behind their float pointers.
+// Per element every kernel keeps one order, so (+, x) results match the bounds in tests/spmm_bound*.py: generic, the
+// ⊕-chain from zero() in entry order, then the old C row (accumulate), then the addend; long rows, each warp's chain
+// over entries begin + w, begin + w + 8, ..., then warps 0..7, then the slots in order, the addend and the old C row.
+// The partial kernel reduces each 128-column chunk through a fixed [8 warps][128] shared array before the next chunk,
+// so its shared memory does not grow with k (a [warps][k] array passes the H100's 227 KB per block at k > 7264 in fp32).
 // ------------------------------------------------------------------------------------------------
-template <bool ROWMAP, bool ACC>
+template <class V>
+struct PlusTimes {
+    using T = V;
+    static constexpr bool kValues = true;
+    __device__ __forceinline__ static V zero() { return V(0); }
+    __device__ __forceinline__ static V plus(V a, V b) { return a + b; }
+    __device__ __forceinline__ static V mac(V acc, V v, V x) { return fma(v, x, acc); }
+};
+
+template <class SR, bool ROWMAP, bool ACC>
 __global__ void __launch_bounds__(256) k_spmm_generic(SpmmArgs a) {
+    using T = typename SR::T;
+    const T *vals = reinterpret_cast<const T *>(a.vals);
+    const T *add_src = reinterpret_cast<const T *>(a.add_src);
     const int lane = threadIdx.x & 31;
     const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
     const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -1257,22 +1280,23 @@ __global__ void __launch_bounds__(256) k_spmm_generic(SpmmArgs a) {
             orow = __ldg(a.rowmap + row);
             if (orow < 0) continue;
         }
-        float *crow = a.C + orow * a.k;
+        T *crow = reinterpret_cast<T *>(a.C) + orow * a.k;
         if (a.out_ptr != nullptr) {
-            crow = a.out_ptr[row];
+            crow = reinterpret_cast<T *>(a.out_ptr[row]);
             if (crow == nullptr) continue;
         }
         for (int c0 = 0; c0 < a.k; c0 += 128) {
-            float acc[4] = {0.f, 0.f, 0.f, 0.f};
+            T acc[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
             for (int p = s; p < e; ++p) {
                 const int c = __ldg(a.indices + p);
-                const float v = __ldg(a.vals + p);
+                T v{};
+                if constexpr (SR::kValues) v = __ldg(vals + p);
                 if (c < 0) continue;
-                const float *xr = x_row_ptr(a, c);
+                const T *xr = x_row_ptr<T>(a, c);
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int col = c0 + lane + 32 * i;
-                    if (col < a.k) acc[i] = fmaf(v, __ldg(xr + col), acc[i]);
+                    if (col < a.k) acc[i] = SR::mac(acc[i], v, __ldg(xr + col));
                 }
             }
             const int am = (a.add_map != nullptr) ? __ldg(a.add_map + row) : -1;
@@ -1280,9 +1304,9 @@ __global__ void __launch_bounds__(256) k_spmm_generic(SpmmArgs a) {
             for (int i = 0; i < 4; ++i) {
                 const int col = c0 + lane + 32 * i;
                 if (col < a.k) {
-                    float *dst = crow + col;
-                    float r = ACC ? (*dst + acc[i]) : acc[i];
-                    if (am >= 0) r += a.add_src[(long long)am * a.k + col];
+                    T *dst = crow + col;
+                    T r = ACC ? SR::plus(*dst, acc[i]) : acc[i];
+                    if (am >= 0) r = SR::plus(r, add_src[(long long)am * a.k + col]);
                     *dst = r;
                 }
             }
@@ -1290,14 +1314,6 @@ __global__ void __launch_bounds__(256) k_spmm_generic(SpmmArgs a) {
     }
 }
 
-// ------------------------------------------------------------------------------------------------
-// long rows (hubs of the arrow head): one CTA per segment of `segment` non-zeros, partial sums to
-// scratch, then an in-order reduction per row -- deterministic, no atomics.  The partial kernels
-// reduce each 128-column chunk through a fixed [8 warps][128] shared array before the next chunk,
-// so their shared memory does not grow with k (a [warps][k] array passes the H100's 227 KB per
-// block at k > 7264 in fp32).  Per element the order is the same at every k: each warp's chain in
-// entry order, then warps 0..7.
-// ------------------------------------------------------------------------------------------------
 constexpr int LONG_WARPS = 8;        // 256 threads per partial CTA
 constexpr int LONG_CHUNK = 128;      // columns per chunk: 32 lanes x 4
 struct LongArgs {
@@ -1311,21 +1327,25 @@ struct LongArgs {
     int x_split;
 };
 
+template <class SR>
 __global__ void __launch_bounds__(256) k_spmm_long_partial(LongArgs a) {
-    __shared__ float red[LONG_WARPS][LONG_CHUNK];
+    using T = typename SR::T;
+    __shared__ T red[LONG_WARPS][LONG_CHUNK];
+    const T *vals = reinterpret_cast<const T *>(a.vals);
     const LongTask t = a.tasks[blockIdx.x];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int c0 = 0; c0 < a.k; c0 += LONG_CHUNK) {
-        float acc[4] = {0.f, 0.f, 0.f, 0.f};
+        T acc[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
         for (int p = t.begin + warp; p < t.end; p += LONG_WARPS) {
             const int c = __ldg(a.indices + p);
-            const float v = __ldg(a.vals + p);
+            T v{};
+            if constexpr (SR::kValues) v = __ldg(vals + p);
             if (c < 0) continue;
-            const float *xr = (a.X2 != nullptr && c >= a.x_split) ? a.X2 + (long long)(c - a.x_split) * a.k : a.X + (long long)c * a.k;
+            const T *xr = x_row_ptr<T>(a, c);
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int col = c0 + lane + 32 * i;
-                if (col < a.k) acc[i] = fmaf(v, __ldg(xr + col), acc[i]);
+                if (col < a.k) acc[i] = SR::mac(acc[i], v, __ldg(xr + col));
             }
         }
 #pragma unroll
@@ -1333,42 +1353,42 @@ __global__ void __launch_bounds__(256) k_spmm_long_partial(LongArgs a) {
         __syncthreads();
         const int col = c0 + threadIdx.x;
         if (threadIdx.x < LONG_CHUNK && col < a.k) {
-            float sum = 0.f;
-            for (int w = 0; w < LONG_WARPS; ++w) sum += red[w][threadIdx.x];
-            a.scratch[(long long)t.slot * a.k + col] = sum;
+            T sum = SR::zero();
+            for (int w = 0; w < LONG_WARPS; ++w) sum = SR::plus(sum, red[w][threadIdx.x]);
+            reinterpret_cast<T *>(a.scratch)[(long long)t.slot * a.k + col] = sum;
         }
         __syncthreads();
     }
 }
 
-template <bool ROWMAP, bool ACC>
-__global__ void __launch_bounds__(128) k_spmm_long_reduce(const int *__restrict__ long_rows,
+template <class SR, bool ROWMAP, bool ACC>
+__global__ void __launch_bounds__(128) k_spmm_long_reduce(SpmmArgs a, const int *__restrict__ long_rows,
                                                           const int *__restrict__ long_first,
-                                                          const float *__restrict__ scratch,
-                                                          float *__restrict__ C, const int *__restrict__ rowmap, int k,
-                                                          const float *__restrict__ add_src, const int *__restrict__ add_map,
-                                                          float *const *__restrict__ out_ptr) {
+                                                          const typename SR::T *__restrict__ scratch) {
+    using T = typename SR::T;
+    const T *add_src = reinterpret_cast<const T *>(a.add_src);
+    const int k = a.k;
     const int r = long_rows[blockIdx.x];
     long long orow = r;
     if (ROWMAP) {
-        orow = rowmap[r];
+        orow = a.rowmap[r];
         if (orow < 0) return;
     }
-    float *crow = C + orow * k;
-    if (out_ptr != nullptr) {
-        crow = out_ptr[r];
+    T *crow = reinterpret_cast<T *>(a.C) + orow * k;
+    if (a.out_ptr != nullptr) {
+        crow = reinterpret_cast<T *>(a.out_ptr[r]);
         if (crow == nullptr) return;
     }
     const int s0 = long_first[blockIdx.x], s1 = long_first[blockIdx.x + 1];
     for (int col = threadIdx.x; col < k; col += blockDim.x) {
-        float sum = 0.f;
-        for (int s = s0; s < s1; ++s) sum += scratch[(long long)s * k + col];
-        if (add_map != nullptr) {
-            const int am = add_map[r];
-            if (am >= 0) sum += add_src[(long long)am * k + col];
+        T sum = SR::zero();
+        for (int s = s0; s < s1; ++s) sum = SR::plus(sum, scratch[(long long)s * k + col]);
+        if (a.add_map != nullptr) {
+            const int am = a.add_map[r];
+            if (am >= 0) sum = SR::plus(sum, add_src[(long long)am * k + col]);
         }
-        float *dst = crow + col;
-        *dst = ACC ? (*dst + sum) : sum;
+        T *dst = crow + col;
+        *dst = ACC ? SR::plus(*dst, sum) : sum;
     }
 }
 
@@ -1377,7 +1397,7 @@ __global__ void __launch_bounds__(128) k_spmm_long_reduce(const int *__restrict_
 // slices streamed by cp.async.bulk on an mbarrier, two stages, persistent CTAs on the atomic ticket, a lane group per
 // row -- with X and C moved as double2 (16 B: the vector path needs k % 2 == 0) and 8-byte values in shared memory.
 // Every element is one fma chain in entry order (after the old C row or the addend), so a result does not depend on
-// the grid.  The generic and long-row kernels are the fp32 ones in double.
+// the grid.  The generic and long-row kernels are the row-parallel templates on PlusTimes<double>.
 // ------------------------------------------------------------------------------------------------
 struct SpmmArgsF64 {
     const int *__restrict__ indptr;
@@ -1573,117 +1593,6 @@ __global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles_f64(TileArgsF64 
         }
         __syncthreads();            // stage `st` may be refilled by the next iteration's copy
         tile = s_next[st];
-    }
-}
-
-// odd k or k > 256: warp per row, lanes over columns, scalar accesses
-template <bool ROWMAP, bool ACC>
-__global__ void __launch_bounds__(256) k_spmm_generic_f64(SpmmArgsF64 a) {
-    const int lane = threadIdx.x & 31;
-    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
-    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    for (long long row = warp_id; row < a.n_rows; row += warps_total) {
-        const int s = __ldg(a.indptr + row);
-        const int e = __ldg(a.indptr + row + 1);
-        if (e - s > a.long_threshold) continue;
-        long long orow = row;
-        if (ROWMAP) {
-            orow = __ldg(a.rowmap + row);
-            if (orow < 0) continue;
-        }
-        double *crow = a.C + orow * a.k;
-        for (int c0 = 0; c0 < a.k; c0 += 128) {
-            double acc[4] = {0.0, 0.0, 0.0, 0.0};
-            for (int p = s; p < e; ++p) {
-                const int c = __ldg(a.indices + p);
-                const double v = __ldg(a.vals + p);
-                if (c < 0) continue;
-                const double *xr = a.X + (long long)c * a.k;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int col = c0 + lane + 32 * i;
-                    if (col < a.k) acc[i] = fma(v, __ldg(xr + col), acc[i]);
-                }
-            }
-            const int am = (a.add_map != nullptr) ? __ldg(a.add_map + row) : -1;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int col = c0 + lane + 32 * i;
-                if (col < a.k) {
-                    double *dst = crow + col;
-                    double r = ACC ? (*dst + acc[i]) : acc[i];
-                    if (am >= 0) r += a.add_src[(long long)am * a.k + col];
-                    *dst = r;
-                }
-            }
-        }
-    }
-}
-
-// long rows: segment partials to scratch, then the in-order reduction (k_spmm_long_partial / k_spmm_long_reduce)
-struct LongArgsF64 {
-    const LongTask *__restrict__ tasks;
-    const int *__restrict__ indices;
-    const double *__restrict__ vals;
-    const double *__restrict__ X;
-    double *__restrict__ scratch;     // [slot][k]
-    int k;
-};
-
-__global__ void __launch_bounds__(256) k_spmm_long_partial_f64(LongArgsF64 a) {
-    __shared__ double red_f64[LONG_WARPS][LONG_CHUNK];
-    const LongTask t = a.tasks[blockIdx.x];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int c0 = 0; c0 < a.k; c0 += LONG_CHUNK) {
-        double acc[4] = {0.0, 0.0, 0.0, 0.0};
-        for (int p = t.begin + warp; p < t.end; p += LONG_WARPS) {
-            const int c = __ldg(a.indices + p);
-            const double v = __ldg(a.vals + p);
-            if (c < 0) continue;
-            const double *xr = a.X + (long long)c * a.k;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int col = c0 + lane + 32 * i;
-                if (col < a.k) acc[i] = fma(v, __ldg(xr + col), acc[i]);
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) red_f64[warp][lane + 32 * i] = acc[i];
-        __syncthreads();
-        const int col = c0 + threadIdx.x;
-        if (threadIdx.x < LONG_CHUNK && col < a.k) {
-            double sum = 0.0;
-            for (int w = 0; w < LONG_WARPS; ++w) sum += red_f64[w][threadIdx.x];
-            a.scratch[(long long)t.slot * a.k + col] = sum;
-        }
-        __syncthreads();
-    }
-}
-
-template <bool ROWMAP, bool ACC>
-__global__ void __launch_bounds__(128) k_spmm_long_reduce_f64(const int *__restrict__ long_rows,
-                                                              const int *__restrict__ long_first,
-                                                              const double *__restrict__ scratch,
-                                                              double *__restrict__ C, const int *__restrict__ rowmap, int k,
-                                                              const double *__restrict__ add_src,
-                                                              const int *__restrict__ add_map) {
-    const int r = long_rows[blockIdx.x];
-    long long orow = r;
-    if (ROWMAP) {
-        orow = rowmap[r];
-        if (orow < 0) return;
-    }
-    double *crow = C + orow * k;
-    const int s0 = long_first[blockIdx.x], s1 = long_first[blockIdx.x + 1];
-    for (int col = threadIdx.x; col < k; col += blockDim.x) {
-        double sum = 0.0;
-        for (int s = s0; s < s1; ++s) sum += scratch[(long long)s * k + col];
-        if (add_map != nullptr) {
-            const int am = add_map[r];
-            if (am >= 0) sum += add_src[(long long)am * k + col];
-        }
-        double *dst = crow + col;
-        *dst = ACC ? (*dst + sum) : sum;
     }
 }
 
@@ -1939,6 +1848,99 @@ int grid_for(arrow_ctx *ctx, const void *fn, int threads, size_t smem, long long
     return (int)g;
 }
 
+// f(ROWMAP, ACC) with both as std::bool_constant; only (+, x) has the row-map and accumulate epilogues
+template <class SR, class F>
+void with_epilogue(bool rowmap, bool acc, F &&f) {
+    if constexpr (std::is_same<SR, PlusTimes<typename SR::T>>::value) {
+        if (rowmap && acc) f(std::true_type{}, std::true_type{});
+        else if (rowmap) f(std::true_type{}, std::false_type{});
+        else if (acc) f(std::false_type{}, std::true_type{});
+        else f(std::false_type{}, std::false_type{});
+    } else {
+        f(std::false_type{}, std::false_type{});
+    }
+}
+
+// the generic kernel over every row of `a` (rows past the long-row threshold are left to launch_long_rows)
+template <class SR>
+void launch_generic(arrow_ctx *ctx, const SpmmArgs &a, bool rowmap, bool acc) {
+    with_epilogue<SR>(rowmap, acc, [&](auto rm, auto ac) {
+        auto fn = k_spmm_generic<SR, decltype(rm)::value, decltype(ac)::value>;
+        const int grid = grid_for(ctx, (const void *)fn, 256, 0, (a.n_rows + 7) / 8);
+        fn<<<grid, 256, 0, cur_stream(ctx)>>>(a);
+    });
+    ctx->launches++;
+}
+
+// Grows the current lane's long-row scratch to at least `need` bytes.  Growing frees and allocates, which a graph
+// capture cannot record: the step has to run once outside the capture first.
+int grow_long_scratch(arrow_ctx *ctx, size_t need) {
+    const int lane = ctx->cur_lane;
+    if (need <= ctx->long_scratch_bytes[lane]) return ARROW_OK;
+    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
+    CUDA_TRY(ctx, cudaStreamSynchronize(cur_stream(ctx)));
+    if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
+    ctx->long_scratch[lane] = nullptr;
+    ctx->long_scratch_bytes[lane] = 0;
+    CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
+    ctx->long_scratch_bytes[lane] = need;
+    return ARROW_OK;
+}
+
+// the long rows of A: segment partials into the lane's scratch, then the in-order reduction with a's epilogue
+template <class SR>
+int launch_long_rows(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool rowmap, bool acc) {
+    using T = typename SR::T;
+    if (A->n_long_tasks == 0) return ARROW_OK;
+    const int rc = grow_long_scratch(ctx, (size_t)A->n_long_tasks * a.k * sizeof(T));
+    if (rc != ARROW_OK) return rc;
+    cudaStream_t stream = cur_stream(ctx);
+    LongArgs la;
+    la.tasks = A->long_tasks;
+    la.indices = a.indices;
+    la.vals = a.vals;
+    la.X = a.X;
+    la.scratch = ctx->long_scratch[ctx->cur_lane];
+    la.k = a.k;
+    la.X2 = a.X2;
+    la.x_split = a.x_split;
+    k_spmm_long_partial<SR><<<A->n_long_tasks, 256, 0, stream>>>(la);
+    ctx->launches++;
+    with_epilogue<SR>(rowmap, acc, [&](auto rm, auto ac) {
+        k_spmm_long_reduce<SR, decltype(rm)::value, decltype(ac)::value><<<A->n_long_rows, 128, 0, stream>>>(
+            a, A->long_rows, A->long_first, reinterpret_cast<const T *>(la.scratch));
+    });
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return ARROW_OK;
+}
+
+// A persistent tile kernel: as many CTAs as are resident (capped by ARROW_OPT_SPMM_CTAS_PER_SM / _SPMM_SM_LIMIT), at
+// most one per tile, taking tiles from the atomic ticket.  KERNEL is a template argument so that each kernel keeps its
+// own per-device attribute and occupancy cache.
+template <auto KERNEL, size_t SMEM, class Args>
+int launch_persistent(arrow_ctx *ctx, const Args &args, int n_tiles, int *ticket) {
+    static bool attr_set[64] = {};            /* function attributes are per device */
+    static int occ_dev[64] = {};
+    const int dv = ctx->device & 63;
+    if (!attr_set[dv]) {
+        cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], KERNEL, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
+        attr_set[dv] = true;
+    }
+    const int occ = occ_dev[dv];
+    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
+    int sms = ctx->sm_count;
+    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
+    int grid = (int)std::min<long long>((long long)per_sm * sms, n_tiles);
+    // the scheduler words are zeroed before every launch: the round-1 kernel (which shares them) leaves its ticket behind,
+    // and a launch must never depend on how the previous one on this lane ended
+    cudaMemsetAsync(ticket, 0, 2 * sizeof(int), cur_stream(ctx));
+    KERNEL<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(args);
+    ctx->launches++;
+    return ARROW_OK;
+}
+
 template <int G, int VPL>
 int launch_vec(arrow_ctx *ctx, const SpmmArgs &a, bool rowmap, bool acc, int variant) {
     constexpr int RPW = 32 / G;
@@ -1999,55 +2001,19 @@ struct TileLaunch {
 
 template <int G, int VPL, int OUT, bool ACC, int TR, int TN, int RPG, int MINB, bool DUALX>
 int launch_tiles_one(arrow_ctx *ctx, const TileArgs &t) {
-    constexpr size_t SMEM = TileCfg<TR, TN>::SMEM_BYTES;
-    auto fn = k_spmm_tiles<G, VPL, OUT, ACC, TR, TN, RPG, MINB, DUALX>;
-    static bool attr_set[64] = {};            /* function attributes are per device */
-    static int occ_dev[64] = {};
-    const int dv = ctx->device & 63;
-    if (!attr_set[dv]) {
-        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
-        attr_set[dv] = true;
-    }
+    constexpr auto fn = k_spmm_tiles<G, VPL, OUT, ACC, TR, TN, RPG, MINB, DUALX>;
     static int carve_dev[64];
+    const int dv = ctx->device & 63;
     if (ctx->smem_carveout != carve_dev[dv] - 1000) {       // measurement switch: how much of the 256 KB is L1
         cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, ctx->smem_carveout);
         carve_dev[dv] = ctx->smem_carveout + 1000;
     }
-    const int occ = occ_dev[dv];
-    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
-    int sms = ctx->sm_count;
-    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
-    int grid = (int)std::min<long long>((long long)per_sm * sms, t.n_tiles);
-    // the scheduler words are zeroed before every launch: the round-1 kernel (which shares them) leaves its ticket behind,
-    // and a launch must never depend on how the previous one on this lane ended
-    cudaMemsetAsync(t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
-    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(t);
-    ctx->launches++;
-    return ARROW_OK;
+    return launch_persistent<fn, TileCfg<TR, TN>::SMEM_BYTES>(ctx, t, t.n_tiles, t.ticket);
 }
 
 template <int G, int VPL, bool ROWMAP, bool ACC, int TR, int TN>
 int launch_tiles_v1(arrow_ctx *ctx, const TileArgs &t) {
-    constexpr size_t SMEM = TileCfg<TR, TN>::SMEM_BYTES;
-    auto fn = k_spmm_tiles_v1<G, VPL, ROWMAP, ACC, TR, TN>;
-    static bool attr_set[64] = {};
-    static int occ_dev[64] = {};
-    const int dv = ctx->device & 63;
-    if (!attr_set[dv]) {
-        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
-        attr_set[dv] = true;
-    }
-    const int occ = occ_dev[dv];
-    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
-    int sms = ctx->sm_count;
-    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
-    int grid = (int)std::min<long long>((long long)per_sm * sms, t.n_tiles);
-    cudaMemsetAsync(t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
-    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(t);
-    ctx->launches++;
-    return ARROW_OK;
+    return launch_persistent<k_spmm_tiles_v1<G, VPL, ROWMAP, ACC, TR, TN>, TileCfg<TR, TN>::SMEM_BYTES>(ctx, t, t.n_tiles, t.ticket);
 }
 
 template <int G, int VPL, int TR, int TN, int RPG, int MINB>
@@ -2147,25 +2113,7 @@ int pick_variant(int k) {
 // ---- float64 dispatch (one GPU): the tile kernel for even k <= 256, the generic kernel otherwise, long rows as fp32 ----
 template <int G, int VPL, bool ROWMAP, bool ACC>
 int launch_tiles_f64_one(arrow_ctx *ctx, const TileArgsF64 &t) {
-    constexpr size_t SMEM = TileCfgF64::SMEM_BYTES;
-    auto fn = k_spmm_tiles_f64<G, VPL, ROWMAP, ACC>;
-    static bool attr_set[64] = {};            /* function attributes are per device */
-    static int occ_dev[64] = {};
-    const int dv = ctx->device & 63;
-    if (!attr_set[dv]) {
-        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
-        attr_set[dv] = true;
-    }
-    const int occ = occ_dev[dv];
-    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
-    int sms = ctx->sm_count;
-    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
-    int grid = (int)std::min<long long>((long long)per_sm * sms, t.n_tiles);
-    cudaMemsetAsync(t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
-    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(t);
-    ctx->launches++;
-    return ARROW_OK;
+    return launch_persistent<k_spmm_tiles_f64<G, VPL, ROWMAP, ACC>, TileCfgF64::SMEM_BYTES>(ctx, t, t.n_tiles, t.ticket);
 }
 
 template <int G, int VPL>
@@ -2194,79 +2142,34 @@ int launch_tiles_f64(arrow_ctx *ctx, const TileArgsF64 &t, bool rowmap, bool acc
 
 // the product of spmm_impl for float64 operands; `a` carries the validated operands (value / tile pointers are double)
 int spmm_f64(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool rowmap, bool acc) {
-    SpmmArgsF64 b;
-    b.indptr = a.indptr;
-    b.indices = a.indices;
-    b.vals = reinterpret_cast<const double *>(a.vals);
-    b.X = reinterpret_cast<const double *>(a.X);
-    b.C = reinterpret_cast<double *>(a.C);
-    b.rowmap = a.rowmap;
-    b.n_rows = a.n_rows;
-    b.k = a.k;
-    b.k2 = a.k / 2;
-    b.long_threshold = a.long_threshold;
-    b.add_src = reinterpret_cast<const double *>(a.add_src);
-    b.add_map = a.add_map;
     const int k = a.k;
-    const int lane = ctx->cur_lane;
-    cudaStream_t stream = cur_stream(ctx);
     if (k % 2 != 0 || k > 256) {
-        const long long ctas = (A->n_rows + 7) / 8;
-#define LAUNCH_G64(KERNEL)                                                                            \
-    do {                                                                                              \
-        auto fn = KERNEL;                                                                             \
-        int grid = grid_for(ctx, (const void *)fn, 256, 0, ctas);                                     \
-        fn<<<grid, 256, 0, stream>>>(b);                                                              \
-    } while (0)
-        if (rowmap && acc) LAUNCH_G64((k_spmm_generic_f64<true, true>));
-        else if (rowmap) LAUNCH_G64((k_spmm_generic_f64<true, false>));
-        else if (acc) LAUNCH_G64((k_spmm_generic_f64<false, true>));
-        else LAUNCH_G64((k_spmm_generic_f64<false, false>));
-#undef LAUNCH_G64
-        ctx->launches++;
+        launch_generic<PlusTimes<double>>(ctx, a, rowmap, acc);
     } else if (A->n_tiles[TILE_LIST_SMALL] > 0) {
         TileArgsF64 t;
-        t.a = b;
+        t.a.indptr = a.indptr;
+        t.a.indices = a.indices;
+        t.a.vals = reinterpret_cast<const double *>(a.vals);
+        t.a.X = reinterpret_cast<const double *>(a.X);
+        t.a.C = reinterpret_cast<double *>(a.C);
+        t.a.rowmap = a.rowmap;
+        t.a.n_rows = a.n_rows;
+        t.a.k = k;
+        t.a.k2 = k / 2;
+        t.a.long_threshold = a.long_threshold;
+        t.a.add_src = reinterpret_cast<const double *>(a.add_src);
+        t.a.add_map = a.add_map;
         const int list = tile_list_for(ctx, k, 8, false);              // one tile kernel size: TR = 64
         t.tiles = A->tiles[list];
         t.n_tiles = A->n_tiles[list];
         t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
-        t.ticket = ctx->tile_ticket + 2 * lane;
+        t.ticket = ctx->tile_ticket + 2 * ctx->cur_lane;
         t.l2_hints = (rowmap || acc) ? ctx->l2_hints_fused : ctx->l2_hints_plain;
         const int rc = launch_tiles_f64(ctx, t, rowmap, acc);
         if (rc != ARROW_OK) return rc;
     }
     CUDA_TRY(ctx, cudaGetLastError());
-
-    if (A->n_long_tasks > 0) {
-        const size_t need = (size_t)A->n_long_tasks * k * sizeof(double);
-        if (need > ctx->long_scratch_bytes[lane]) {
-            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
-            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
-            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
-            ctx->long_scratch[lane] = nullptr;
-            ctx->long_scratch_bytes[lane] = 0;
-            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
-            ctx->long_scratch_bytes[lane] = need;
-        }
-        double *scr = reinterpret_cast<double *>(ctx->long_scratch[lane]);
-        LongArgsF64 la;
-        la.tasks = A->long_tasks;
-        la.indices = b.indices;
-        la.vals = b.vals;
-        la.X = b.X;
-        la.scratch = scr;
-        la.k = k;
-        k_spmm_long_partial_f64<<<A->n_long_tasks, 256, 0, stream>>>(la);
-        ctx->launches++;
-        if (rowmap && acc) k_spmm_long_reduce_f64<true, true><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
-        else if (rowmap) k_spmm_long_reduce_f64<true, false><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
-        else if (acc) k_spmm_long_reduce_f64<false, true><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
-        else k_spmm_long_reduce_f64<false, false><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, b.C, b.rowmap, k, b.add_src, b.add_map);
-        ctx->launches++;
-        CUDA_TRY(ctx, cudaGetLastError());
-    }
-    return ARROW_OK;
+    return launch_long_rows<PlusTimes<double>>(ctx, A, a, rowmap, acc);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2276,14 +2179,20 @@ int spmm_f64(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool rowmap, bool 
 // and times(); (+, x) keeps the kernels above.
 // ------------------------------------------------------------------------------------------------
 struct SrMinPlus {
+    using T = float;
+    static constexpr bool kValues = true;
     __device__ __forceinline__ static float zero() { return __int_as_float(0x7f800000); }       // +inf
     __device__ __forceinline__ static float plus(float a, float b) { return fminf(a, b); }
     __device__ __forceinline__ static float times(float a, float x) { return __fadd_rn(a, x); }
+    __device__ __forceinline__ static float mac(float acc, float v, float x) { return plus(acc, times(v, x)); }
 };
 struct SrMaxPlus {
+    using T = float;
+    static constexpr bool kValues = true;
     __device__ __forceinline__ static float zero() { return __int_as_float(0xff800000); }       // -inf
     __device__ __forceinline__ static float plus(float a, float b) { return fmaxf(a, b); }
     __device__ __forceinline__ static float times(float a, float x) { return __fadd_rn(a, x); }
+    __device__ __forceinline__ static float mac(float acc, float v, float x) { return plus(acc, times(v, x)); }
 };
 
 template <class SR>
@@ -2456,95 +2365,6 @@ __global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles_sr(TileArgs t) {
     }
 }
 
-// k not a multiple of 4 or k > 256: warp per row, lanes over columns, scalar accesses
-template <class SR>
-__global__ void __launch_bounds__(256) k_spmm_generic_sr(SpmmArgs a) {
-    const int lane = threadIdx.x & 31;
-    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
-    const long long warp_id = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    for (long long row = warp_id; row < a.n_rows; row += warps_total) {
-        const int s = __ldg(a.indptr + row);
-        const int e = __ldg(a.indptr + row + 1);
-        if (e - s > a.long_threshold) continue;
-        float *crow = a.C + row * a.k;
-        const int am = (a.add_map != nullptr) ? __ldg(a.add_map + row) : -1;
-        for (int c0 = 0; c0 < a.k; c0 += 128) {
-            float acc[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
-            for (int p = s; p < e; ++p) {
-                const int c = __ldg(a.indices + p);
-                const float v = __ldg(a.vals + p);
-                if (c < 0) continue;
-                const float *xr = a.X + (long long)c * a.k;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int col = c0 + lane + 32 * i;
-                    if (col < a.k) acc[i] = SR::plus(acc[i], SR::times(v, __ldg(xr + col)));
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int col = c0 + lane + 32 * i;
-                if (col < a.k) {
-                    float r = acc[i];
-                    if (am >= 0) r = SR::plus(r, a.add_src[(long long)am * a.k + col]);
-                    crow[col] = r;
-                }
-            }
-        }
-    }
-}
-
-// long rows: one CTA per segment ⊕-reduces its entries into a scratch slot, then one CTA per row ⊕-reduces the slots and
-// the addend (k_spmm_long_partial / k_spmm_long_reduce)
-template <class SR>
-__global__ void __launch_bounds__(256) k_spmm_long_partial_sr(LongArgs a) {
-    __shared__ float red_sr[LONG_WARPS][LONG_CHUNK];
-    const LongTask t = a.tasks[blockIdx.x];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int c0 = 0; c0 < a.k; c0 += LONG_CHUNK) {
-        float acc[4] = {SR::zero(), SR::zero(), SR::zero(), SR::zero()};
-        for (int p = t.begin + warp; p < t.end; p += LONG_WARPS) {
-            const int c = __ldg(a.indices + p);
-            const float v = __ldg(a.vals + p);
-            if (c < 0) continue;
-            const float *xr = a.X + (long long)c * a.k;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int col = c0 + lane + 32 * i;
-                if (col < a.k) acc[i] = SR::plus(acc[i], SR::times(v, __ldg(xr + col)));
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) red_sr[warp][lane + 32 * i] = acc[i];
-        __syncthreads();
-        const int col = c0 + threadIdx.x;
-        if (threadIdx.x < LONG_CHUNK && col < a.k) {
-            float r = SR::zero();
-            for (int w = 0; w < LONG_WARPS; ++w) r = SR::plus(r, red_sr[w][threadIdx.x]);
-            a.scratch[(long long)t.slot * a.k + col] = r;
-        }
-        __syncthreads();
-    }
-}
-
-template <class SR>
-__global__ void __launch_bounds__(128) k_spmm_long_reduce_sr(const int *__restrict__ long_rows,
-                                                             const int *__restrict__ long_first,
-                                                             const float *__restrict__ scratch, float *__restrict__ C,
-                                                             int k, const float *__restrict__ add_src,
-                                                             const int *__restrict__ add_map) {
-    const int r = long_rows[blockIdx.x];
-    float *crow = C + (long long)r * k;
-    const int am = (add_map != nullptr) ? add_map[r] : -1;
-    const int s0 = long_first[blockIdx.x], s1 = long_first[blockIdx.x + 1];
-    for (int col = threadIdx.x; col < k; col += blockDim.x) {
-        float acc = SR::zero();
-        for (int s = s0; s < s1; ++s) acc = SR::plus(acc, scratch[(long long)s * k + col]);
-        if (am >= 0) acc = SR::plus(acc, add_src[(long long)am * k + col]);
-        crow[col] = acc;
-    }
-}
-
 // dst[r] = dst[r] ⊕ src[map[r]] (map[r] >= 0): the backward exchange of a semiring step (k_gather_rows without peers)
 template <typename VT, int G, class SR>
 __global__ void __launch_bounds__(256) k_gather_rows_sr(VT *__restrict__ dst, const VT *__restrict__ src,
@@ -2597,25 +2417,7 @@ __global__ void __launch_bounds__(256) k_count_diff(const T *__restrict__ a, con
 
 template <int G, int VPL, class SR, int TR, int TN>
 int launch_tiles_sr_one(arrow_ctx *ctx, const TileArgs &t) {
-    constexpr size_t SMEM = TileCfg<TR, TN>::SMEM_BYTES;
-    auto fn = k_spmm_tiles_sr<G, VPL, SR, TR, TN>;
-    static bool attr_set[64] = {};            /* function attributes are per device */
-    static int occ_dev[64] = {};
-    const int dv = ctx->device & 63;
-    if (!attr_set[dv]) {
-        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
-        attr_set[dv] = true;
-    }
-    const int occ = occ_dev[dv];
-    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
-    int sms = ctx->sm_count;
-    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
-    int grid = (int)std::min<long long>((long long)per_sm * sms, t.n_tiles);
-    cudaMemsetAsync(t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
-    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(t);
-    ctx->launches++;
-    return ARROW_OK;
+    return launch_persistent<k_spmm_tiles_sr<G, VPL, SR, TR, TN>, TileCfg<TR, TN>::SMEM_BYTES>(ctx, t, t.n_tiles, t.ticket);
 }
 
 // (lanes per row, float4 per lane) and tile size as launch_tiles picks them for a plain launch with the default options
@@ -2645,54 +2447,20 @@ int launch_tiles_sr_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A, bool min_pl
 template <class SR>
 int spmm_sr(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool min_plus) {
     const int k = a.k;
-    const int lane = ctx->cur_lane;
-    cudaStream_t stream = cur_stream(ctx);
     if (k % 4 != 0 || k > 256) {
-        const long long ctas = (A->n_rows + 7) / 8;
-        auto fn = k_spmm_generic_sr<SR>;
-        const int grid = grid_for(ctx, (const void *)fn, 256, 0, ctas);
-        fn<<<grid, 256, 0, stream>>>(a);
-        ctx->launches++;
+        launch_generic<SR>(ctx, a, false, false);
     } else if (A->n_tiles[TILE_LIST_SMALL] > 0) {
         TileArgs t;
         t.a = a;
         t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
-        t.ticket = ctx->tile_ticket + 2 * lane;
+        t.ticket = ctx->tile_ticket + 2 * ctx->cur_lane;
         t.l2_hints = ctx->l2_hints_plain;
         t.prefetch = 0;
         const int rc = launch_tiles_sr_shape(ctx, t, A, min_plus);
         if (rc != ARROW_OK) return rc;
     }
     CUDA_TRY(ctx, cudaGetLastError());
-
-    if (A->n_long_tasks > 0) {
-        const size_t need = (size_t)A->n_long_tasks * k * 4;
-        if (need > ctx->long_scratch_bytes[lane]) {
-            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
-            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
-            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
-            ctx->long_scratch[lane] = nullptr;
-            ctx->long_scratch_bytes[lane] = 0;
-            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
-            ctx->long_scratch_bytes[lane] = need;
-        }
-        LongArgs la;
-        la.tasks = A->long_tasks;
-        la.indices = a.indices;
-        la.vals = a.vals;
-        la.X = a.X;
-        la.scratch = ctx->long_scratch[lane];
-        la.k = k;
-        la.X2 = nullptr;
-        la.x_split = 0;
-        k_spmm_long_partial_sr<SR><<<A->n_long_tasks, 256, 0, stream>>>(la);
-        ctx->launches++;
-        k_spmm_long_reduce_sr<SR><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, la.scratch, a.C, k,
-                                                                       a.add_src, a.add_map);
-        ctx->launches++;
-        CUDA_TRY(ctx, cudaGetLastError());
-    }
-    return ARROW_OK;
+    return launch_long_rows<SR>(ctx, A, a, false, false);
 }
 
 template <class SR>
@@ -2741,7 +2509,6 @@ int gather_rows_sr(arrow_ctx *ctx, DenseBuf *D, const DenseBuf *S, const IdxMap 
 __device__ __forceinline__ void u4_or(uint4 &acc, const uint4 &x) {
     acc.x |= x.x; acc.y |= x.y; acc.z |= x.z; acc.w |= x.w;
 }
-__device__ __forceinline__ uint4 u4_zero() { return make_uint4(0u, 0u, 0u, 0u); }
 __device__ __forceinline__ void u4_or(unsigned &acc, const unsigned &x) { acc |= x; }        // one-word rows
 template <class V> __device__ __forceinline__ V v_zero();
 template <> __device__ __forceinline__ uint4 v_zero<uint4>() { return make_uint4(0u, 0u, 0u, 0u); }
@@ -2894,58 +2661,14 @@ __global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles_bits(TileArgs t)
     }
 }
 
-// long rows: one CTA per segment ORs its entries' X rows into a scratch slot (warps over entries, lanes over words), then
-// one CTA per row ORs the slots and the addend (k_spmm_long_partial / k_spmm_long_reduce on words)
-__global__ void __launch_bounds__(256) k_spmm_long_partial_bits(LongArgs a) {
-    extern __shared__ unsigned int red_bits[];   // [warps][words]
-    const LongTask t = a.tasks[blockIdx.x];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-    const int words = a.k;                        // a.k carries the row's words here
-    const unsigned int *X = reinterpret_cast<const unsigned int *>(a.X);
-    for (int c0 = 0; c0 < words; c0 += 128) {
-        unsigned int acc[4] = {0u, 0u, 0u, 0u};
-        for (int p = t.begin + warp; p < t.end; p += nwarps) {
-            const int c = __ldg(a.indices + p);
-            if (c < 0) continue;
-            const unsigned int *xr = X + (long long)c * words;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int w = c0 + lane + 32 * i;
-                if (w < words) acc[i] |= __ldg(xr + w);
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int w = c0 + lane + 32 * i;
-            if (w < words) red_bits[warp * words + w] = acc[i];
-        }
-    }
-    __syncthreads();
-    unsigned int *scratch = reinterpret_cast<unsigned int *>(a.scratch);
-    for (int w = threadIdx.x; w < words; w += blockDim.x) {
-        unsigned int r = 0u;
-        for (int q = 0; q < nwarps; ++q) r |= red_bits[q * words + w];
-        scratch[(long long)t.slot * words + w] = r;
-    }
-}
-
-__global__ void __launch_bounds__(128) k_spmm_long_reduce_bits(const int *__restrict__ long_rows,
-                                                               const int *__restrict__ long_first,
-                                                               const unsigned int *__restrict__ scratch,
-                                                               unsigned int *__restrict__ C, int words,
-                                                               const unsigned int *__restrict__ add_src,
-                                                               const int *__restrict__ add_map) {
-    const int r = long_rows[blockIdx.x];
-    unsigned int *crow = C + (long long)r * words;
-    const int am = (add_map != nullptr) ? add_map[r] : -1;
-    const int s0 = long_first[blockIdx.x], s1 = long_first[blockIdx.x + 1];
-    for (int w = threadIdx.x; w < words; w += blockDim.x) {
-        unsigned int acc = 0u;
-        for (int s = s0; s < s1; ++s) acc |= scratch[(long long)s * words + w];
-        if (am >= 0) acc |= add_src[(long long)am * words + w];
-        crow[w] = acc;
-    }
-}
+// (or, and) for the row-parallel long-row kernels, on uint32 words (a.k carries the row's words)
+struct OrAnd {
+    using T = unsigned;
+    static constexpr bool kValues = false;
+    __device__ __forceinline__ static unsigned zero() { return 0u; }
+    __device__ __forceinline__ static unsigned plus(unsigned a, unsigned b) { return a | b; }
+    __device__ __forceinline__ static unsigned mac(unsigned acc, unsigned, unsigned x) { return acc | x; }
+};
 
 // dst[r] |= src[map[r]] (map[r] >= 0): the backward exchange of an (or, and) step; a lane group of G lanes per row,
 // whole uint4 of the padded rows
@@ -3032,25 +2755,7 @@ __global__ void __launch_bounds__(256) k_bits_mark_new(const unsigned int *__res
 
 template <int G, int VPL, int TR, int TN, class V = uint4>
 int launch_tiles_bits_one(arrow_ctx *ctx, const TileArgs &t) {
-    constexpr size_t SMEM = TileCfgBits<TR, TN>::SMEM_BYTES;
-    auto fn = k_spmm_tiles_bits<G, VPL, TR, TN, V>;
-    static bool attr_set[64] = {};            /* function attributes are per device */
-    static int occ_dev[64] = {};
-    const int dv = ctx->device & 63;
-    if (!attr_set[dv]) {
-        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
-        attr_set[dv] = true;
-    }
-    const int occ = occ_dev[dv];
-    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
-    int sms = ctx->sm_count;
-    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
-    int grid = (int)std::min<long long>((long long)per_sm * sms, t.n_tiles);
-    cudaMemsetAsync(t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
-    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(t);
-    ctx->launches++;
-    return ARROW_OK;
+    return launch_persistent<k_spmm_tiles_bits<G, VPL, TR, TN, V>, TileCfgBits<TR, TN>::SMEM_BYTES>(ctx, t, t.n_tiles, t.ticket);
 }
 
 // (lanes per row, uint4 per lane) from k4 = words / 4 as launch_tiles_sr_shape picks them from an fp32 row of `words`
@@ -3088,51 +2793,18 @@ int launch_tiles_bits_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A) {
 
 // the product of arrow_spmm_sr in (or, and); `a` carries the validated bit operands, a.k = the row's words
 int spmm_bits(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a) {
-    const int words = a.k;
-    const int lane = ctx->cur_lane;
-    cudaStream_t stream = cur_stream(ctx);
     if (A->n_tiles[TILE_LIST_SMALL] > 0) {
         TileArgs t;
         t.a = a;
         t.skip = (A->may_skip || ctx->force_skip_path) ? 1 : 0;
-        t.ticket = ctx->tile_ticket + 2 * lane;
+        t.ticket = ctx->tile_ticket + 2 * ctx->cur_lane;
         t.l2_hints = ctx->l2_hints_plain;
         t.prefetch = 0;
         const int rc = launch_tiles_bits_shape(ctx, t, A);
         if (rc != ARROW_OK) return rc;
     }
     CUDA_TRY(ctx, cudaGetLastError());
-
-    if (A->n_long_tasks > 0) {
-        const size_t need = (size_t)A->n_long_tasks * words * 4;
-        if (need > ctx->long_scratch_bytes[lane]) {
-            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
-            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
-            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
-            ctx->long_scratch[lane] = nullptr;
-            ctx->long_scratch_bytes[lane] = 0;
-            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
-            ctx->long_scratch_bytes[lane] = need;
-        }
-        LongArgs la;
-        la.tasks = A->long_tasks;
-        la.indices = a.indices;
-        la.vals = nullptr;
-        la.X = a.X;
-        la.scratch = ctx->long_scratch[lane];
-        la.k = words;
-        la.X2 = nullptr;
-        la.x_split = 0;
-        const size_t smem = (size_t)8 * words * 4;             // <= 8 KB: words <= 256
-        k_spmm_long_partial_bits<<<A->n_long_tasks, 256, smem, stream>>>(la);
-        ctx->launches++;
-        k_spmm_long_reduce_bits<<<A->n_long_rows, 128, 0, stream>>>(
-            A->long_rows, A->long_first, reinterpret_cast<const unsigned int *>(la.scratch),
-            reinterpret_cast<unsigned int *>(a.C), words, reinterpret_cast<const unsigned int *>(a.add_src), a.add_map);
-        ctx->launches++;
-        CUDA_TRY(ctx, cudaGetLastError());
-    }
-    return ARROW_OK;
+    return launch_long_rows<OrAnd>(ctx, A, a, false, false);
 }
 
 constexpr int BITS_MAX_K = 8192;    // 256 words = 64 uint4 per row: the widest (G, VPL) = (32, 2) tile shape
@@ -3821,25 +3493,7 @@ __global__ void __launch_bounds__(128) k_spmm_long_reduce_wit(const int *__restr
 
 template <int G, int VPL, class SR, int TR, int TN>
 int launch_tiles_wit_one(arrow_ctx *ctx, const WitArgs &w) {
-    constexpr size_t SMEM = TileCfg<TR, TN>::SMEM_BYTES;
-    auto fn = k_spmm_tiles_wit<G, VPL, SR, TR, TN>;
-    static bool attr_set[64] = {};            /* function attributes are per device */
-    static int occ_dev[64] = {};
-    const int dv = ctx->device & 63;
-    if (!attr_set[dv]) {
-        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_dev[dv], fn, TILE_THREADS, SMEM) != cudaSuccess || occ_dev[dv] < 1) occ_dev[dv] = 1;
-        attr_set[dv] = true;
-    }
-    const int occ = occ_dev[dv];
-    const int per_sm = (ctx->spmm_ctas_per_sm > 0) ? std::min(occ, ctx->spmm_ctas_per_sm) : occ;
-    int sms = ctx->sm_count;
-    if (ctx->spmm_sm_limit > 0) sms = std::min(sms, ctx->spmm_sm_limit);
-    int grid = (int)std::min<long long>((long long)per_sm * sms, w.t.n_tiles);
-    cudaMemsetAsync(w.t.ticket, 0, 2 * sizeof(int), cur_stream(ctx));
-    fn<<<grid, TILE_THREADS, SMEM, cur_stream(ctx)>>>(w);
-    ctx->launches++;
-    return ARROW_OK;
+    return launch_persistent<k_spmm_tiles_wit<G, VPL, SR, TR, TN>, TileCfg<TR, TN>::SMEM_BYTES>(ctx, w, w.t.n_tiles, w.t.ticket);
 }
 
 // (lanes per row, float4 per lane): one float4 per lane up to 32 lanes (k <= 128), then two (k <= 256); big tiles as
@@ -3892,16 +3546,8 @@ int spmm_wit(arrow_ctx *ctx, const Csr *A, WitArgs &w, bool min_plus) {
 
     if (A->n_long_tasks > 0) {
         const size_t slots = (size_t)A->n_long_tasks * k;
-        const size_t need = slots * 8;                     // values, then labels
-        if (need > ctx->long_scratch_bytes[lane]) {
-            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
-            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
-            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
-            ctx->long_scratch[lane] = nullptr;
-            ctx->long_scratch_bytes[lane] = 0;
-            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
-            ctx->long_scratch_bytes[lane] = need;
-        }
+        const int rc = grow_long_scratch(ctx, slots * 8);  // values, then labels
+        if (rc != ARROW_OK) return rc;
         LongArgs la;
         la.tasks = A->long_tasks;
         la.indices = a.indices;
@@ -4697,7 +4343,6 @@ static int spmm_impl(arrow_ctx *ctx, const SpmmCall &q) {
     const bool acc = (q.flags & ARROW_ACCUMULATE) != 0;
     const int k = X->k;
     const int lane = ctx->cur_lane;
-    cudaStream_t stream = cur_stream(ctx);
     SpmmArgs a;
     a.indptr = A->indptr;
     a.indices = A->indices;
@@ -4745,19 +4390,7 @@ static int spmm_impl(arrow_ctx *ctx, const SpmmCall &q) {
 
     const bool vec_ok = (k % 4 == 0) && k <= 256;
     if (!vec_ok) {
-        const long long ctas = (A->n_rows + 7) / 8;
-#define LAUNCH_G(KERNEL)                                                                              \
-    do {                                                                                              \
-        auto fn = KERNEL;                                                                             \
-        int grid = grid_for(ctx, (const void *)fn, 256, 0, ctas);                                     \
-        fn<<<grid, 256, 0, stream>>>(a);                                                              \
-    } while (0)
-        if (rm && acc) LAUNCH_G((k_spmm_generic<true, true>));
-        else if (rm) LAUNCH_G((k_spmm_generic<true, false>));
-        else if (acc) LAUNCH_G((k_spmm_generic<false, true>));
-        else LAUNCH_G((k_spmm_generic<false, false>));
-#undef LAUNCH_G
-        ctx->launches++;
+        launch_generic<PlusTimes<float>>(ctx, a, rm != nullptr, acc);
     } else if (variant == 3) {
         if (A->n_tiles[TILE_LIST_SMALL] > 0) {
             TileArgs t;
@@ -4790,40 +4423,7 @@ static int spmm_impl(arrow_ctx *ctx, const SpmmCall &q) {
         else launch_vec<32, 2>(ctx, a, rm != nullptr, acc, variant);
     }
     CUDA_TRY(ctx, cudaGetLastError());
-
-    if (A->n_long_tasks > 0) {
-        const size_t need = (size_t)A->n_long_tasks * k * 4;
-        if (need > ctx->long_scratch_bytes[lane]) {
-            if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "long-row scratch would grow during graph capture: run the step once first");
-            CUDA_TRY(ctx, cudaStreamSynchronize(stream));
-            if (ctx->long_scratch[lane]) cudaFree(ctx->long_scratch[lane]);
-            ctx->long_scratch[lane] = nullptr;
-            ctx->long_scratch_bytes[lane] = 0;
-            CUDA_TRY(ctx, cudaMalloc(&ctx->long_scratch[lane], need));
-            ctx->long_scratch_bytes[lane] = need;
-        }
-        LongArgs la;
-        la.tasks = A->long_tasks;
-        la.indices = A->indices;
-        la.vals = A->vals;
-        la.X = X->p;
-        la.scratch = ctx->long_scratch[lane];
-        la.k = k;
-        la.X2 = a.X2;
-        la.x_split = a.x_split;
-        k_spmm_long_partial<<<A->n_long_tasks, 256, 0, stream>>>(la);
-        ctx->launches++;
-        const int *rmp = rm ? rm->p : nullptr;
-        float *cp = C ? C->p : nullptr;
-        float *scr = ctx->long_scratch[lane];
-        if (rm && acc) k_spmm_long_reduce<true, true><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, cp, rmp, k, a.add_src, a.add_map, a.out_ptr);
-        else if (rm) k_spmm_long_reduce<true, false><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, cp, rmp, k, a.add_src, a.add_map, a.out_ptr);
-        else if (acc) k_spmm_long_reduce<false, true><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, cp, rmp, k, a.add_src, a.add_map, a.out_ptr);
-        else k_spmm_long_reduce<false, false><<<A->n_long_rows, 128, 0, stream>>>(A->long_rows, A->long_first, scr, cp, rmp, k, a.add_src, a.add_map, a.out_ptr);
-        ctx->launches++;
-        CUDA_TRY(ctx, cudaGetLastError());
-    }
-    return ARROW_OK;
+    return launch_long_rows<PlusTimes<float>>(ctx, A, a, rm != nullptr, acc);
 }
 
 // ---- pointer tables -------------------------------------------------------------------------------

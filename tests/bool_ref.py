@@ -169,7 +169,7 @@ def source_bits_shapes(path: str) -> set:
 
 # ---- a block whose long rows depend on every part of the long-row path ------------------------------------------------
 LONG_SEGMENT = 2048      # arrow_ctx default segment of the long-row kernels (tests/tile_dispatch.py)
-CTA_WARPS = 8            # warps of k_spmm_long_partial_bits: warp w takes the entries begin + w, begin + w + 8, ...
+CTA_WARPS = 8            # warps of k_spmm_long_partial<OrAnd>: warp w takes the entries begin + w, begin + w + 8, ...
 
 
 def hub_block(rng) -> sparse.csr_matrix:

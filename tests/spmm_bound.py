@@ -20,12 +20,13 @@ kernels in ``arrow_matrix_b200/csrc/arrow_b200.cu`` use for a row with ``n`` sto
   ``fmaf`` per entry in ascending order (``f4_fma`` in the batches and the predicated tail) -> ``n + 1``.
   Skipped entries (column -1) and padding lanes add ``fmaf(v, 0, acc) == acc``: no rounding.
 * ``k_spmm_direct`` / ``k_spmm_shfl`` / ``k_spmm_tma``: ``n`` fmaf from zero, then ``acc + old`` -> ``n + 1``.
-* ``k_spmm_generic``: ``n`` fmaf from zero, ``*dst + acc`` (accumulate), ``r += add`` -> ``n + 2``.
-* long rows (``n > threshold``), ``k_spmm_long_partial``: a segment of at most ``s = min(segment, n)`` entries is
-  split over 8 warps (256 threads), warp ``w`` chains the entries ``begin + w, begin + w + 8, ...`` -> at most
-  ``ceil(s / 8)`` fmaf; the 8 warp partials are added in order from 0 -> 7 more roundings (the first add is
-  exact, count 8); ``k_spmm_long_reduce`` adds the ``ceil(n / segment)`` segment partials in order from 0, then the
-  addend, then ``*dst + sum`` -> ``ceil(s / 8) + 8 + ceil(n / segment) + 2``.
+* ``k_spmm_generic<PlusTimes<float>>``: ``n`` fmaf from zero, ``*dst + acc`` (accumulate), ``r += add`` -> ``n + 2``.
+* long rows (``n > threshold``), ``k_spmm_long_partial<PlusTimes<float>>``: a segment of at most
+  ``s = min(segment, n)`` entries is split over 8 warps (256 threads), warp ``w`` chains the entries
+  ``begin + w, begin + w + 8, ...`` -> at most ``ceil(s / 8)`` fmaf; the 8 warp partials are added in order from 0 ->
+  7 more roundings (the first add is exact, count 8); ``k_spmm_long_reduce<PlusTimes<float>>`` adds the
+  ``ceil(n / segment)`` segment partials in order from 0, then the addend, then ``*dst + sum`` ->
+  ``ceil(s / 8) + 8 + ceil(n / segment) + 2``.
 
 A row gets the largest ``m`` of the kernels that may evaluate it: ``n + 2`` for a row at or below the long-row
 threshold, the long-row height above it.  The float64 reference itself is off by at most
@@ -45,7 +46,7 @@ from scipy import sparse
 U32 = 2.0 ** -24
 U64 = 2.0 ** -53
 ETA32 = 2.0 ** -150          # half the smallest fp32 subnormal: the absolute error of a rounding in the subnormal range
-WARPS_PER_LONG_CTA = 8       # k_spmm_long_partial runs 256 threads
+WARPS_PER_LONG_CTA = 8       # k_spmm_long_partial<SR> runs 256 threads
 
 
 def gamma(m, u=U32):

@@ -20,9 +20,9 @@ smallest subnormal).  ``m`` for a row with ``n`` stored entries, from the float6
 * ``k_spmm_tiles_f64``: ``acc`` starts at zero, or at the addend (one exact add to zero), then one ``fma`` per entry
   in ascending order, then ``acc + C_old`` in accumulate mode -> ``n + 1``.  Skipped entries (column -1), predicated
   tail slots and padding lanes add ``fma(v, 0, acc) == acc``: no rounding.
-* ``k_spmm_generic_f64``: ``n`` fma from zero, ``*dst + acc`` (accumulate), ``r += add`` -> ``n + 2``.
-* long rows (``n > threshold``), ``k_spmm_long_partial_f64`` / ``k_spmm_long_reduce_f64``: the fp32 structure ->
-  ``ceil(s / 8) + 8 + ceil(n / segment) + 2`` with ``s = min(segment, n)``.
+* ``k_spmm_generic<PlusTimes<double>>``: ``n`` fma from zero, ``*dst + acc`` (accumulate), ``r += add`` -> ``n + 2``.
+* long rows (``n > threshold``), ``k_spmm_long_partial`` / ``k_spmm_long_reduce`` on ``PlusTimes<double>``: the fp32
+  structure -> ``ceil(s / 8) + 8 + ceil(n / segment) + 2`` with ``s = min(segment, n)``.
 
 That is ``spmm_bound.tree_height``: a row gets ``n + 2`` at or below the threshold, the long-row height above it.  The
 extended-precision reference (``u = 2^-64`` on x86-64) is off by at most ``gamma_{n+2}(2^-64)`` of the same magnitude,
