@@ -49,9 +49,9 @@ EXPORTS = [
     "arrow_spmm_sr_witness", "arrow_tile_rows", "arrow_tile_rows_rule", "arrow_bits_mark_new",
     "arrow_adj_build", "arrow_adj_free", "arrow_adj_info", "arrow_adj_d2h", "arrow_bits_mark_frontier",
     "arrow_bits_push_frontier", "arrow_adj_build_weighted", "arrow_adj_values_d2h", "arrow_sr_mark_frontier",
-    "arrow_sr_push_frontier",
+    "arrow_sr_push_frontier", "arrow_adj_build_in", "arrow_bits_parents",
 ]
-ABI_VERSION = 9        # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 10       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -163,6 +163,8 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_adj_values_d2h": (c_int, [P, I, P]),
         "arrow_sr_mark_frontier": (c_int, [P, I, I, I, pI64, pI64, pI64]),
         "arrow_sr_push_frontier": (c_int, [P, I, I, I, I]),
+        "arrow_adj_build_in": (c_int, [P, I, pI, pI, I64, pI]),
+        "arrow_bits_parents": (c_int, [P, I, I, I, I, I, pI64]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -471,16 +473,24 @@ class Context:
         self._check(self.lib.arrow_bits_mark_new(self._h, new.h, old.h, dist.h, int(level), byref(n)))
         return int(n.value)
 
-    def adj_build(self, parts: Sequence[tuple], n_vertices: int, weighted: bool = False) -> "Adjacency":
+    def adj_build(self, parts: Sequence[tuple], n_vertices: int, weighted: bool = False,
+                  direction: str = "out") -> "Adjacency":
         """The push adjacency of a BFS (``arrow_adj_build``): ``parts`` is a sequence of ``(Csr, RowMap or None)``; entry
         (r, c) of a block gives the edge map(c) -> map(r) (None: the identity), edges with an end at -1 and u == v are
         dropped.  ``weighted`` (``arrow_adj_build_weighted``): every edge carries its entry's fp32 value and the edges
-        u == v are kept -- the adjacency of the min-plus / max-plus push.  Synchronises."""
+        u == v are kept -- the adjacency of the min-plus / max-plus push.  ``direction="in"`` (``arrow_adj_build_in``):
+        the same edges stored by destination, row v listing its sources u in ascending order -- the adjacency of
+        ``bits_parents``.  Synchronises."""
+        if direction not in ("out", "in"):
+            raise ValueError(f"direction must be 'out' or 'in', got {direction!r}")
+        if direction == "in" and weighted:
+            raise ValueError("the in-adjacency carries no weights")
         n = len(parts)
         csrs = (c_int * max(n, 1))(*[A.h for A, _ in parts])
         maps = (c_int * max(n, 1))(*[m.h if m is not None else -1 for _, m in parts])
         h = c_int()
-        build = self.lib.arrow_adj_build_weighted if weighted else self.lib.arrow_adj_build
+        build = self.lib.arrow_adj_build_weighted if weighted else \
+            self.lib.arrow_adj_build_in if direction == "in" else self.lib.arrow_adj_build
         self._check(build(self._h, n, csrs, maps, int(n_vertices), byref(h)))
         return Adjacency(self, h.value)
 
@@ -496,6 +506,17 @@ class Context:
         """out = x, then out[v] |= x[u] along the adjacency's edges of the recorded frontier rows u
         (``arrow_bits_push_frontier``); ``x`` must be the tile of the last ``bits_mark_frontier`` on ``adj``"""
         self._check(self.lib.arrow_bits_push_frontier(self._h, adj.h, x.h, out.h))
+
+    def bits_parents(self, in_adj: "Adjacency", adj: "Adjacency", new: "Dense", old: "Dense", parent: "Dense",
+                     count: bool = False) -> Optional[int]:
+        """parent[v, s] = the smallest u of ``in_adj``'s row v whose bit s is set in ``old``, for every bit (v, s) set in
+        ``new`` and clear in ``old`` of the rows recorded in ``adj`` by the last ``bits_mark_frontier(adj, new, old, ...)``
+        (``arrow_bits_parents``); other elements of the int32 tile ``parent`` are left alone.  With ``count`` returns the
+        in-edges gathered (synchronises), else None (stream-ordered)."""
+        n = c_int64()
+        self._check(self.lib.arrow_bits_parents(self._h, in_adj.h, adj.h, new.h, old.h, parent.h,
+                                                byref(n) if count else None))
+        return int(n.value) if count else None
 
     def sr_mark_frontier(self, adj: "Adjacency", new: "Dense", old: "Dense"):
         """(rows changed by value -- ``count_diff``'s figure --, frontier rows, frontier edges) of two fp32 tiles; records
@@ -633,7 +654,8 @@ class RowMap(_Handle):
 
 class Adjacency(_Handle):
     """push adjacency (``arrow_adj_build``): a CSR, row u listing the destinations v of u; without values, or with the
-    edges' fp32 weights (``arrow_adj_build_weighted``)"""
+    edges' fp32 weights (``arrow_adj_build_weighted``); or the in-adjacency (``arrow_adj_build_in``), row v listing the
+    sources u of v"""
 
     def info(self):
         n, m = c_int64(), c_int64()

@@ -177,6 +177,18 @@ class ArrowDecompositionMPI:
             raise ValueError("bfs_levels runs on one GPU only")
         return eng.bfs_levels(max_steps, out)
 
+    def bfs_tree(self, max_steps: int, levels_out: Optional[np.ndarray] = None,
+                 parents_out: Optional[np.ndarray] = None):
+        """Extension (one GPU, ``or_and`` with ``add_identity``): ``bfs_levels`` and the BFS parents, both int32 in
+        ``result_tile()`` row order; a parent is a level-0 row, ``-1`` for sources and elements never reached (see
+        ``ArrowEngine.bfs_tree``).  Level 0's permutation maps the parents to vertex ids like the rows."""
+        if self.comm.Get_size() > 1:
+            raise ValueError("bfs_tree runs on one GPU only")
+        eng = self._require_engine()
+        if not isinstance(eng, ArrowEngine):
+            raise ValueError("bfs_tree runs on one GPU only")
+        return eng.bfs_tree(max_steps, levels_out, parents_out)
+
     def iterate_to_fixed_point(self, max_steps: int) -> int:
         """Extension (one GPU): ``step()`` until a step changes no level-0 row, at most ``max_steps`` times; returns the
         number of steps taken.  Direction-optimising in ``min_plus`` / ``max_plus`` with ``add_identity`` (multi-source

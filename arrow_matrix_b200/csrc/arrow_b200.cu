@@ -112,6 +112,9 @@ struct Adj {                          // push adjacency (arrow_adj_build / arrow
     int tag = -1;                     // dense handle whose fresh rows the record holds (-1: no record)
     const void *tag_p = nullptr;      // and its storage and width (a freed and re-used handle does not match)
     int tag_k = 0;
+    bool incoming = false;            // in-adjacency (arrow_adj_build_in): row v lists its sources u; no frontier record
+    int4 *segs = nullptr;             // device (in-adjacency): {v, first, end, 0} per segment of the rows longer than
+    int n_segs = 0;                   //   PARENT_SEG in-edges, which arrow_bits_parents splits across warps
     bool live = false;
 };
 
@@ -277,6 +280,7 @@ void adj_release(Adj &a) {
     cudaFree(a.values);
     cudaFree(a.front_rows);
     cudaFree(a.front_off);
+    cudaFree(a.segs);
     a = Adj();
 }
 
@@ -2867,8 +2871,8 @@ __device__ __forceinline__ int last_le(const int *__restrict__ a, int lo, int hi
 // edges of one block: entry (r, c) with c >= 0 gives u -> v = map(c) -> map(r); an end at -1 drops it, and so does u == v
 // unless W (the weighted adjacency keeps self-loops: a negative one changes a min-plus step).  Counts them into *count;
 // with `keys` also appends (u << 32) | v at a warp-aggregated cursor (the order is fixed by the sort), and with W the
-// entry's value w_in[e] at the same slot of w_out.
-template <bool W>
+// entry's value w_in[e] at the same slot of w_out.  IN appends (v << 32) | u instead: the in-adjacency, row v by source.
+template <bool W, bool IN = false>
 __global__ void __launch_bounds__(256) k_adj_edges(AdjPart p, unsigned long long *__restrict__ count,
                                                    unsigned long long *__restrict__ keys,
                                                    const float *__restrict__ w_in = nullptr, float *__restrict__ w_out = nullptr) {
@@ -2885,7 +2889,8 @@ __global__ void __launch_bounds__(256) k_adj_edges(AdjPart p, unsigned long long
                 const int u = p.map ? __ldg(p.map + c) : c;
                 const int v = p.map ? __ldg(p.map + r) : r;
                 ok = u >= 0 && v >= 0 && (W || u != v);
-                key = ((unsigned long long)(unsigned)u << 32) | (unsigned)v;
+                key = IN ? ((unsigned long long)(unsigned)v << 32) | (unsigned)u
+                         : ((unsigned long long)(unsigned)u << 32) | (unsigned)v;
             }
         }
         const unsigned ball = __ballot_sync(0xffffffffu, ok);
@@ -3039,6 +3044,180 @@ __global__ void __launch_bounds__(PUSH_THREADS) k_bits_push(const V *__restrict_
         }
         __syncthreads();                                      // s_lo / s_hi are rewritten by the next chunk
     }
+}
+
+// ------------------------------------------------------------------------------------------------
+// BFS parents on bit tiles.  Inside a BFS, X_h = X_{h-1} | M X_{h-1}.  A bit (v, s) fresh at level h (set in X_h, clear in
+// X_{h-1}) has an in-neighbour u of v in M holding bit s in X_{h-1}, and every such u has hop level exactly h - 1 (had u
+// reached s by level h - 2, v would hold s in X_{h-1}).  So the parent of (v, s), the smallest in-neighbour one hop
+// closer, is the first u of v's ascending in-list (arrow_adj_build_in) whose bit s is set in X_{h-1}: a bottom-up search
+// over the frontier rows that stops once every fresh bit of the row has its first hit.
+// ------------------------------------------------------------------------------------------------
+constexpr int PARENT_SEG = 512;     // in-edges per segment: longer rows are split into segments across warps
+
+__device__ __forceinline__ unsigned bv_and(unsigned a, unsigned b) { return a & b; }
+__device__ __forceinline__ unsigned bv_andn(unsigned a, unsigned b) { return a & ~b; }
+__device__ __forceinline__ unsigned bv_or(unsigned a, unsigned b) { return a | b; }
+__device__ __forceinline__ bool bv_any(unsigned a) { return a != 0u; }
+__device__ __forceinline__ unsigned bv_zero(unsigned) { return 0u; }
+__device__ __forceinline__ unsigned bv_shfl_up(unsigned a, int d) { return __shfl_up_sync(0xffffffffu, a, d); }
+__device__ __forceinline__ unsigned bv_shfl(unsigned a, int l) { return __shfl_sync(0xffffffffu, a, l); }
+__device__ __forceinline__ unsigned bv_word(unsigned a, int) { return a; }
+__device__ __forceinline__ unsigned bv_cols(unsigned, int q, int k) { return bit_col_mask(q, k); }
+__device__ __forceinline__ uint4 bv_and(uint4 a, uint4 b) { return make_uint4(a.x & b.x, a.y & b.y, a.z & b.z, a.w & b.w); }
+__device__ __forceinline__ uint4 bv_andn(uint4 a, uint4 b) { return make_uint4(a.x & ~b.x, a.y & ~b.y, a.z & ~b.z, a.w & ~b.w); }
+__device__ __forceinline__ uint4 bv_or(uint4 a, uint4 b) { return make_uint4(a.x | b.x, a.y | b.y, a.z | b.z, a.w | b.w); }
+__device__ __forceinline__ bool bv_any(uint4 a) { return (a.x | a.y | a.z | a.w) != 0u; }
+__device__ __forceinline__ uint4 bv_zero(uint4) { return make_uint4(0u, 0u, 0u, 0u); }
+__device__ __forceinline__ uint4 bv_shfl_up(uint4 a, int d) {
+    return make_uint4(__shfl_up_sync(0xffffffffu, a.x, d), __shfl_up_sync(0xffffffffu, a.y, d),
+                      __shfl_up_sync(0xffffffffu, a.z, d), __shfl_up_sync(0xffffffffu, a.w, d));
+}
+__device__ __forceinline__ uint4 bv_shfl(uint4 a, int l) {
+    return make_uint4(__shfl_sync(0xffffffffu, a.x, l), __shfl_sync(0xffffffffu, a.y, l), __shfl_sync(0xffffffffu, a.z, l),
+                      __shfl_sync(0xffffffffu, a.w, l));
+}
+__device__ __forceinline__ unsigned bv_word(const uint4 &a, int i) { return i == 0 ? a.x : i == 1 ? a.y : i == 2 ? a.z : a.w; }
+__device__ __forceinline__ uint4 bv_cols(uint4, int q, int k) {
+    return make_uint4(bit_col_mask(4 * q, k), bit_col_mask(4 * q + 1, k), bit_col_mask(4 * q + 2, k), bit_col_mask(4 * q + 3, k));
+}
+
+struct ParentArgs {
+    const void *__restrict__ nw;        // X_h (bit tile, row_vecs V per row)
+    const void *__restrict__ old;       // X_{h-1}
+    int *__restrict__ parent;           // int32 [rows x k]
+    const int *__restrict__ in_ptr;     // in-adjacency
+    const int *__restrict__ in_idx;
+    const int *__restrict__ rows;       // frontier rows (row pass), or nullptr: the segment pass over segs
+    const int4 *__restrict__ segs;
+    int n_items;                        // frontier rows, or segments
+    int k, row_vecs, vecs;              // columns, V per row, V that hold columns < k
+    unsigned long long *__restrict__ scanned;   // optional: in-edges gathered
+};
+
+// A warp per item: a frontier row (row pass; a row of more than PARENT_SEG in-edges only has its fresh elements set to
+// -1, its segments follow in the segment pass) or a segment {v, first, end} of a long row (segment pass: skipped unless v
+// has a fresh bit).  Lane = (edge slot g, vector q): G lanes share an edge, 32 / G edges go at once, lane q holds vectors
+// q, q + G, ... of the row's fresh bits.  For a batch of edges (ascending u) an exclusive OR-scan over the edge slots of
+// X_{h-1}[u] & fresh gives each fresh bit's first hit, which is its parent within the batch; the row pass stores it, the
+// segment pass folds it with a non-returning unsigned min (-1 is above every label, so the result is exact whatever the
+// order of the segments).  A row or segment stops once no fresh bit is left.
+// parent = -1 for the bits of f (every edge slot holds the same f: slot 0 writes)
+template <class V, int G, int VPL>
+__device__ __forceinline__ void set_no_parent(int *prow, const V (&f)[VPL], int g, int q) {
+    constexpr int WORDS = (int)(sizeof(V) / 4);
+    if (g != 0) return;
+#pragma unroll
+    for (int j = 0; j < VPL; ++j)
+        for (int w = 0; w < WORDS; ++w)
+            for (unsigned m = bv_word(f[j], w); m; m &= m - 1u) prow[((q + j * G) * WORDS + w) * 32 + __ffs(m) - 1] = -1;
+}
+
+template <class V, int G, int VPL>
+__global__ void __launch_bounds__(256) k_bits_parents(ParentArgs a) {
+    constexpr int E = 32 / G;                                 // edges per batch
+    constexpr int WORDS = (int)(sizeof(V) / 4);
+    const V *__restrict__ nw = reinterpret_cast<const V *>(a.nw);
+    const V *__restrict__ old = reinterpret_cast<const V *>(a.old);
+    const int lane = threadIdx.x & 31, g = lane / G, q = lane % G;
+    const long long warps_total = (long long)gridDim.x * (blockDim.x >> 5);
+    unsigned long long scanned = 0;
+    for (long long it = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); it < a.n_items; it += warps_total) {
+        int v, b, e;
+        if (a.rows) {
+            v = __ldg(a.rows + it);
+            b = __ldg(a.in_ptr + v);
+            e = __ldg(a.in_ptr + v + 1);
+        } else {
+            const int4 s = __ldg(a.segs + it);
+            v = s.x, b = s.y, e = s.z;
+        }
+        const bool seg = a.rows == nullptr;
+        const bool long_row = !seg && e - b > PARENT_SEG;
+        V f[VPL];
+        bool any = false;
+#pragma unroll
+        for (int j = 0; j < VPL; ++j) {
+            const int qq = q + j * G;
+            f[j] = bv_zero(V());
+            if (qq < a.vecs) {
+                const long long at = (long long)v * a.row_vecs + qq;
+                f[j] = bv_and(bv_andn(nw[at], old[at]), bv_cols(V(), qq, a.k));
+            }
+            any |= bv_any(f[j]);
+        }
+        if (!__any_sync(0xffffffffu, any)) continue;
+        int *prow = a.parent + (long long)v * a.k;
+        if (long_row) {                                       // the segment pass folds into -1
+            set_no_parent<V, G, VPL>(prow, f, g, q);
+            continue;
+        }
+        for (int base = b; base < e; base += E) {
+            const int edge = base + g;
+            const int u = edge < e ? __ldg(a.in_idx + edge) : -1;
+            bool left = false;
+#pragma unroll
+            for (int j = 0; j < VPL; ++j) {
+                const int qq = q + j * G;
+                V x = bv_zero(V());
+                if (u >= 0 && qq < a.vecs) x = bv_and(old[(long long)u * a.row_vecs + qq], f[j]);
+                V incl = x;                                   // inclusive OR-scan over the edge slots
+#pragma unroll
+                for (int d = G; d < 32; d <<= 1) {
+                    const V y = bv_shfl_up(incl, d);
+                    if (lane >= d) incl = bv_or(incl, y);
+                }
+                V first = x;                                  // bits whose first hit in the batch is this edge
+                if (E > 1) {
+                    const V before = bv_shfl_up(incl, G);
+                    if (g > 0) first = bv_andn(x, before);
+                }
+                for (int w = 0; w < WORDS; ++w)
+                    for (unsigned m = bv_word(first, w); m; m &= m - 1u) {
+                        int *p = prow + (qq * WORDS + w) * 32 + __ffs(m) - 1;
+                        if (seg) asm volatile("red.global.min.u32 [%0], %1;" ::"l"(p), "r"(u) : "memory");
+                        else *p = u;
+                    }
+                f[j] = bv_andn(f[j], E > 1 ? bv_shfl(incl, 32 - G + q) : incl);
+                left |= bv_any(f[j]);
+            }
+            scanned += (unsigned long long)min(E, e - base);
+            if (!__any_sync(0xffffffffu, left)) break;
+        }
+        if (!seg) set_no_parent<V, G, VPL>(prow, f, g, q);      // fresh bits without a hit (none inside a BFS)
+    }
+    if (a.scanned && lane == 0 && scanned) atomicAdd(a.scanned, scanned);
+}
+
+template <class V, int G, int VPL>
+void launch_parents(arrow_ctx *ctx, const ParentArgs &p, int grid) {
+    k_bits_parents<V, G, VPL><<<grid, 256, 0, cur_stream(ctx)>>>(p);
+    ctx->launches++;
+}
+// the row pass over the recorded frontier rows, then the segment pass over the long rows' segments
+int bits_parents(arrow_ctx *ctx, ParentArgs p, const Adj *in, const Adj *a) {
+    const int per_sm = ctx->spmm_ctas_per_sm > 0 ? std::min(ctx->spmm_ctas_per_sm, 8) : 8;
+    const int sms = ctx->spmm_sm_limit > 0 ? std::min(ctx->sm_count, ctx->spmm_sm_limit) : ctx->sm_count;
+    const bool word = p.row_vecs == 1 && p.k <= 32;
+    int g = 1;
+    while (g < 32 && g * (p.vecs > 32 ? 2 : 1) < p.vecs) g <<= 1;     // lanes per edge
+    for (int pass = 0; pass < 2; ++pass) {
+        p.rows = pass == 0 ? a->front_rows : nullptr;
+        p.segs = pass == 0 ? nullptr : in->segs;
+        p.n_items = pass == 0 ? (int)a->n_front : in->n_segs;
+        if (p.n_items == 0) continue;
+        const int grid = (int)std::min<long long>((p.n_items + 7) / 8, (long long)per_sm * sms);
+        if (word) launch_parents<unsigned, 1, 1>(ctx, p, grid);
+        else if (p.vecs > 32) launch_parents<uint4, 32, 2>(ctx, p, grid);
+        else if (g == 1) launch_parents<uint4, 1, 1>(ctx, p, grid);
+        else if (g == 2) launch_parents<uint4, 2, 1>(ctx, p, grid);
+        else if (g == 4) launch_parents<uint4, 4, 1>(ctx, p, grid);
+        else if (g == 8) launch_parents<uint4, 8, 1>(ctx, p, grid);
+        else if (g == 16) launch_parents<uint4, 16, 1>(ctx, p, grid);
+        else launch_parents<uint4, 32, 1>(ctx, p, grid);
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
+    return ARROW_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -4805,9 +4984,11 @@ int arrow_bits_mark_new(arrow_ctx *ctx, int new_buf, int old_buf, int dist_buf, 
 }
 
 namespace {
-// arrow_adj_build (weighted false) and arrow_adj_build_weighted: one validation, one edge pass, one sort
-int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, bool weighted, int *adj_out) {
-    const char *fn = weighted ? "arrow_adj_build_weighted" : "arrow_adj_build";
+// arrow_adj_build (weighted false), arrow_adj_build_weighted and arrow_adj_build_in (incoming): one validation, one edge
+// pass, one sort
+int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, bool weighted, bool incoming,
+              int *adj_out) {
+    const char *fn = weighted ? "arrow_adj_build_weighted" : incoming ? "arrow_adj_build_in" : "arrow_adj_build";
     if (!adj_out || n_parts < 0 || (n_parts > 0 && (!csrs || !maps)) || n_vertices < 0)
         return fail(ctx, ARROW_ERR_ARG, "bad arguments (n_parts=%d, n_vertices=%lld)", n_parts, (long long)n_vertices);
     if (n_vertices > 2147483646LL) return fail(ctx, ARROW_ERR_RANGE, "%lld vertices exceed the int32 device layout", (long long)n_vertices);
@@ -4850,6 +5031,7 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
     CUDA_TRY(ctx, cudaMemsetAsync(count, 0, sizeof m, s));
     for (const AdjPart &p : parts) {
         if (weighted) k_adj_edges<true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
+        else if (incoming) k_adj_edges<false, true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
         else k_adj_edges<false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
         ctx->launches++;
     }
@@ -4862,11 +5044,12 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
     a.n = n_vertices;
     a.m = (int64_t)m;
     a.weighted = weighted;
+    a.incoming = incoming;
     cudaError_t e = cudaMalloc(&a.indptr, (size_t)(n_vertices + 1) * 4);
     if (e == cudaSuccess) e = cudaMalloc(&a.indices, (size_t)std::max<unsigned long long>(m, 1) * 4);
     if (e == cudaSuccess && weighted) e = cudaMalloc(&a.values, (size_t)std::max<unsigned long long>(m, 1) * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&a.front_rows, (size_t)std::max<int64_t>(n_vertices, 1) * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&a.front_off, (size_t)std::max<int64_t>(n_vertices, 1) * 4);
+    if (e == cudaSuccess && !incoming) e = cudaMalloc(&a.front_rows, (size_t)std::max<int64_t>(n_vertices, 1) * 4);
+    if (e == cudaSuccess && !incoming) e = cudaMalloc(&a.front_off, (size_t)std::max<int64_t>(n_vertices, 1) * 4);
     // build scratch: 16 bytes per edge (24 weighted) and the sort's temporary storage
     DevTmp keys, alt, wk, walt, temp;
     const unsigned long long *sorted = nullptr;
@@ -4882,13 +5065,15 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
                 const AdjPart &p = parts[i];
                 if (weighted)
                     k_adj_edges<true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp, weights[i], reinterpret_cast<float *>(wk.p));
+                else if (incoming)
+                    k_adj_edges<false, true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp);
                 else
                     k_adj_edges<false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp);
                 ctx->launches++;
             }
             e = cudaGetLastError();
         }
-        int end_bit = 33;                                     // keys are (u << 32) | v with u < n_vertices
+        int end_bit = 33;                                     // keys are (u << 32) | v with u < n_vertices (in: v, u)
         while (end_bit < 64 && (1LL << (end_bit - 32)) < n_vertices) ++end_bit;
         cub::DoubleBuffer<unsigned long long> db(reinterpret_cast<unsigned long long *>(keys.p),
                                                  reinterpret_cast<unsigned long long *>(alt.p));
@@ -4913,6 +5098,19 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess && incoming && m > (unsigned long long)PARENT_SEG) {   // the segments of the long in-lists
+        std::vector<int> ptr((size_t)n_vertices + 1);
+        e = cudaMemcpy(ptr.data(), a.indptr, ptr.size() * 4, cudaMemcpyDeviceToHost);
+        std::vector<int4> segs;
+        for (int64_t v = 0; e == cudaSuccess && v < n_vertices; ++v)
+            if (ptr[v + 1] - ptr[v] > PARENT_SEG)
+                for (int b = ptr[v]; b < ptr[v + 1]; b += PARENT_SEG)
+                    segs.push_back(make_int4((int)v, b, std::min(b + PARENT_SEG, ptr[v + 1]), 0));
+        if (e == cudaSuccess && !segs.empty()) e = cudaMalloc(&a.segs, segs.size() * sizeof(int4));
+        if (e == cudaSuccess && !segs.empty())
+            e = cudaMemcpy(a.segs, segs.data(), segs.size() * sizeof(int4), cudaMemcpyHostToDevice);
+        a.n_segs = (int)segs.size();
+    }
     if (e != cudaSuccess) {
         cudaGetLastError();
         adj_release(a);
@@ -4930,20 +5128,27 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
 int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out) {
     CHECK_CTX(ctx);
     CHECK_POISON(ctx);
-    return adj_build(ctx, n_parts, csrs, maps, n_vertices, false, adj_out);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, false, false, adj_out);
+}
+
+int arrow_adj_build_in(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, false, true, adj_out);
 }
 
 int arrow_adj_build_weighted(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices,
                              int *adj_out) {
     CHECK_CTX(ctx);
     CHECK_POISON(ctx);
-    return adj_build(ctx, n_parts, csrs, maps, n_vertices, true, adj_out);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, true, false, adj_out);
 }
 
 int arrow_adj_values_d2h(arrow_ctx *ctx, int adj, float *values) {
     CHECK_CTX(ctx);
     const Adj *a = get_adj(ctx, adj);
     if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
     if (!a->weighted) return fail(ctx, ARROW_ERR_ARG, "the adjacency carries no weights (built by arrow_adj_build)");
     if (a->m > 0 && !values) return fail(ctx, ARROW_ERR_ARG, "null host buffer");
     if (a->m > 0) CUDA_TRY(ctx, cudaMemcpyAsync(values, a->values, (size_t)a->m * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -4986,6 +5191,7 @@ int arrow_bits_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, 
     CHECK_POISON(ctx);
     Adj *a = get_adj(ctx, adj);
     if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
     DenseBuf *N = get_dense(ctx, new_buf), *O = get_dense(ctx, old_buf), *D = get_dense(ctx, dist_buf);
     if (!N || !O || !D) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (new=%d old=%d dist=%d)", new_buf, old_buf, dist_buf);
     if (!n_new || !frontier_rows || !frontier_edges) return fail(ctx, ARROW_ERR_ARG, "null output");
@@ -5031,6 +5237,7 @@ int arrow_bits_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf) {
     CHECK_POISON(ctx);
     const Adj *a = get_adj(ctx, adj);
     if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
     DenseBuf *X = get_dense(ctx, x_buf), *O = get_dense(ctx, out_buf);
     if (!X || !O) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x=%d out=%d)", x_buf, out_buf);
     if (X->dtype != ARROW_B1 || O->dtype != ARROW_B1)
@@ -5069,12 +5276,64 @@ int arrow_bits_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf) {
     return ARROW_OK;
 }
 
+int arrow_bits_parents(arrow_ctx *ctx, int in_adj, int adj, int new_buf, int old_buf, int parent_buf, int64_t *edges_scanned) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    const Adj *in = get_adj(ctx, in_adj), *a = get_adj(ctx, adj);
+    if (!in || !a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle (in=%d adj=%d)", in_adj, adj);
+    DenseBuf *N = get_dense(ctx, new_buf), *O = get_dense(ctx, old_buf), *P = get_dense(ctx, parent_buf);
+    if (!N || !O || !P) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (new=%d old=%d parent=%d)", new_buf, old_buf, parent_buf);
+    if (!in->incoming || a->incoming)
+        return fail(ctx, ARROW_ERR_ARG, "in_adj is the in-adjacency (arrow_adj_build_in) and adj the push adjacency");
+    if (in->n != a->n)
+        return fail(ctx, ARROW_ERR_ARG, "the adjacencies differ in vertices: in %lld, push %lld", (long long)in->n, (long long)a->n);
+    if (N->dtype != ARROW_B1 || O->dtype != ARROW_B1 || P->dtype != ARROW_I32)
+        return fail(ctx, ARROW_ERR_ARG, "new / old are bit tiles and parent an int32 tile: got %s / %s / %s", dtype_name(N->dtype),
+                    dtype_name(O->dtype), dtype_name(P->dtype));
+    if (N->rows != a->n || O->rows != N->rows || P->rows != N->rows || O->k != N->k || P->k != N->k)
+        return fail(ctx, ARROW_ERR_ARG, "shape: new %lld x %d, old %lld x %d, parent %lld x %d, adjacency %lld rows",
+                    (long long)N->rows, N->k, (long long)O->rows, O->k, (long long)P->rows, P->k, (long long)a->n);
+    if (new_buf == old_buf || N->p == O->p) return fail(ctx, ARROW_ERR_ARG, "old aliases new");
+    if (a->tag < 0) return fail(ctx, ARROW_ERR_ARG, "no frontier record: run arrow_bits_mark_frontier on the adjacency first");
+    if (new_buf != a->tag || N->p != a->tag_p || N->k != a->tag_k)
+        return fail(ctx, ARROW_ERR_ARG, "new (tile %d) is not the tile of the last arrow_bits_mark_frontier (tile %d)", new_buf, a->tag);
+    if (N->k > BITS_MAX_K) return fail(ctx, ARROW_ERR_UNSUPPORTED, "k=%d > %d", N->k, BITS_MAX_K);
+    if (edges_scanned) *edges_scanned = 0;
+    if (N->rows == 0 || N->k == 0 || a->n_front == 0) return ARROW_OK;
+    const int words = bit_row_words(N->k);
+    ParentArgs p{};
+    p.nw = N->p;
+    p.old = O->p;
+    p.parent = reinterpret_cast<int *>(P->p);
+    p.in_ptr = in->indptr;
+    p.in_idx = in->indices;
+    p.k = N->k;
+    p.row_vecs = words == 1 ? 1 : words / 4;
+    p.vecs = words == 1 ? 1 : ((N->k + 31) / 32 + 3) / 4;
+    DevTmp cnt;
+    if (edges_scanned) {
+        CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof(unsigned long long)));
+        CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof(unsigned long long), cur_stream(ctx)));
+        p.scanned = reinterpret_cast<unsigned long long *>(cnt.p);
+    }
+    const int rc = bits_parents(ctx, p, in, a);
+    if (rc != ARROW_OK) return rc;
+    if (edges_scanned) {
+        unsigned long long h = 0;
+        CUDA_TRY(ctx, cudaMemcpyAsync(&h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, cur_stream(ctx)));
+        CUDA_TRY(ctx, cudaStreamSynchronize(cur_stream(ctx)));
+        *edges_scanned = (int64_t)h;
+    }
+    return ARROW_OK;
+}
+
 int arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int64_t *rows_changed, int64_t *frontier_rows,
                            int64_t *frontier_edges) {
     CHECK_CTX(ctx);
     CHECK_POISON(ctx);
     Adj *a = get_adj(ctx, adj);
     if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
     DenseBuf *N = get_dense(ctx, new_buf), *O = get_dense(ctx, old_buf);
     if (!N || !O) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (new=%d old=%d)", new_buf, old_buf);
     if (!rows_changed || !frontier_rows || !frontier_edges) return fail(ctx, ARROW_ERR_ARG, "null output");
@@ -5118,6 +5377,7 @@ int arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int 
     if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS) return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
     const Adj *a = get_adj(ctx, adj);
     if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
     DenseBuf *X = get_dense(ctx, x_buf), *O = get_dense(ctx, out_buf);
     if (!X || !O) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (x=%d out=%d)", x_buf, out_buf);
     if (X->dtype != ARROW_F32 || O->dtype != ARROW_F32)

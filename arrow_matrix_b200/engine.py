@@ -135,6 +135,8 @@ class ArrowEngine:
         self.last_bfs_steps = 0                                  # steps the last bfs_levels() call took
         self.last_bfs_directions: List[str] = []                 # "push" / "pull" per level of the last bfs_levels()
         self._adj: Optional[_lib.Adjacency] = None               # bfs_levels(): the push adjacency, built on first use
+        self._in_adj: Optional[_lib.Adjacency] = None            # bfs_tree(): the in-adjacency, built on first use
+        self._bfs_parents: Optional[_lib.Dense] = None           # bfs_tree(): the int32 parent tile
         self._push_limit: Optional[int] = None                   # None: bfs_direction() decides; else push iff edges < it
         self.last_fixed_point_directions: List[str] = []         # "push" / "pull" per step of iterate_to_fixed_point()
         self._sr_adj: Optional[_lib.Adjacency] = None            # iterate_to_fixed_point(): weighted push adjacency
@@ -542,12 +544,47 @@ class ArrowEngine:
         levels ``j >= 1`` (``result(j)``) are not that level's product; the next ``step()`` rewrites them."""
         return self._bfs_run(max_steps).d2h(out)
 
-    def _bfs_run(self, max_steps: int) -> _lib.Dense:
-        """the device part of ``bfs_levels``: runs the levels and returns the int32 level tile, left on the device"""
+    def bfs_tree(self, max_steps: int, levels_out: Optional[np.ndarray] = None,
+                 parents_out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """``bfs_levels`` that also returns the BFS parents (both int32 [n x k], level-0 row order like ``result()``):
+        ``P[v, s]`` is the smallest level-0 row ``u`` with an edge ``u -> v`` of the fused step's operator (``u != v``)
+        whose level is ``L[v, s] - 1``, where ``L[v, s] > 0``; ``-1`` for the sources and for elements not reached
+        (within ``max_steps``).  On unit weights this is what ``predecessors()`` gives after ``iterate_to_fixed_point()``
+        on a ``min_plus`` engine with ``add_identity``.  The levels, ``last_bfs_steps``, ``last_bfs_directions`` and the
+        features are those of ``bfs_levels``.
+
+        After each level's record one more device pass searches the in-lists of the rows that gained a bit, in ascending
+        ``u``, for the first source row holding the bit one level earlier (DESIGN.md §4).  The in-adjacency is built on
+        the first call and kept until ``close()``; an engine that does not push (exchange mode with one level) builds the
+        push adjacency for the frontier record and still pulls every level.  Raises ``ValueError`` before any CUDA work
+        outside ``or_and`` with ``add_identity``, and when a level reads rows behind the sentinel (``fused_ok`` is false:
+        such a row has no vertex identity).  Synchronises."""
+        self._bfs_checks("bfs_tree")
+        if not self.fused_ok:
+            raise ValueError("bfs_tree needs a level-0 row behind every non-zero, but a level reads rows behind the "
+                             "sentinel")
+        dist, parents = self._bfs_tree_run(max_steps)
+        return dist.d2h(levels_out), parents.d2h(parents_out)
+
+    def _bfs_tree_run(self, max_steps: int) -> Tuple[_lib.Dense, _lib.Dense]:
+        """the device part of ``bfs_tree``: the int32 level and parent tiles, left on the device"""
+        if self._in_adj is None:
+            parts = [(st.csr, st.cmap_dev) for st in self.levels]
+            self._in_adj = self.ctx.adj_build(parts, self.levels[0].rows, direction="in")
+        if self._bfs_parents is None:
+            self._bfs_parents = self.ctx.dense_alloc(self.levels[0].rows, self.k, np.int32)
+        return self._bfs_run(max_steps, self._bfs_parents), self._bfs_parents
+
+    def _bfs_checks(self, what: str):
         if not self.bits:
-            raise ValueError(f"bfs_levels runs the or_and semiring, the engine runs {self.semiring}")
+            raise ValueError(f"{what} runs the or_and semiring, the engine runs {self.semiring}")
         if not self.add_identity:
-            raise ValueError("bfs_levels needs add_identity=True: a step must keep the bits it already has")
+            raise ValueError(f"{what} needs add_identity=True: a step must keep the bits it already has")
+
+    def _bfs_run(self, max_steps: int, parents: Optional[_lib.Dense] = None) -> _lib.Dense:
+        """the device part of ``bfs_levels``: runs the levels and returns the int32 level tile, left on the device.  With
+        ``parents`` (``bfs_tree``) also writes the parent of every element into that int32 tile."""
+        self._bfs_checks("bfs_levels")
         self.sync()
         st0 = self.levels[0]
         if self._bfs_tiles is None:
@@ -557,7 +594,9 @@ class ArrowEngine:
         dist, zero, ones = self._bfs_tiles
         # an exchange-mode step of one level has no backward exchange and leaves level 0's features where they are, so a
         # push (which advances them like a fused step) would not match it: that engine pulls every level
-        adj = self._push_adjacency() if self.fused_ok and (self.mode == "fused" or self.L > 1) else None
+        pushes = self.fused_ok and (self.mode == "fused" or self.L > 1)
+        # the parent pass reads the frontier record, so bfs_tree keeps one even on an engine that only pulls
+        adj = self._push_adjacency() if pushes or parents is not None else None
         limit = self._push_limit
 
         def mark(new, old, level):
@@ -565,9 +604,15 @@ class ArrowEngine:
             if adj is None:
                 return self.ctx.bits_mark_new(new, old, dist, level), False
             n_new, _, edges = self.ctx.bits_mark_frontier(adj, new, old, dist, level)
+            if parents is not None and level > 0:        # old is X_{h-1} until the next level writes its tile
+                self.ctx.bits_parents(self._in_adj, adj, new, old, parents)
+            if not pushes:
+                return n_new, False
             push = edges < limit if limit is not None else bfs_direction(edges, self.total_nnz) == "push"
             return n_new, push
 
+        if parents is not None:                          # the sources have no parent
+            self.ctx.bits_mark_new(st0.bufs[st0.xi], zero, parents, -1)
         _, push = mark(st0.bufs[st0.xi], zero, 0)
         steps, directions = 0, []
         for level in range(1, int(max_steps) + 1):
@@ -586,6 +631,8 @@ class ArrowEngine:
         self.last_bfs_directions = directions
         # every element reached in this call was written by it; the others (clear in the final bits) become -1
         self.ctx.bits_mark_new(ones, st0.bufs[st0.xi], dist, -1)
+        if parents is not None:
+            self.ctx.bits_mark_new(ones, st0.bufs[st0.xi], parents, -1)
         return dist
 
     def _push_adjacency(self) -> _lib.Adjacency:
@@ -705,8 +752,9 @@ class ArrowEngine:
     def close(self):
         for b in (self._wit_labels or []) + list(self._wit_values.values()) + list(self._bfs_tiles or ()):
             b.free()
-        for a in (self._adj, self._sr_adj):
+        for a in (self._adj, self._sr_adj, self._in_adj, self._bfs_parents):
             if a is not None:
                 a.free()
         self._wit_labels, self._wit_values, self._bfs_tiles, self._adj, self._sr_adj = None, {}, None, None, None
+        self._in_adj = self._bfs_parents = None
         self.ctx.close()

@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 9
+#define ARROW_ABI_VERSION 10
 
 /* error codes */
 #define ARROW_OK              0
@@ -269,6 +269,21 @@ int  arrow_bits_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf,
  * X_{h-1}'s tile (x alone is read).  ARROW_ERR_ARG: non-bit tiles, no record, x not the recorded tile, out == x, rows
  * other than the adjacency's, out of another shape or k; ARROW_ERR_UNSUPPORTED: k > 8192. */
 int  arrow_bits_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf);
+/* In-adjacency of the same M: row v lists every u with an edge u -> v in ascending order, duplicates kept; the edges are
+ * arrow_adj_build's (same blocks, maps and dropped edges) and so are the refusals.  It keeps 4 (n + 1) + 4 m bytes and no
+ * frontier record; rows of more than 512 entries are also listed as 512-entry segments (16 bytes each) for
+ * arrow_bits_parents.  arrow_adj_info, arrow_adj_d2h and arrow_adj_free accept it; every other call taking an adjacency
+ * refuses it with ARROW_ERR_ARG.  Synchronises. */
+int  arrow_adj_build_in(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out);
+/* BFS parents of one level.  For every row v of adj's frontier record (written by arrow_bits_mark_frontier for new_buf
+ * against old_buf) and every bit (v, s), s < k, set in new_buf and clear in old_buf: parent[v, s] = the smallest u of
+ * in_adj's row v whose bit s is set in old_buf, -1 when there is none.  Every other element of parent_buf is left alone.
+ * When new = X_h = X_{h-1} | M X_{h-1} and old = X_{h-1}, that u is the smallest in-neighbour of v one hop closer to s.
+ * Exact: the result depends on neither the grid nor the kernel.  edges_scanned (may be NULL; then the call does not
+ * synchronise) receives the in-edges gathered.  ARROW_ERR_ARG: non-bit new / old, a parent tile that is not ARROW_I32 of
+ * the same rows and k, in_adj not an in-adjacency or adj one, adjacencies of different vertex counts, rows other than
+ * theirs, no record in adj or one for another tile, new_buf == old_buf; ARROW_ERR_UNSUPPORTED: k > 8192. */
+int  arrow_bits_parents(arrow_ctx *ctx, int in_adj, int adj, int new_buf, int old_buf, int parent_buf, int64_t *edges_scanned);
 
 /* ---- direction-optimising shortest and critical paths (one GPU, min-plus / max-plus on fp32 tiles) ---------------------- */
 /* The push adjacency of arrow_adj_build carrying each edge's fp32 weight (the entry's value), with the edges u == v kept
