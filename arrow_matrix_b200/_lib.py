@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import (POINTER, byref, c_char_p, c_float, c_int, c_int32, c_int64, c_size_t, c_void_p)
+from ctypes import (POINTER, byref, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_void_p)
 from typing import Optional, Sequence
 
 import numpy as np
@@ -49,9 +49,10 @@ EXPORTS = [
     "arrow_spmm_sr_witness", "arrow_tile_rows", "arrow_tile_rows_rule", "arrow_bits_mark_new",
     "arrow_adj_build", "arrow_adj_free", "arrow_adj_info", "arrow_adj_d2h", "arrow_bits_mark_frontier",
     "arrow_bits_push_frontier", "arrow_adj_build_weighted", "arrow_adj_values_d2h", "arrow_sr_mark_frontier",
-    "arrow_sr_push_frontier", "arrow_adj_build_in", "arrow_bits_parents",
+    "arrow_sr_push_frontier", "arrow_adj_build_in", "arrow_bits_parents", "arrow_bits_path_counts",
+    "arrow_adj_keep_record", "arrow_bits_dependencies", "arrow_bits_fill_f64", "arrow_dense_row_sum",
 ]
-ABI_VERSION = 10       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 11       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -165,6 +166,11 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_sr_push_frontier": (c_int, [P, I, I, I, I]),
         "arrow_adj_build_in": (c_int, [P, I, pI, pI, I64, pI]),
         "arrow_bits_parents": (c_int, [P, I, I, I, I, I, pI64]),
+        "arrow_bits_path_counts": (c_int, [P, I, I, I, I, I, pI64]),
+        "arrow_adj_keep_record": (c_int, [P, I, I]),
+        "arrow_bits_dependencies": (c_int, [P, I, I, I, I, I, pI64]),
+        "arrow_bits_fill_f64": (c_int, [P, I, I, I, c_double]),
+        "arrow_dense_row_sum": (c_int, [P, I, I]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -517,6 +523,40 @@ class Context:
         self._check(self.lib.arrow_bits_parents(self._h, in_adj.h, adj.h, new.h, old.h, parent.h,
                                                 byref(n) if count else None))
         return int(n.value) if count else None
+
+    def bits_path_counts(self, in_adj: "Adjacency", adj: "Adjacency", new: "Dense", old: "Dense", sigma: "Dense",
+                         count: bool = False) -> Optional[int]:
+        """sigma[v, s] = the sum of sigma[u, s] over the distinct u of ``in_adj``'s row v whose bit s is set in ``old``,
+        for every bit (v, s) set in ``new`` and clear in ``old`` of the rows recorded in ``adj`` by the last
+        ``bits_mark_frontier(adj, new, old, ...)`` (``arrow_bits_path_counts``); other elements of the float64 tile
+        ``sigma`` are left alone.  With ``count`` returns the in-list entries read (synchronises), else None."""
+        n = c_int64()
+        self._check(self.lib.arrow_bits_path_counts(self._h, in_adj.h, adj.h, new.h, old.h, sigma.h,
+                                                    byref(n) if count else None))
+        return int(n.value) if count else None
+
+    def adj_keep_record(self, adj: "Adjacency", level: int):
+        """copies ``adj``'s frontier record into its history as ``level`` (0 restarts it; otherwise the next level)
+        (``arrow_adj_keep_record``)"""
+        self._check(self.lib.arrow_adj_keep_record(self._h, adj.h, int(level)))
+
+    def bits_dependencies(self, adj: "Adjacency", level: int, dist: "Dense", sigma: "Dense", delta: "Dense",
+                          count: bool = False) -> Optional[int]:
+        """delta[u, s] = sigma[u, s] * sum of (1 + delta[w, s]) / sigma[w, s] over the distinct w of ``adj``'s row u
+        with dist[w, s] == level + 1, for the rows u of the history's ``level`` and the columns with dist[u, s] == level
+        (``arrow_bits_dependencies``).  With ``count`` returns the out-list entries read (synchronises), else None."""
+        n = c_int64()
+        self._check(self.lib.arrow_bits_dependencies(self._h, adj.h, int(level), dist.h, sigma.h, delta.h,
+                                                     byref(n) if count else None))
+        return int(n.value) if count else None
+
+    def bits_fill_f64(self, new: "Dense", old: "Dense", out: "Dense", value: float):
+        """out[r, s] = value for every bit set in ``new`` and clear in ``old`` (float64 ``out``; ``arrow_bits_fill_f64``)"""
+        self._check(self.lib.arrow_bits_fill_f64(self._h, new.h, old.h, out.h, float(value)))
+
+    def row_sum(self, x: "Dense", out: "Dense"):
+        """out[r, 0] = x[r, 0] + ... + x[r, k - 1], left to right (float64 tiles; ``arrow_dense_row_sum``)"""
+        self._check(self.lib.arrow_dense_row_sum(self._h, x.h, out.h))
 
     def sr_mark_frontier(self, adj: "Adjacency", new: "Dense", old: "Dense"):
         """(rows changed by value -- ``count_diff``'s figure --, frontier rows, frontier edges) of two fp32 tiles; records

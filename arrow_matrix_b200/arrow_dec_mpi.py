@@ -189,6 +189,27 @@ class ArrowDecompositionMPI:
             raise ValueError("bfs_tree runs on one GPU only")
         return eng.bfs_tree(max_steps, levels_out, parents_out)
 
+    def bfs_path_counts(self, max_steps: int, levels_out: Optional[np.ndarray] = None,
+                        counts_out: Optional[np.ndarray] = None):
+        """Extension (one GPU, ``or_and`` with ``add_identity``): ``bfs_levels`` and the shortest-path counts, int32 and
+        float64 in ``result_tile()`` row order (see ``ArrowEngine.bfs_path_counts``)."""
+        return self._bfs_engine("bfs_path_counts").bfs_path_counts(max_steps, levels_out, counts_out)
+
+    def betweenness(self, max_steps: int, out: Optional[np.ndarray] = None,
+                    dependencies_out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension (one GPU, ``or_and`` with ``add_identity``): Brandes betweenness over the feature columns as
+        sources, float64 [n] in ``result_tile()`` row order (see ``ArrowEngine.betweenness``).  Level 0's permutation
+        maps the rows to vertex ids."""
+        return self._bfs_engine("betweenness").betweenness(max_steps, out, dependencies_out)
+
+    def _bfs_engine(self, what: str) -> ArrowEngine:
+        if self.comm.Get_size() > 1:
+            raise ValueError(f"{what} runs on one GPU only")
+        eng = self._require_engine()
+        if not isinstance(eng, ArrowEngine):
+            raise ValueError(f"{what} runs on one GPU only")
+        return eng
+
     def iterate_to_fixed_point(self, max_steps: int) -> int:
         """Extension (one GPU): ``step()`` until a step changes no level-0 row, at most ``max_steps`` times; returns the
         number of steps taken.  Direction-optimising in ``min_plus`` / ``max_plus`` with ``add_identity`` (multi-source

@@ -113,8 +113,15 @@ struct Adj {                          // push adjacency (arrow_adj_build / arrow
     const void *tag_p = nullptr;      // and its storage and width (a freed and re-used handle does not match)
     int tag_k = 0;
     bool incoming = false;            // in-adjacency (arrow_adj_build_in): row v lists its sources u; no frontier record
-    int4 *segs = nullptr;             // device (in-adjacency): {v, first, end, 0} per segment of the rows longer than
-    int n_segs = 0;                   //   PARENT_SEG in-edges, which arrow_bits_parents splits across warps
+    int4 *segs = nullptr;             // device: {v, first, end, 0} per segment of the rows longer than PARENT_SEG entries,
+    int n_segs = 0;                   //   which arrow_bits_parents and the betweenness passes split across warps
+    bool has_segs = false;            // segs lists every list longer than PARENT_SEG (built for the in-adjacency, and on
+                                      //   arrow_bits_dependencies' first call for the push adjacency)
+    double *seg_part = nullptr;       // device: [n_segs x k] partial sums of the betweenness segment passes
+    size_t seg_part_bytes = 0;
+    int *hist = nullptr;              // device: the frontier records kept by arrow_adj_keep_record, level after level
+    int64_t hist_cap = 0;             //   (its capacity in rows)
+    std::vector<int64_t> hist_off;    // host: level h's rows are hist[hist_off[h], hist_off[h + 1])
     bool live = false;
 };
 
@@ -281,6 +288,8 @@ void adj_release(Adj &a) {
     cudaFree(a.front_rows);
     cudaFree(a.front_off);
     cudaFree(a.segs);
+    cudaFree(a.hist);
+    cudaFree(a.seg_part);
     a = Adj();
 }
 
@@ -3221,6 +3230,240 @@ int bits_parents(arrow_ctx *ctx, ParentArgs p, const Adj *in, const Adj *a) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Betweenness on bit tiles (Brandes over k source columns).  M is taken as a set: a list entry equal to its predecessor in
+// the (sorted) list is skipped.  Path counts: a bit (v, s) fresh at level h has sigma[v, s] = the sum of sigma[u, s] over
+// the in-neighbours u holding s in X_{h-1} (exactly those at level h - 1, see the parents pass).  Dependencies: for
+// L[u, s] = h, delta[u, s] = sigma[u, s] * sum of fl((1 + delta[w, s]) / sigma[w, s]) over the out-neighbours w with
+// L[w, s] = h + 1.  Both sums run over the list in ascending order, PATH_SEG entries at a time from the row's start: each
+// segment's terms are summed left to right into a partial that starts at 0, and the partials are added in segment order.
+// A warp takes one (row, 32-column word), a lane per column.  A list of at most PATH_SEG entries is summed by that warp;
+// a longer one is split at the adjacency's segments (Adj::segs): a segment pass gives each (segment, word) its own warp,
+// which stores its partial in Adj::seg_part, and the row pass adds the row's partials in segment order.  The order depends
+// on the adjacency alone and no floating-point atomics are needed: the results are exact functions of the inputs.
+// ------------------------------------------------------------------------------------------------
+constexpr int PATH_SEG = PARENT_SEG;    // list entries per partial sum: the adjacencies' segment length
+
+struct PathArgs {
+    const unsigned *__restrict__ nw;    // X_h (path counts) -- bit tiles of `words` words per row
+    const unsigned *__restrict__ old;   // X_{h-1}
+    const int *__restrict__ dist;       // level tile (dependencies)
+    double *sigma;                      // path counts: read at level h - 1, written at the fresh bits of level h
+    double *delta;                      // dependencies: read at level h + 1, written at level h
+    const int *__restrict__ ptr;        // in-adjacency (path counts) or push adjacency (dependencies)
+    const int *__restrict__ idx;
+    const int *__restrict__ rows;       // frontier rows of level h (row pass), or nullptr: the segment pass over segs
+    const int4 *__restrict__ segs;      // {row, first, end, 0} per segment of the lists longer than PATH_SEG, by row
+    int n_segs;
+    double *seg_part;                   // [n_segs x k] partial sums of the segment pass
+    int n_items;                        // (rows or segments) x used words (below 2^31 whenever the fp64 tiles fit)
+    int k, words, used, level;
+    unsigned long long *__restrict__ scanned;   // optional: list entries read, once per (row or segment, word) (a 64-bit
+                                                //   sum kept in registers across the division's slow-path call would spill)
+};
+
+// the first segment of row v in segs (sorted by row; v has at least one)
+__device__ __forceinline__ int first_seg(const int4 *__restrict__ segs, int n, int v) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(&segs[mid].x) < v) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// item `it` of a pass: (row, list [b, e) of the row, range [sb, se) summed here, word w, segment index or -1)
+struct PathItem {
+    int v, b, e, sb, se, w, seg;
+};
+__device__ __forceinline__ PathItem path_item(const PathArgs &a, int it) {
+    PathItem t;
+    const int i = it / a.used;
+    t.w = it - i * a.used;
+    if (a.rows) {
+        t.v = __ldg(a.rows + i);
+        t.b = __ldg(a.ptr + t.v);
+        t.e = __ldg(a.ptr + t.v + 1);
+        t.sb = t.b;
+        t.se = t.e;
+        t.seg = -1;
+    } else {
+        const int4 g = __ldg(a.segs + i);
+        t.v = g.x;
+        t.b = __ldg(a.ptr + t.v);
+        t.e = __ldg(a.ptr + t.v + 1);
+        t.sb = g.y;
+        t.se = g.z;
+        t.seg = i;
+    }
+    return t;
+}
+
+// the row pass's total for lane column c of a long row: its segment partials added in order (active lanes only)
+__device__ __forceinline__ double seg_total(const PathArgs &a, int v, int c) {
+    double total = 0.0;
+    for (int j = first_seg(a.segs, a.n_segs, v); j < a.n_segs && __ldg(&a.segs[j].x) == v; ++j)
+        total += a.seg_part[(long long)j * a.k + c];
+    return total;
+}
+
+// sigma[v, c] for the fresh bits c of word w of every frontier row v.  Per batch of 32 list entries lane j loads entry j
+// and the hit mask X_{h-1}[u] & fresh; then the entries with a hit are taken in order, each lane adding sigma[u, c] for its
+// own column c when hit.  Only the sigma words of hit columns are read.
+__global__ void __launch_bounds__(256) k_bits_path_counts(PathArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int warps_total = gridDim.x * (blockDim.x >> 5);
+    for (int it = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); it < a.n_items; it += warps_total) {
+        const PathItem t = path_item(a, it);
+        const long long vw = (long long)t.v * a.words + t.w;
+        const unsigned fresh = __ldg(a.nw + vw) & ~__ldg(a.old + vw) & bit_col_mask(t.w, a.k);
+        if (fresh == 0u) continue;
+        const int c = t.w * 32 + lane;
+        const bool on = (fresh >> lane) & 1u;
+        const bool split = t.seg < 0 && t.e - t.b > PATH_SEG;     // a long row: its segments were summed by the segment pass
+        double total = 0.0;
+        if (split) {
+            if (on) total = seg_total(a, t.v, c);
+        } else {
+            double part = 0.0;
+            for (int base = t.sb; base < t.se; base += 32) {
+                const int edge = base + lane;
+                int u = 0;
+                unsigned hit = 0u;
+                if (edge < t.se) {
+                    u = __ldg(a.idx + edge);
+                    if (edge == t.b || __ldg(a.idx + edge - 1) != u) hit = __ldg(a.old + (long long)u * a.words + t.w) & fresh;
+                }
+                for (unsigned bal = __ballot_sync(0xffffffffu, hit != 0u); bal; bal &= bal - 1u) {
+                    const int j = __ffs(bal) - 1;
+                    const int uj = __shfl_sync(0xffffffffu, u, j);
+                    const unsigned hj = __shfl_sync(0xffffffffu, hit, j);
+                    if ((hj >> lane) & 1u) part += a.sigma[(long long)uj * a.k + c];
+                }
+            }
+            total += part;
+            if (a.scanned && lane == 0) atomicAdd(a.scanned, (unsigned long long)(t.se - t.sb));
+        }
+        if (!on) continue;
+        if (t.seg >= 0) a.seg_part[(long long)t.seg * a.k + c] = total;
+        else a.sigma[(long long)t.v * a.k + c] = total;
+    }
+}
+
+// delta[u, c] for the columns c of word w of every recorded row u of level h with L[u, c] = h.  Per batch of 32 list
+// entries the warp takes each distinct w in order and reads its level row (one 128-byte line per word); the lanes whose
+// column is at level h + 1 there add (1 + delta[w, c]) / sigma[w, c].
+__global__ void __launch_bounds__(256) k_bits_dependencies(PathArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int warps_total = gridDim.x * (blockDim.x >> 5);
+    for (int it = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); it < a.n_items; it += warps_total) {
+        const PathItem t = path_item(a, it);
+        const int c = t.w * 32 + lane;
+        const bool mine = c < a.k && __ldg(a.dist + (long long)t.v * a.k + c) == a.level;
+        if (!__any_sync(0xffffffffu, mine)) continue;
+        const bool split = t.seg < 0 && t.e - t.b > PATH_SEG;
+        double total = 0.0;
+        if (split) {
+            if (mine) total = seg_total(a, t.v, c);
+        } else {
+            double part = 0.0;
+            for (int base = t.sb; base < t.se; base += 32) {
+                const int edge = base + lane;
+                int x = 0;
+                bool ok = false;
+                if (edge < t.se) {
+                    x = __ldg(a.idx + edge);
+                    ok = edge == t.b || __ldg(a.idx + edge - 1) != x;
+                }
+                for (unsigned bal = __ballot_sync(0xffffffffu, ok); bal; bal &= bal - 1u) {
+                    const long long at = (long long)__shfl_sync(0xffffffffu, x, __ffs(bal) - 1) * a.k + c;
+                    if (mine && __ldg(a.dist + at) == a.level + 1) part += (1.0 + a.delta[at]) / a.sigma[at];
+                }
+            }
+            total += part;
+            if (a.scanned && lane == 0) atomicAdd(a.scanned, (unsigned long long)(t.se - t.sb));
+        }
+        if (!mine) continue;
+        if (t.seg >= 0) a.seg_part[(long long)t.seg * a.k + c] = total;
+        else a.delta[(long long)t.v * a.k + c] = a.sigma[(long long)t.v * a.k + c] * total;
+    }
+}
+
+// out[r, c] = value for every column c < k whose bit is set in `nw` and clear in `old` (fp64 tile); one thread per
+// (row, word)
+__global__ void __launch_bounds__(256) k_bits_fill_f64(const unsigned *__restrict__ nw, const unsigned *__restrict__ old,
+                                                       double *__restrict__ out, long long rows, int k, int words, double value) {
+    const int used = (k + 31) / 32;
+    const long long total = rows * used;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long r = i / used;
+        const int w = (int)(i - r * used);
+        double *orow = out + r * k + w * 32;
+        for (unsigned m = nw[r * words + w] & ~old[r * words + w] & bit_col_mask(w, k); m; m &= m - 1u) orow[__ffs(m) - 1] = value;
+    }
+}
+
+// out[r] = x[r, 0] + x[r, 1] + ... + x[r, k - 1], left to right from 0 (fp64); a thread per row
+__global__ void __launch_bounds__(256) k_row_sum_f64(const double *__restrict__ x, double *__restrict__ out, long long rows, int k) {
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (long long)gridDim.x * blockDim.x) {
+        const double *xr = x + r * k;
+        double s = 0.0;
+        for (int c = 0; c < k; ++c) s += xr[c];
+        out[r] = s;
+    }
+}
+
+// the segments of the lists longer than PATH_SEG entries, {row, first, end, 0} sorted by row and first (synchronises)
+cudaError_t build_segs(Adj &a) {
+    a.has_segs = true;
+    if (a.m <= (int64_t)PATH_SEG) return cudaSuccess;
+    std::vector<int> ptr((size_t)a.n + 1);
+    cudaError_t e = cudaMemcpy(ptr.data(), a.indptr, ptr.size() * 4, cudaMemcpyDeviceToHost);
+    std::vector<int4> segs;
+    for (int64_t v = 0; e == cudaSuccess && v < a.n; ++v)
+        if (ptr[v + 1] - ptr[v] > PATH_SEG)
+            for (int b = ptr[v]; b < ptr[v + 1]; b += PATH_SEG)
+                segs.push_back(make_int4((int)v, b, std::min(b + PATH_SEG, ptr[v + 1]), 0));
+    if (e == cudaSuccess && !segs.empty()) e = cudaMalloc(&a.segs, segs.size() * sizeof(int4));
+    if (e == cudaSuccess && !segs.empty()) e = cudaMemcpy(a.segs, segs.data(), segs.size() * sizeof(int4), cudaMemcpyHostToDevice);
+    a.n_segs = e == cudaSuccess ? (int)segs.size() : 0;
+    return e;
+}
+
+// the segment pass over the adjacency's segments (their partials into a.seg_part, grown to n_segs x k), then the row pass
+// over `n_rows` rows, on the parents pass's grid
+int launch_paths(arrow_ctx *ctx, PathArgs p, Adj *adj, long long n_rows, bool dependencies) {
+    if (n_rows == 0) return ARROW_OK;
+    const int per_sm = ctx->spmm_ctas_per_sm > 0 ? std::min(ctx->spmm_ctas_per_sm, 8) : 8;
+    const int sms = ctx->spmm_sm_limit > 0 ? std::min(ctx->sm_count, ctx->spmm_sm_limit) : ctx->sm_count;
+    if (std::max<long long>(n_rows, adj->n_segs) * p.used > INT_MAX)
+        return fail(ctx, ARROW_ERR_RANGE, "%lld rows x %d words exceed the int32 item count", std::max<long long>(n_rows, adj->n_segs), p.used);
+    const size_t part_bytes = (size_t)adj->n_segs * p.k * sizeof(double);
+    if (part_bytes > adj->seg_part_bytes) {
+        cudaFree(adj->seg_part);                              // waits for the launches that read it
+        adj->seg_part = nullptr;
+        adj->seg_part_bytes = 0;
+        CUDA_TRY(ctx, cudaMalloc(&adj->seg_part, part_bytes));
+        adj->seg_part_bytes = part_bytes;
+    }
+    p.segs = adj->segs;
+    p.n_segs = adj->n_segs;
+    p.seg_part = adj->seg_part;
+    const int *rows = p.rows;
+    for (int pass = 0; pass < 2; ++pass) {
+        p.rows = pass == 0 ? nullptr : rows;
+        p.n_items = (int)((pass == 0 ? adj->n_segs : n_rows) * p.used);
+        if (p.n_items == 0) continue;
+        const int grid = (int)std::min<long long>((p.n_items + 7) / 8, (long long)per_sm * sms);
+        if (dependencies) k_bits_dependencies<<<grid, 256, 0, cur_stream(ctx)>>>(p);
+        else k_bits_path_counts<<<grid, 256, 0, cur_stream(ctx)>>>(p);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+    }
+    return ARROW_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // direction-optimising shortest and critical paths on fp32 tiles (min-plus, max-plus).  With add_identity a fused step is
 // F(X)[v] = ⊕ over in-edges (u, a) of v of fl(a + X[u]), NaN terms dropped, the in-edges being the identity diagonal and
 // every level's entries through its row map.  Inside a fixed-point loop, X_h = F(X_{h-1}) <= X_{h-1}; a row whose bits did
@@ -5098,19 +5341,7 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e == cudaSuccess && incoming && m > (unsigned long long)PARENT_SEG) {   // the segments of the long in-lists
-        std::vector<int> ptr((size_t)n_vertices + 1);
-        e = cudaMemcpy(ptr.data(), a.indptr, ptr.size() * 4, cudaMemcpyDeviceToHost);
-        std::vector<int4> segs;
-        for (int64_t v = 0; e == cudaSuccess && v < n_vertices; ++v)
-            if (ptr[v + 1] - ptr[v] > PARENT_SEG)
-                for (int b = ptr[v]; b < ptr[v + 1]; b += PARENT_SEG)
-                    segs.push_back(make_int4((int)v, b, std::min(b + PARENT_SEG, ptr[v + 1]), 0));
-        if (e == cudaSuccess && !segs.empty()) e = cudaMalloc(&a.segs, segs.size() * sizeof(int4));
-        if (e == cudaSuccess && !segs.empty())
-            e = cudaMemcpy(a.segs, segs.data(), segs.size() * sizeof(int4), cudaMemcpyHostToDevice);
-        a.n_segs = (int)segs.size();
-    }
+    if (e == cudaSuccess && incoming) e = build_segs(a);       // the segments of the long in-lists
     if (e != cudaSuccess) {
         cudaGetLastError();
         adj_release(a);
@@ -5324,6 +5555,178 @@ int arrow_bits_parents(arrow_ctx *ctx, int in_adj, int adj, int new_buf, int old
         CUDA_TRY(ctx, cudaStreamSynchronize(cur_stream(ctx)));
         *edges_scanned = (int64_t)h;
     }
+    return ARROW_OK;
+}
+
+namespace {
+// reads back the optional edge counter of a path-count / dependency pass (synchronises)
+int read_scanned(arrow_ctx *ctx, const DevTmp &cnt, int64_t *edges_scanned) {
+    if (!edges_scanned) return ARROW_OK;
+    unsigned long long h = 0;
+    CUDA_TRY(ctx, cudaMemcpyAsync(&h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, cur_stream(ctx)));
+    CUDA_TRY(ctx, cudaStreamSynchronize(cur_stream(ctx)));
+    *edges_scanned = (int64_t)h;
+    return ARROW_OK;
+}
+int alloc_scanned(arrow_ctx *ctx, DevTmp &cnt, int64_t *edges_scanned, PathArgs &p) {
+    if (!edges_scanned) return ARROW_OK;
+    *edges_scanned = 0;
+    CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof(unsigned long long)));
+    CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof(unsigned long long), cur_stream(ctx)));
+    p.scanned = reinterpret_cast<unsigned long long *>(cnt.p);
+    return ARROW_OK;
+}
+}  // namespace
+
+int arrow_bits_path_counts(arrow_ctx *ctx, int in_adj, int adj, int new_buf, int old_buf, int sigma_buf, int64_t *edges_scanned) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    Adj *in = get_adj(ctx, in_adj);
+    const Adj *a = get_adj(ctx, adj);
+    if (!in || !a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle (in=%d adj=%d)", in_adj, adj);
+    DenseBuf *N = get_dense(ctx, new_buf), *O = get_dense(ctx, old_buf), *S = get_dense(ctx, sigma_buf);
+    if (!N || !O || !S) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (new=%d old=%d sigma=%d)", new_buf, old_buf, sigma_buf);
+    if (!in->incoming || a->incoming)
+        return fail(ctx, ARROW_ERR_ARG, "in_adj is the in-adjacency (arrow_adj_build_in) and adj the push adjacency");
+    if (in->n != a->n)
+        return fail(ctx, ARROW_ERR_ARG, "the adjacencies differ in vertices: in %lld, push %lld", (long long)in->n, (long long)a->n);
+    if (N->dtype != ARROW_B1 || O->dtype != ARROW_B1 || S->dtype != ARROW_F64)
+        return fail(ctx, ARROW_ERR_ARG, "new / old are bit tiles and sigma a float64 tile: got %s / %s / %s", dtype_name(N->dtype),
+                    dtype_name(O->dtype), dtype_name(S->dtype));
+    if (N->rows != a->n || O->rows != N->rows || S->rows != N->rows || O->k != N->k || S->k != N->k)
+        return fail(ctx, ARROW_ERR_ARG, "shape: new %lld x %d, old %lld x %d, sigma %lld x %d, adjacency %lld rows",
+                    (long long)N->rows, N->k, (long long)O->rows, O->k, (long long)S->rows, S->k, (long long)a->n);
+    if (new_buf == old_buf || N->p == O->p) return fail(ctx, ARROW_ERR_ARG, "old aliases new");
+    if (a->tag < 0) return fail(ctx, ARROW_ERR_ARG, "no frontier record: run arrow_bits_mark_frontier on the adjacency first");
+    if (new_buf != a->tag || N->p != a->tag_p || N->k != a->tag_k)
+        return fail(ctx, ARROW_ERR_ARG, "new (tile %d) is not the tile of the last arrow_bits_mark_frontier (tile %d)", new_buf, a->tag);
+    if (N->k > BITS_MAX_K) return fail(ctx, ARROW_ERR_UNSUPPORTED, "k=%d > %d", N->k, BITS_MAX_K);
+    PathArgs p{};
+    DevTmp cnt;
+    if (const int rc = alloc_scanned(ctx, cnt, edges_scanned, p)) return rc;
+    if (N->rows == 0 || N->k == 0 || a->n_front == 0) return read_scanned(ctx, cnt, edges_scanned);
+    p.nw = reinterpret_cast<const unsigned *>(N->p);
+    p.old = reinterpret_cast<const unsigned *>(O->p);
+    p.sigma = reinterpret_cast<double *>(S->p);
+    p.ptr = in->indptr;
+    p.idx = in->indices;
+    p.rows = a->front_rows;
+    p.k = N->k;
+    p.words = bit_row_words(N->k);
+    p.used = (N->k + 31) / 32;
+    if (const int rc = launch_paths(ctx, p, in, a->n_front, false)) return rc;
+    return read_scanned(ctx, cnt, edges_scanned);
+}
+
+int arrow_adj_keep_record(arrow_ctx *ctx, int adj, int level) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
+    if (a->tag < 0) return fail(ctx, ARROW_ERR_ARG, "no frontier record: run arrow_bits_mark_frontier on the adjacency first");
+    const int kept = a->hist_off.empty() ? 0 : (int)a->hist_off.size() - 1;
+    if (level != 0 && level != kept)
+        return fail(ctx, ARROW_ERR_ARG, "level %d: the history holds levels 0..%d, the next one kept is %d (or 0 to restart)", level,
+                    kept - 1, kept);
+    if (level == 0) a->hist_off.assign(1, 0);
+    const int64_t at = a->hist_off.back(), need = at + a->n_front;
+    cudaStream_t s = cur_stream(ctx);
+    if (need > a->hist_cap) {
+        const int64_t cap = std::max<int64_t>({need, 2 * a->hist_cap, 1024});
+        int *grown = nullptr;
+        CUDA_TRY(ctx, cudaMalloc(&grown, (size_t)cap * 4));
+        if (at > 0) {
+            const cudaError_t e = cudaMemcpyAsync(grown, a->hist, (size_t)at * 4, cudaMemcpyDeviceToDevice, s);
+            if (e != cudaSuccess) {
+                cudaFree(grown);
+                return fail(ctx, ARROW_ERR_CUDA, "history copy: %s", cudaGetErrorString(e));
+            }
+        }
+        cudaFree(a->hist);                                    // waits for the copy
+        a->hist = grown;
+        a->hist_cap = cap;
+    }
+    if (a->n_front > 0) CUDA_TRY(ctx, cudaMemcpyAsync(a->hist + at, a->front_rows, (size_t)a->n_front * 4, cudaMemcpyDeviceToDevice, s));
+    a->hist_off.push_back(need);
+    return ARROW_OK;
+}
+
+int arrow_bits_dependencies(arrow_ctx *ctx, int adj, int level, int dist_buf, int sigma_buf, int delta_buf, int64_t *edges_scanned) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    Adj *a = get_adj(ctx, adj);
+    if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
+    if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
+    if (a->weighted) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is weighted (it keeps the edges u == v)", adj);
+    DenseBuf *D = get_dense(ctx, dist_buf), *S = get_dense(ctx, sigma_buf), *T = get_dense(ctx, delta_buf);
+    if (!D || !S || !T) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (dist=%d sigma=%d delta=%d)", dist_buf, sigma_buf, delta_buf);
+    if (D->dtype != ARROW_I32 || S->dtype != ARROW_F64 || T->dtype != ARROW_F64)
+        return fail(ctx, ARROW_ERR_ARG, "dist is an int32 tile and sigma / delta float64 tiles: got %s / %s / %s", dtype_name(D->dtype),
+                    dtype_name(S->dtype), dtype_name(T->dtype));
+    if (D->rows != a->n || S->rows != D->rows || T->rows != D->rows || S->k != D->k || T->k != D->k)
+        return fail(ctx, ARROW_ERR_ARG, "shape: dist %lld x %d, sigma %lld x %d, delta %lld x %d, adjacency %lld rows",
+                    (long long)D->rows, D->k, (long long)S->rows, S->k, (long long)T->rows, T->k, (long long)a->n);
+    if (sigma_buf == delta_buf || S->p == T->p) return fail(ctx, ARROW_ERR_ARG, "delta aliases sigma");
+    const int kept = a->hist_off.empty() ? 0 : (int)a->hist_off.size() - 1;
+    if (level < 1 || level >= kept)
+        return fail(ctx, ARROW_ERR_ARG, "level %d: the history holds levels 0..%d (arrow_adj_keep_record), the sweep runs 1..%d", level,
+                    kept - 1, kept - 1);
+    PathArgs p{};
+    DevTmp cnt;
+    if (const int rc = alloc_scanned(ctx, cnt, edges_scanned, p)) return rc;
+    const int64_t n_rows = a->hist_off[level + 1] - a->hist_off[level];
+    if (D->k == 0 || n_rows == 0) return read_scanned(ctx, cnt, edges_scanned);
+    if (!a->has_segs) CUDA_TRY(ctx, build_segs(*a));         // the segments of the long out-lists, on first use
+    p.dist = reinterpret_cast<const int *>(D->p);
+    p.sigma = reinterpret_cast<double *>(S->p);
+    p.delta = reinterpret_cast<double *>(T->p);
+    p.ptr = a->indptr;
+    p.idx = a->indices;
+    p.rows = a->hist + a->hist_off[level];
+    p.k = D->k;
+    p.used = (D->k + 31) / 32;
+    p.level = level;
+    if (const int rc = launch_paths(ctx, p, a, n_rows, true)) return rc;
+    return read_scanned(ctx, cnt, edges_scanned);
+}
+
+int arrow_bits_fill_f64(arrow_ctx *ctx, int new_buf, int old_buf, int out_buf, double value) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    DenseBuf *N = get_dense(ctx, new_buf), *O = get_dense(ctx, old_buf), *X = get_dense(ctx, out_buf);
+    if (!N || !O || !X) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (new=%d old=%d out=%d)", new_buf, old_buf, out_buf);
+    if (N->dtype != ARROW_B1 || O->dtype != ARROW_B1 || X->dtype != ARROW_F64)
+        return fail(ctx, ARROW_ERR_ARG, "new / old are bit tiles and out a float64 tile: got %s / %s / %s", dtype_name(N->dtype),
+                    dtype_name(O->dtype), dtype_name(X->dtype));
+    if (N->rows != O->rows || N->k != O->k || X->rows != N->rows || X->k != N->k)
+        return fail(ctx, ARROW_ERR_ARG, "tiles differ in shape: new %lld x %d, old %lld x %d, out %lld x %d", (long long)N->rows, N->k,
+                    (long long)O->rows, O->k, (long long)X->rows, X->k);
+    const long long items = N->rows * (long long)((N->k + 31) / 32);
+    if (items == 0) return ARROW_OK;
+    const int grid = (int)std::min<long long>((items + 255) / 256, (long long)ctx->sm_count * 8);
+    k_bits_fill_f64<<<grid, 256, 0, cur_stream(ctx)>>>(reinterpret_cast<const unsigned *>(N->p), reinterpret_cast<const unsigned *>(O->p),
+                                                       reinterpret_cast<double *>(X->p), N->rows, N->k, bit_row_words(N->k), value);
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return ARROW_OK;
+}
+
+int arrow_dense_row_sum(arrow_ctx *ctx, int in_buf, int out_buf) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    DenseBuf *X = get_dense(ctx, in_buf), *Y = get_dense(ctx, out_buf);
+    if (!X || !Y) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (in=%d out=%d)", in_buf, out_buf);
+    if (X->dtype != ARROW_F64 || Y->dtype != ARROW_F64)
+        return fail(ctx, ARROW_ERR_ARG, "in / out are float64 tiles: got %s / %s", dtype_name(X->dtype), dtype_name(Y->dtype));
+    if (Y->rows != X->rows || Y->k != 1)
+        return fail(ctx, ARROW_ERR_ARG, "out is %lld x %d, expected %lld x 1", (long long)Y->rows, Y->k, (long long)X->rows);
+    if (in_buf == out_buf || X->p == Y->p) return fail(ctx, ARROW_ERR_ARG, "out aliases in");
+    if (X->rows == 0) return ARROW_OK;
+    const int grid = (int)std::min<long long>((X->rows + 255) / 256, (long long)ctx->sm_count * 8);
+    k_row_sum_f64<<<grid, 256, 0, cur_stream(ctx)>>>(reinterpret_cast<const double *>(X->p), reinterpret_cast<double *>(Y->p), X->rows, X->k);
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
     return ARROW_OK;
 }
 

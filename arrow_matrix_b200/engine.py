@@ -137,6 +137,8 @@ class ArrowEngine:
         self._adj: Optional[_lib.Adjacency] = None               # bfs_levels(): the push adjacency, built on first use
         self._in_adj: Optional[_lib.Adjacency] = None            # bfs_tree(): the in-adjacency, built on first use
         self._bfs_parents: Optional[_lib.Dense] = None           # bfs_tree(): the int32 parent tile
+        self._bfs_sigma: Optional[_lib.Dense] = None            # bfs_path_counts(): the float64 path-count tile
+        self._bfs_delta: Optional[Tuple[_lib.Dense, ...]] = None  # betweenness(): float64 dependencies and [n x 1] bc
         self._push_limit: Optional[int] = None                   # None: bfs_direction() decides; else push iff edges < it
         self.last_fixed_point_directions: List[str] = []         # "push" / "pull" per step of iterate_to_fixed_point()
         self._sr_adj: Optional[_lib.Adjacency] = None            # iterate_to_fixed_point(): weighted push adjacency
@@ -575,15 +577,95 @@ class ArrowEngine:
             self._bfs_parents = self.ctx.dense_alloc(self.levels[0].rows, self.k, np.int32)
         return self._bfs_run(max_steps, self._bfs_parents), self._bfs_parents
 
+    def bfs_path_counts(self, max_steps: int, levels_out: Optional[np.ndarray] = None,
+                        counts_out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """``bfs_levels`` that also returns the shortest-path counts (levels int32, counts float64, both [n x k] in
+        level-0 row order like ``result()``): ``sigma[v, s]`` is 1 where ``L[v, s] = 0``, 0 where ``L[v, s] = -1``, and
+        otherwise the sum of ``sigma[u, s]`` over the distinct edges ``u -> v`` of the fused step's operator (``u != v``)
+        with ``L[u, s] = L[v, s] - 1``.  A column with several sources counts paths from any of them.  The sums run in
+        ascending ``u``, 512 in-list entries at a time, the partials added in order (DESIGN.md §4): the counts are exact
+        below 2^53 and bit-reproducible beyond.  The levels, ``last_bfs_steps``, ``last_bfs_directions`` and the features
+        are those of ``bfs_levels``.
+
+        After each level's record one more device pass sums the in-lists of the rows that gained a bit.  The in-adjacency
+        and the float64 count tile (8 bytes per element: 10.2 GB at 10M rows and k = 128, beside the 5.1 GB level tile)
+        are made on the first call and kept until ``close()``.  Raises ``ValueError`` before any CUDA work where
+        ``bfs_tree`` does.  Synchronises."""
+        dist, sigma = self._bfs_paths_run(max_steps, "bfs_path_counts")
+        return dist.d2h(levels_out), sigma.d2h(counts_out)
+
+    def betweenness(self, max_steps: int, out: Optional[np.ndarray] = None,
+                    dependencies_out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Brandes betweenness over the engine's ``k`` source columns: float64 ``bc[v] = sum over s < k of delta[v, s]``,
+        in level-0 row order like ``result()``, summed in column order.  ``delta[v, s]`` is 0 where ``L[v, s] <= 0``, and
+        otherwise ``sigma[v, s]`` (``bfs_path_counts``) times the sum of ``fl((1 + delta[w, s]) / sigma[w, s])`` over the
+        distinct edges ``v -> w`` with ``L[w, s] = L[v, s] + 1`` (0 at the last level and at ``max_steps``), summed in
+        ascending ``w`` like the counts.  With one source per column this is the unnormalised betweenness restricted to
+        those sources, counting ordered pairs ``(s, t)``: twice networkx's undirected figure on a symmetric operator.
+        ``dependencies_out`` (float64 [n x k]) receives ``delta``.  Levels run as in ``bfs_levels``
+        (``last_bfs_steps``, ``last_bfs_directions``).
+
+        The forward part is ``bfs_path_counts`` keeping each level's frontier rows (4 bytes per row and level in which
+        it gained a bit); the backward sweep then visits, from the deepest level to 1, only that level's rows along the
+        push adjacency's out-lists, and one pass sums each row.  The dependency tile (8 bytes per element, as the count
+        tile) is allocated on the first call and kept until ``close()``.  Raises ``ValueError`` before any CUDA work where
+        ``bfs_tree`` does.  Synchronises."""
+        self._paths_checks("betweenness")
+        n = self.levels[0].rows
+        for name, arr, shape in (("out", out, (n,)), ("dependencies_out", dependencies_out, (n, self.k))):
+            if arr is not None and (arr.dtype != np.float64 or arr.shape != shape or not arr.flags.c_contiguous):
+                raise ValueError(f"{name} must be a C-contiguous float64 array of shape {shape}, got {arr.dtype} "
+                                 f"{arr.shape}{'' if arr.flags.c_contiguous else ' (not contiguous)'}")
+        delta, bc = self._betweenness_run(max_steps)
+        if dependencies_out is not None:
+            delta.d2h(dependencies_out)
+        if out is None:
+            return bc.d2h().reshape(-1)
+        bc.d2h(out[:, None])                    # a view of out: the rows land in it
+        return out
+
+    def _betweenness_run(self, max_steps: int) -> Tuple[_lib.Dense, _lib.Dense]:
+        """the device part of ``betweenness``: the float64 dependency and [n x 1] betweenness tiles, left on the device"""
+        dist, sigma = self._bfs_paths_run(max_steps, "betweenness")
+        if self._bfs_delta is None:
+            n = self.levels[0].rows
+            self._bfs_delta = (self.ctx.dense_alloc(n, self.k, np.float64), self.ctx.dense_alloc(n, 1, np.float64))
+        delta, bc = self._bfs_delta
+        delta.fill(0.0)
+        for level in range(self.last_bfs_steps, 0, -1):
+            self.ctx.bits_dependencies(self._adj, level, dist, sigma, delta)
+        self.ctx.row_sum(delta, bc)
+        return delta, bc
+
+    def _bfs_paths_run(self, max_steps: int, what: str) -> Tuple[_lib.Dense, _lib.Dense]:
+        """the device part of ``bfs_path_counts``: the int32 level and float64 count tiles, left on the device, with the
+        frontier rows of levels 0 .. ``last_bfs_steps`` kept in the push adjacency's history"""
+        self._paths_checks(what)
+        if self._in_adj is None:
+            parts = [(st.csr, st.cmap_dev) for st in self.levels]
+            self._in_adj = self.ctx.adj_build(parts, self.levels[0].rows, direction="in")
+        if self._bfs_sigma is None:
+            self._bfs_sigma = self.ctx.dense_alloc(self.levels[0].rows, self.k, np.float64)
+        return self._bfs_run(max_steps, sigma=self._bfs_sigma), self._bfs_sigma
+
+    def _paths_checks(self, what: str):
+        self._bfs_checks(what)
+        if not self.fused_ok:
+            raise ValueError(f"{what} needs a level-0 row behind every non-zero, but a level reads rows behind the "
+                             "sentinel")
+
     def _bfs_checks(self, what: str):
         if not self.bits:
             raise ValueError(f"{what} runs the or_and semiring, the engine runs {self.semiring}")
         if not self.add_identity:
             raise ValueError(f"{what} needs add_identity=True: a step must keep the bits it already has")
 
-    def _bfs_run(self, max_steps: int, parents: Optional[_lib.Dense] = None) -> _lib.Dense:
+    def _bfs_run(self, max_steps: int, parents: Optional[_lib.Dense] = None,
+                 sigma: Optional[_lib.Dense] = None) -> _lib.Dense:
         """the device part of ``bfs_levels``: runs the levels and returns the int32 level tile, left on the device.  With
-        ``parents`` (``bfs_tree``) also writes the parent of every element into that int32 tile."""
+        ``parents`` (``bfs_tree``) also writes the parent of every element into that int32 tile; with ``sigma``
+        (``bfs_path_counts``) the path count of every element into that float64 tile, and keeps every level's frontier
+        rows in the push adjacency's history."""
         self._bfs_checks("bfs_levels")
         self.sync()
         st0 = self.levels[0]
@@ -595,8 +677,8 @@ class ArrowEngine:
         # an exchange-mode step of one level has no backward exchange and leaves level 0's features where they are, so a
         # push (which advances them like a fused step) would not match it: that engine pulls every level
         pushes = self.fused_ok and (self.mode == "fused" or self.L > 1)
-        # the parent pass reads the frontier record, so bfs_tree keeps one even on an engine that only pulls
-        adj = self._push_adjacency() if pushes or parents is not None else None
+        # the parent and path-count passes read the frontier record, so they keep one even on an engine that only pulls
+        adj = self._push_adjacency() if pushes or parents is not None or sigma is not None else None
         limit = self._push_limit
 
         def mark(new, old, level):
@@ -606,6 +688,10 @@ class ArrowEngine:
             n_new, _, edges = self.ctx.bits_mark_frontier(adj, new, old, dist, level)
             if parents is not None and level > 0:        # old is X_{h-1} until the next level writes its tile
                 self.ctx.bits_parents(self._in_adj, adj, new, old, parents)
+            if sigma is not None:
+                if level > 0:
+                    self.ctx.bits_path_counts(self._in_adj, adj, new, old, sigma)
+                self.ctx.adj_keep_record(adj, level)
             if not pushes:
                 return n_new, False
             push = edges < limit if limit is not None else bfs_direction(edges, self.total_nnz) == "push"
@@ -613,6 +699,9 @@ class ArrowEngine:
 
         if parents is not None:                          # the sources have no parent
             self.ctx.bits_mark_new(st0.bufs[st0.xi], zero, parents, -1)
+        if sigma is not None:                            # one path to each source, none to an element never reached
+            sigma.fill(0.0)
+            self.ctx.bits_fill_f64(st0.bufs[st0.xi], zero, sigma, 1.0)
         _, push = mark(st0.bufs[st0.xi], zero, 0)
         steps, directions = 0, []
         for level in range(1, int(max_steps) + 1):
@@ -756,5 +845,8 @@ class ArrowEngine:
             if a is not None:
                 a.free()
         self._wit_labels, self._wit_values, self._bfs_tiles, self._adj, self._sr_adj = None, {}, None, None, None
-        self._in_adj = self._bfs_parents = None
+        for b in (self._bfs_sigma,) + (self._bfs_delta or ()):
+            if b is not None:
+                b.free()
+        self._in_adj = self._bfs_parents = self._bfs_sigma = self._bfs_delta = None
         self.ctx.close()

@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 10
+#define ARROW_ABI_VERSION 11
 
 /* error codes */
 #define ARROW_OK              0
@@ -284,6 +284,45 @@ int  arrow_adj_build_in(arrow_ctx *ctx, int n_parts, const int *csrs, const int 
  * the same rows and k, in_adj not an in-adjacency or adj one, adjacencies of different vertex counts, rows other than
  * theirs, no record in adj or one for another tile, new_buf == old_buf; ARROW_ERR_UNSUPPORTED: k > 8192. */
 int  arrow_bits_parents(arrow_ctx *ctx, int in_adj, int adj, int new_buf, int old_buf, int parent_buf, int64_t *edges_scanned);
+
+/* ---- betweenness on bit tiles (one GPU): shortest-path counts and Brandes dependencies over k source columns ---------- */
+/* M is taken as a set here: a list entry equal to its predecessor is skipped.  Every sum below runs over a list in
+ * ascending order, 512 entries at a time from the row's start: each segment is summed left to right into a partial starting
+ * at 0 and the partials are added in segment order.  Lists longer than 512 entries are split across warps at the
+ * adjacency's 512-entry segments, their partials kept in a scratch of 8 * k bytes per segment owned by the adjacency.  No
+ * floating-point atomics: the results depend on neither the grid nor the launch. */
+/* Path counts of one level.  For every row v of adj's frontier record (written by arrow_bits_mark_frontier for new_buf
+ * against old_buf) and every bit (v, s), s < k, set in new_buf and clear in old_buf: sigma[v, s] = the sum of sigma[u, s]
+ * over the distinct u of in_adj's row v whose bit s is set in old_buf.  Every other element of sigma_buf is left alone.
+ * When new = X_h = X_{h-1} | M X_{h-1} and old = X_{h-1} those u are the in-neighbours at level h - 1, so sigma holds the
+ * shortest-path counts of level h once it holds those of level h - 1.  edges_scanned (may be NULL; then the call does
+ * not synchronise) receives the in-list entries read, once per row and 32-column word with a fresh bit.  ARROW_ERR_ARG:
+ * non-bit new / old, a sigma tile that is not ARROW_F64 of the same rows and k, in_adj not an in-adjacency or adj one,
+ * adjacencies of different vertex counts, rows other than theirs, no record in adj or one for another tile,
+ * new_buf == old_buf; ARROW_ERR_UNSUPPORTED: k > 8192. */
+int  arrow_bits_path_counts(arrow_ctx *ctx, int in_adj, int adj, int new_buf, int old_buf, int sigma_buf, int64_t *edges_scanned);
+/* Keeps a copy of adj's current frontier record as level `level` of the adjacency's history: level 0 clears the history
+ * first, any other level must be the next one (the number of levels kept).  4 bytes per recorded row (one BFS keeps at
+ * most n * min(k, levels + 1) rows); the device buffer doubles when it runs out, so it holds up to twice the rows kept (at
+ * least 1024), the old and new buffers coexist while it grows (up to three times), and it is kept at its largest size
+ * until the adjacency is freed.
+ * ARROW_ERR_ARG: an in-adjacency, no record, another level.  Stream-ordered. */
+int  arrow_adj_keep_record(arrow_ctx *ctx, int adj, int level);
+/* Dependencies of one level, 1 <= level < the levels kept.  For every row u of the history's level `level` and every
+ * column s with dist[u, s] == level: delta[u, s] = sigma[u, s] * (the sum of fl((1 + delta[w, s]) / sigma[w, s]) over
+ * the distinct w of adj's row u with dist[w, s] == level + 1; 0 when there is none).  Every other element of delta_buf is
+ * left alone; run the levels from the deepest down to 1.  edges_scanned (may be NULL; then the call does not synchronise)
+ * receives the out-list entries read, once per row and 32-column word holding the level.  ARROW_ERR_ARG: an in-adjacency,
+ * a weighted adjacency, dist not ARROW_I32 or sigma / delta not ARROW_F64, shapes other than the adjacency's rows and
+ * dist's k, delta aliasing sigma, a level outside the history.  The first call lists the push adjacency's segments
+ * (synchronises). */
+int  arrow_bits_dependencies(arrow_ctx *ctx, int adj, int level, int dist_buf, int sigma_buf, int delta_buf, int64_t *edges_scanned);
+/* out[r, s] = value for every bit (r, s), s < k, set in new_buf and clear in old_buf; out is an ARROW_F64 tile of the
+ * same rows and k, its other elements left alone.  ARROW_ERR_ARG: non-bit new / old, another out type or shape. */
+int  arrow_bits_fill_f64(arrow_ctx *ctx, int new_buf, int old_buf, int out_buf, double value);
+/* out[r, 0] = in[r, 0] + in[r, 1] + ... + in[r, k - 1], summed left to right from 0; in ARROW_F64 [rows x k], out
+ * ARROW_F64 [rows x 1].  ARROW_ERR_ARG: other types or shapes, out aliasing in. */
+int  arrow_dense_row_sum(arrow_ctx *ctx, int in_buf, int out_buf);
 
 /* ---- direction-optimising shortest and critical paths (one GPU, min-plus / max-plus on fp32 tiles) ---------------------- */
 /* The push adjacency of arrow_adj_build carrying each edge's fp32 weight (the entry's value), with the edges u == v kept
