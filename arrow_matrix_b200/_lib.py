@@ -9,7 +9,7 @@ from __future__ import annotations
 import ctypes
 import os
 from ctypes import (POINTER, byref, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_void_p)
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -51,8 +51,9 @@ EXPORTS = [
     "arrow_bits_push_frontier", "arrow_adj_build_weighted", "arrow_adj_values_d2h", "arrow_sr_mark_frontier",
     "arrow_sr_push_frontier", "arrow_adj_build_in", "arrow_bits_parents", "arrow_bits_path_counts",
     "arrow_adj_keep_record", "arrow_bits_dependencies", "arrow_bits_fill_f64", "arrow_dense_row_sum",
+    "arrow_adj_build_loopfree", "arrow_wpaths_counts", "arrow_wpaths_dependencies",
 ]
-ABI_VERSION = 11       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 12       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -171,6 +172,9 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_bits_dependencies": (c_int, [P, I, I, I, I, I, pI64]),
         "arrow_bits_fill_f64": (c_int, [P, I, I, I, c_double]),
         "arrow_dense_row_sum": (c_int, [P, I, I]),
+        "arrow_adj_build_loopfree": (c_int, [P, I, pI, pI, I64, I, pI]),
+        "arrow_wpaths_counts": (c_int, [P, I, I, I, I, I, I, pI64, pI64]),
+        "arrow_wpaths_dependencies": (c_int, [P, I, I, I, I, I, I, pI64]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -557,6 +561,41 @@ class Context:
     def row_sum(self, x: "Dense", out: "Dense"):
         """out[r, 0] = x[r, 0] + ... + x[r, k - 1], left to right (float64 tiles; ``arrow_dense_row_sum``)"""
         self._check(self.lib.arrow_dense_row_sum(self._h, x.h, out.h))
+
+    def adj_build_loopfree(self, parts: Sequence[tuple], n_vertices: int, direction: str = "out") -> "Adjacency":
+        """The weighted adjacency of ``adj_build`` without the edges u == v (``arrow_adj_build_loopfree``): the lists of
+        ``adj_build(parts, n)`` (``direction="out"``) or ``adj_build(parts, n, direction="in")``, every entry carrying its
+        fp32 weight -- the lists of the weighted path passes.  Synchronises."""
+        if direction not in ("out", "in"):
+            raise ValueError(f"direction must be 'out' or 'in', got {direction!r}")
+        n = len(parts)
+        csrs = (c_int * max(n, 1))(*[A.h for A, _ in parts])
+        maps = (c_int * max(n, 1))(*[m.h if m is not None else -1 for _, m in parts])
+        h = c_int()
+        self._check(self.lib.arrow_adj_build_loopfree(self._h, n, csrs, maps, int(n_vertices), int(direction == "in"),
+                                                      byref(h)))
+        return Adjacency(self, h.value)
+
+    def wpaths_counts(self, in_adj: "Adjacency", out_adj: "Adjacency", x0: "Dense", dist: "Dense", state: "Dense",
+                      sigma: "Dense", count: bool = False) -> Tuple[int, Optional[int]]:
+        """sigma[v, s] = [v in S_s] + the sum of sigma[u, s] over the distinct tight pairs u -> v of the fixed point
+        ``dist`` started from ``x0``, by Kahn rounds over the tight pairs; ``state`` (int32) receives -(depth + 2), -1
+        where ``dist`` is not finite, and ``out_adj`` keeps every round's rows (``arrow_wpaths_counts``).  Returns (rounds,
+        list entries read with ``count``, else None); synchronises."""
+        rounds, n = c_int64(), c_int64()
+        self._check(self.lib.arrow_wpaths_counts(self._h, in_adj.h, out_adj.h, x0.h, dist.h, state.h, sigma.h, byref(rounds),
+                                                 byref(n) if count else None))
+        return int(rounds.value), (int(n.value) if count else None)
+
+    def wpaths_dependencies(self, out_adj: "Adjacency", x0: "Dense", dist: "Dense", state: "Dense", sigma: "Dense",
+                            delta: "Dense", count: bool = False) -> Optional[int]:
+        """delta[v, s] = 0 for v in S_s, else sigma[v, s] * the sum of fl((1 + delta[w, s]) / sigma[w, s]) over the
+        distinct tight pairs v -> w, over the rounds of the last ``wpaths_counts`` (``arrow_wpaths_dependencies``).  With
+        ``count`` returns the out-list entries read (synchronises), else None."""
+        n = c_int64()
+        self._check(self.lib.arrow_wpaths_dependencies(self._h, out_adj.h, x0.h, dist.h, state.h, sigma.h, delta.h,
+                                                       byref(n) if count else None))
+        return int(n.value) if count else None
 
     def sr_mark_frontier(self, adj: "Adjacency", new: "Dense", old: "Dense"):
         """(rows changed by value -- ``count_diff``'s figure --, frontier rows, frontier edges) of two fp32 tiles; records

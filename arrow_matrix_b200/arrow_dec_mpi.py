@@ -202,6 +202,20 @@ class ArrowDecompositionMPI:
         maps the rows to vertex ids."""
         return self._bfs_engine("betweenness").betweenness(max_steps, out, dependencies_out)
 
+    def shortest_path_counts(self, max_steps: int, distances_out: Optional[np.ndarray] = None,
+                             counts_out: Optional[np.ndarray] = None):
+        """Extension (one GPU, ``min_plus`` with ``add_identity``): ``iterate_to_fixed_point`` and the number of tight
+        shortest paths to every element, float32 distances and float64 counts in ``result_tile()`` row order (see
+        ``ArrowEngine.shortest_path_counts``)."""
+        return self._bfs_engine("shortest_path_counts").shortest_path_counts(max_steps, distances_out, counts_out)
+
+    def weighted_betweenness(self, max_steps: int, out: Optional[np.ndarray] = None,
+                             dependencies_out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension (one GPU, ``min_plus`` with ``add_identity``): Brandes betweenness over the weighted shortest paths
+        from the feature columns, float64 [n] in ``result_tile()`` row order (see ``ArrowEngine.weighted_betweenness``).
+        Level 0's permutation maps the rows to vertex ids."""
+        return self._bfs_engine("weighted_betweenness").weighted_betweenness(max_steps, out, dependencies_out)
+
     def _bfs_engine(self, what: str) -> ArrowEngine:
         if self.comm.Get_size() > 1:
             raise ValueError(f"{what} runs on one GPU only")

@@ -122,6 +122,9 @@ struct Adj {                          // push adjacency (arrow_adj_build / arrow
     int *hist = nullptr;              // device: the frontier records kept by arrow_adj_keep_record, level after level
     int64_t hist_cap = 0;             //   (its capacity in rows)
     std::vector<int64_t> hist_off;    // host: level h's rows are hist[hist_off[h], hist_off[h + 1])
+    bool loopfree = false;            // weighted without the edges u == v (arrow_adj_build_loopfree)
+    const void *wp_tag_p = nullptr;   // the state tile whose rounds the history holds (arrow_wpaths_counts), and its width
+    int wp_tag_k = 0;
     bool live = false;
 };
 
@@ -2878,10 +2881,10 @@ __device__ __forceinline__ int last_le(const int *__restrict__ a, int lo, int hi
 }
 
 // edges of one block: entry (r, c) with c >= 0 gives u -> v = map(c) -> map(r); an end at -1 drops it, and so does u == v
-// unless W (the weighted adjacency keeps self-loops: a negative one changes a min-plus step).  Counts them into *count;
-// with `keys` also appends (u << 32) | v at a warp-aggregated cursor (the order is fixed by the sort), and with W the
-// entry's value w_in[e] at the same slot of w_out.  IN appends (v << 32) | u instead: the in-adjacency, row v by source.
-template <bool W, bool IN = false>
+// unless LOOPS (the weighted push adjacency keeps self-loops: a negative one changes a min-plus step).  Counts them into
+// *count; with `keys` also appends (u << 32) | v at a warp-aggregated cursor (the order is fixed by the sort), and with W
+// the entry's value w_in[e] at the same slot of w_out.  IN appends (v << 32) | u instead: the in-adjacency, row v by source.
+template <bool W, bool IN = false, bool LOOPS = W>
 __global__ void __launch_bounds__(256) k_adj_edges(AdjPart p, unsigned long long *__restrict__ count,
                                                    unsigned long long *__restrict__ keys,
                                                    const float *__restrict__ w_in = nullptr, float *__restrict__ w_out = nullptr) {
@@ -2897,7 +2900,7 @@ __global__ void __launch_bounds__(256) k_adj_edges(AdjPart p, unsigned long long
                 const int r = last_le(p.indptr, 0, p.n_rows - 1, e);
                 const int u = p.map ? __ldg(p.map + c) : c;
                 const int v = p.map ? __ldg(p.map + r) : r;
-                ok = u >= 0 && v >= 0 && (W || u != v);
+                ok = u >= 0 && v >= 0 && (LOOPS || u != v);
                 key = IN ? ((unsigned long long)(unsigned)v << 32) | (unsigned)u
                          : ((unsigned long long)(unsigned)u << 32) | (unsigned)v;
             }
@@ -3430,12 +3433,18 @@ cudaError_t build_segs(Adj &a) {
     return e;
 }
 
-// the segment pass over the adjacency's segments (their partials into a.seg_part, grown to n_segs x k), then the row pass
-// over `n_rows` rows, on the parents pass's grid
-int launch_paths(arrow_ctx *ctx, PathArgs p, Adj *adj, long long n_rows, bool dependencies) {
-    if (n_rows == 0) return ARROW_OK;
+// the grid of a path pass over `items` warp items: the parents pass's CTAs per SM and SM cap
+int path_grid(const arrow_ctx *ctx, long long items) {
     const int per_sm = ctx->spmm_ctas_per_sm > 0 ? std::min(ctx->spmm_ctas_per_sm, 8) : 8;
     const int sms = ctx->spmm_sm_limit > 0 ? std::min(ctx->sm_count, ctx->spmm_sm_limit) : ctx->sm_count;
+    return (int)std::min<long long>((items + 7) / 8, (long long)per_sm * sms);
+}
+
+// the segment pass over the adjacency's segments (their partials into a.seg_part, grown to n_segs x k), then the row pass
+// over `n_rows` rows, each as launch(grid, args)
+template <class Launch>
+int launch_seg_passes(arrow_ctx *ctx, PathArgs p, Adj *adj, long long n_rows, Launch &&launch) {
+    if (n_rows == 0) return ARROW_OK;
     if (std::max<long long>(n_rows, adj->n_segs) * p.used > INT_MAX)
         return fail(ctx, ARROW_ERR_RANGE, "%lld rows x %d words exceed the int32 item count", std::max<long long>(n_rows, adj->n_segs), p.used);
     const size_t part_bytes = (size_t)adj->n_segs * p.k * sizeof(double);
@@ -3454,13 +3463,152 @@ int launch_paths(arrow_ctx *ctx, PathArgs p, Adj *adj, long long n_rows, bool de
         p.rows = pass == 0 ? nullptr : rows;
         p.n_items = (int)((pass == 0 ? adj->n_segs : n_rows) * p.used);
         if (p.n_items == 0) continue;
-        const int grid = (int)std::min<long long>((p.n_items + 7) / 8, (long long)per_sm * sms);
-        if (dependencies) k_bits_dependencies<<<grid, 256, 0, cur_stream(ctx)>>>(p);
-        else k_bits_path_counts<<<grid, 256, 0, cur_stream(ctx)>>>(p);
+        launch(path_grid(ctx, p.n_items), p);
         ctx->launches++;
         CUDA_TRY(ctx, cudaGetLastError());
     }
     return ARROW_OK;
+}
+
+int launch_paths(arrow_ctx *ctx, PathArgs p, Adj *adj, long long n_rows, bool dependencies) {
+    return launch_seg_passes(ctx, p, adj, n_rows, [&](int grid, const PathArgs &q) {
+        if (dependencies) k_bits_dependencies<<<grid, 256, 0, cur_stream(ctx)>>>(q);
+        else k_bits_path_counts<<<grid, 256, 0, cur_stream(ctx)>>>(q);
+    });
+}
+
+// ------------------------------------------------------------------------------------------------
+// Weighted betweenness on min-plus fp32 tiles.  D is the fixed point reached, X0 the features the loop started from, and
+// the lists are the weighted loop-free adjacencies (arrow_adj_build_loopfree): the entries u -> v of M with u != v, each
+// with its weight a.  An entry is tight in column s when D[u, s] < D[v, s] < +inf and fl(a + D[u, s]) == D[v, s]; a pair (u, v)
+// is tight when one of its entries is, and counts once, at its first entry.  A tight pair strictly increases D, so the
+// tight pairs of a column form a DAG, and Kahn rounds over it order every element after its tight predecessors:
+// - the pending pass stores in `state` the number of tight pairs into every finite element (-1 elsewhere), and -2 (depth
+//   0) where there is none; those elements' counts are [v in S] (S: D == X0, finite) and their rows round 0's;
+// - round r sums sigma over the in-lists of its elements (state -(r + 2)), then releases their tight pairs out with an
+//   integer atomic per pair: an element whose counter reaches 0 is at depth r + 1 and its row is listed for round r + 1;
+// - the backward sweep visits the rounds from the deepest to 0 and sums the dependencies along the out-lists.
+// Each element is written by one lane, after every value it reads is final, and the sums run in the bit passes' order
+// (PATH_SEG segments, partials in order): every result depends on D, X0 and the lists alone, never on the schedule.
+// ------------------------------------------------------------------------------------------------
+enum { WP_PENDING, WP_COUNTS, WP_RELEASE, WP_DEPENDENCIES };
+
+struct WPathArgs {
+    PathArgs p;                         // lists, rows, segments, sigma, delta, k, used; p.level is the round
+    const float *__restrict__ wt;       // the lists' weights
+    const float *__restrict__ D;        // the fixed point reached [n x k]
+    const float *__restrict__ x0;       // the features the loop started from [n x k]
+    int *state;                         // [n x k]: -1 not finite, > 0 tight pairs still to release, -(depth + 2)
+    int *mark;                          // [n]: the last round a row was listed for
+    int *next;                          // the rows listed (pending pass: round 0, release pass: round + 1), at *cursor
+    unsigned long long *cursor;
+};
+
+// u -> v (weight a) is tight: D[u] < D[v] < +inf and fl(a + D[u]) == D[v] (no FMA); the finite target keeps a +inf weight
+// or an overflowing sum out of the pairs into an element that is not reached
+__device__ __forceinline__ bool wp_tight(float a, float du, float dv) {
+    return du < dv && dv < __int_as_float(0x7f800000) && __fadd_rn(a, du) == dv;
+}
+
+// lists row v for `round` unless it is already (one lane of the warp)
+__device__ __forceinline__ void wp_list(const WPathArgs &a, int v, int round) {
+    if (atomicExch(a.mark + v, round) != round) a.next[atomicAdd(a.cursor, 1ull)] = v;
+}
+
+// A warp takes one (row, 32-column word), a lane per column, as in the bit passes.  Per batch of 32 list entries lane j
+// loads entry j; the first entries of their pairs are then taken in order, each lane testing its own column (a pair with
+// duplicates is tight when one of them is: its later entries are read then, past the segment's end if need be).
+// PENDING counts the tight pairs in over every row's whole in-list; COUNTS sums sigma over the in-lists of the round's
+// elements and RELEASE decrements the counters along their out-lists; DEPENDENCIES sums fl((1 + delta) / sigma) along the
+// out-lists.  The two sums split lists longer than PATH_SEG at the adjacency's segments, like the bit passes.
+template <int PASS>
+__global__ void __launch_bounds__(256) k_wpaths(WPathArgs a) {
+    constexpr bool IN = PASS == WP_PENDING || PASS == WP_COUNTS;
+    constexpr bool SUM = PASS == WP_COUNTS || PASS == WP_DEPENDENCIES;
+    const int lane = threadIdx.x & 31;
+    const int warps_total = gridDim.x * (blockDim.x >> 5);
+    const int here = -(a.p.level + 2);                        // the state of the round's elements
+    for (int it = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); it < a.p.n_items; it += warps_total) {
+        PathItem t;
+        if (PASS == WP_PENDING) {                             // every row
+            t.v = it / a.p.used;
+            t.w = it - t.v * a.p.used;
+            t.b = t.sb = __ldg(a.p.ptr + t.v);
+            t.e = t.se = __ldg(a.p.ptr + t.v + 1);
+            t.seg = -1;
+        } else {
+            t = path_item(a.p, it);
+        }
+        const int c = t.w * 32 + lane;
+        const long long vc = (long long)t.v * a.p.k + c;
+        const float dv = c < a.p.k ? __ldg(a.D + vc) : 0.0f;
+        const bool mine = c < a.p.k && (PASS == WP_PENDING ? isfinite(dv) : a.state[vc] == here);
+        const bool any = __any_sync(0xffffffffu, mine);
+        if (PASS != WP_PENDING && !any) continue;
+        const bool split = SUM && t.seg < 0 && t.e - t.b > PATH_SEG;
+        double part = 0.0;
+        int pending = 0;
+        if (any && !split) {
+            for (int base = t.sb; base < t.se; base += 32) {
+                const int e = base + lane;
+                int x = 0;
+                float w = 0.0f;
+                bool first = false, dup = false;
+                if (e < t.se) {
+                    x = __ldg(a.p.idx + e);
+                    w = __ldg(a.wt + e);
+                    first = e == t.b || __ldg(a.p.idx + e - 1) != x;
+                    dup = e + 1 < t.e && __ldg(a.p.idx + e + 1) == x;
+                }
+                for (unsigned bal = __ballot_sync(0xffffffffu, first); bal; bal &= bal - 1u) {
+                    const int j = __ffs(bal) - 1;
+                    const int xj = __shfl_sync(0xffffffffu, x, j);
+                    const float wj = __shfl_sync(0xffffffffu, w, j);
+                    const bool dj = __shfl_sync(0xffffffffu, dup, j);
+                    const long long at = (long long)xj * a.p.k + c;
+                    bool tight = false;
+                    if (mine) {
+                        const float dx = __ldg(a.D + at);
+                        const float from = IN ? dx : dv, to = IN ? dv : dx;
+                        tight = wp_tight(wj, from, to);
+                        for (int d = base + j + 1; dj && !tight && d < t.e && __ldg(a.p.idx + d) == xj; ++d)
+                            tight = wp_tight(__ldg(a.wt + d), from, to);
+                    }
+                    if (PASS == WP_PENDING) {
+                        pending += tight;
+                    } else if (PASS == WP_COUNTS) {
+                        if (tight) part += a.p.sigma[at];
+                    } else if (PASS == WP_DEPENDENCIES) {
+                        if (tight) {                                  // a successor without paths adds nothing
+                            const double sw = a.p.sigma[at];
+                            if (sw != 0.0) part += (1.0 + a.p.delta[at]) / sw;
+                        }
+                    } else {
+                        bool ready = false;
+                        if (tight && atomicSub(a.state + at, 1) == 1) {
+                            a.state[at] = here - 1;
+                            ready = true;
+                        }
+                        if (__any_sync(0xffffffffu, ready) && lane == 0) wp_list(a, xj, a.p.level + 1);
+                    }
+                }
+            }
+            if (a.p.scanned && lane == 0) atomicAdd(a.p.scanned, (unsigned long long)(t.se - t.sb));
+        }
+        if (PASS == WP_PENDING) {
+            if (c < a.p.k) {
+                const int s = !mine ? -1 : pending > 0 ? pending : -2;
+                a.state[vc] = s;
+                if (s < 0) a.p.sigma[vc] = s == -2 && dv == __ldg(a.x0 + vc) ? 1.0 : 0.0;
+            }
+            if (__any_sync(0xffffffffu, mine && pending == 0) && lane == 0) wp_list(a, t.v, 0);
+        }
+        if (!SUM || !mine) continue;
+        const double total = split ? seg_total(a.p, t.v, c) : part;
+        if (t.seg >= 0) a.p.seg_part[(long long)t.seg * a.p.k + c] = total;
+        else if (PASS == WP_COUNTS) a.p.sigma[vc] = (dv == __ldg(a.x0 + vc) ? 1.0 : 0.0) + total;
+        else a.p.delta[vc] = dv == __ldg(a.x0 + vc) ? 0.0 : a.p.sigma[vc] * total;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -5227,11 +5375,12 @@ int arrow_bits_mark_new(arrow_ctx *ctx, int new_buf, int old_buf, int dist_buf, 
 }
 
 namespace {
-// arrow_adj_build (weighted false), arrow_adj_build_weighted and arrow_adj_build_in (incoming): one validation, one edge
-// pass, one sort
+// arrow_adj_build (weighted false), arrow_adj_build_weighted, arrow_adj_build_in (incoming) and arrow_adj_build_loopfree
+// (weighted and loop-free, either direction): one validation, one edge pass, one sort
 int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, bool weighted, bool incoming,
-              int *adj_out) {
-    const char *fn = weighted ? "arrow_adj_build_weighted" : incoming ? "arrow_adj_build_in" : "arrow_adj_build";
+              bool loopfree, int *adj_out) {
+    const char *fn = loopfree ? "arrow_adj_build_loopfree" : weighted ? "arrow_adj_build_weighted"
+                                                          : incoming ? "arrow_adj_build_in" : "arrow_adj_build";
     if (!adj_out || n_parts < 0 || (n_parts > 0 && (!csrs || !maps)) || n_vertices < 0)
         return fail(ctx, ARROW_ERR_ARG, "bad arguments (n_parts=%d, n_vertices=%lld)", n_parts, (long long)n_vertices);
     if (n_vertices > 2147483646LL) return fail(ctx, ARROW_ERR_RANGE, "%lld vertices exceed the int32 device layout", (long long)n_vertices);
@@ -5273,7 +5422,9 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
     unsigned long long *count = reinterpret_cast<unsigned long long *>(cnt.p);
     CUDA_TRY(ctx, cudaMemsetAsync(count, 0, sizeof m, s));
     for (const AdjPart &p : parts) {
-        if (weighted) k_adj_edges<true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
+        if (loopfree && incoming) k_adj_edges<true, true, false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
+        else if (loopfree) k_adj_edges<true, false, false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
+        else if (weighted) k_adj_edges<true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
         else if (incoming) k_adj_edges<false, true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
         else k_adj_edges<false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, nullptr);
         ctx->launches++;
@@ -5288,6 +5439,7 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
     a.m = (int64_t)m;
     a.weighted = weighted;
     a.incoming = incoming;
+    a.loopfree = loopfree;
     cudaError_t e = cudaMalloc(&a.indptr, (size_t)(n_vertices + 1) * 4);
     if (e == cudaSuccess) e = cudaMalloc(&a.indices, (size_t)std::max<unsigned long long>(m, 1) * 4);
     if (e == cudaSuccess && weighted) e = cudaMalloc(&a.values, (size_t)std::max<unsigned long long>(m, 1) * 4);
@@ -5306,8 +5458,13 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
             unsigned long long *kp = reinterpret_cast<unsigned long long *>(keys.p);
             for (size_t i = 0; i < parts.size(); ++i) {
                 const AdjPart &p = parts[i];
-                if (weighted)
-                    k_adj_edges<true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp, weights[i], reinterpret_cast<float *>(wk.p));
+                float *w_out = reinterpret_cast<float *>(wk.p);
+                if (loopfree && incoming)
+                    k_adj_edges<true, true, false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp, weights[i], w_out);
+                else if (loopfree)
+                    k_adj_edges<true, false, false><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp, weights[i], w_out);
+                else if (weighted)
+                    k_adj_edges<true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp, weights[i], w_out);
                 else if (incoming)
                     k_adj_edges<false, true><<<edge_grid(p.nnz), 256, 0, s>>>(p, count, kp);
                 else
@@ -5341,7 +5498,7 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e == cudaSuccess && incoming) e = build_segs(a);       // the segments of the long in-lists
+    if (e == cudaSuccess && (incoming || loopfree)) e = build_segs(a);   // the segments of the long lists
     if (e != cudaSuccess) {
         cudaGetLastError();
         adj_release(a);
@@ -5359,20 +5516,27 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
 int arrow_adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out) {
     CHECK_CTX(ctx);
     CHECK_POISON(ctx);
-    return adj_build(ctx, n_parts, csrs, maps, n_vertices, false, false, adj_out);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, false, false, false, adj_out);
 }
 
 int arrow_adj_build_in(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int *adj_out) {
     CHECK_CTX(ctx);
     CHECK_POISON(ctx);
-    return adj_build(ctx, n_parts, csrs, maps, n_vertices, false, true, adj_out);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, false, true, false, adj_out);
 }
 
 int arrow_adj_build_weighted(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices,
                              int *adj_out) {
     CHECK_CTX(ctx);
     CHECK_POISON(ctx);
-    return adj_build(ctx, n_parts, csrs, maps, n_vertices, true, false, adj_out);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, true, false, false, adj_out);
+}
+
+int arrow_adj_build_loopfree(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int incoming,
+                             int *adj_out) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    return adj_build(ctx, n_parts, csrs, maps, n_vertices, true, incoming != 0, true, adj_out);
 }
 
 int arrow_adj_values_d2h(arrow_ctx *ctx, int adj, float *values) {
@@ -5559,6 +5723,25 @@ int arrow_bits_parents(arrow_ctx *ctx, int in_adj, int adj, int new_buf, int old
 }
 
 namespace {
+// grows the adjacency's history to hold `need` rows, keeping the rows it holds (stream-ordered); it doubles, from 1024
+int hist_reserve(arrow_ctx *ctx, Adj *a, int64_t need) {
+    if (need <= a->hist_cap) return ARROW_OK;
+    const int64_t at = a->hist_off.empty() ? 0 : a->hist_off.back();
+    const int64_t cap = std::max<int64_t>({need, 2 * a->hist_cap, 1024});
+    int *grown = nullptr;
+    CUDA_TRY(ctx, cudaMalloc(&grown, (size_t)cap * 4));
+    if (at > 0) {
+        const cudaError_t e = cudaMemcpyAsync(grown, a->hist, (size_t)at * 4, cudaMemcpyDeviceToDevice, cur_stream(ctx));
+        if (e != cudaSuccess) {
+            cudaFree(grown);
+            return fail(ctx, ARROW_ERR_CUDA, "history copy: %s", cudaGetErrorString(e));
+        }
+    }
+    cudaFree(a->hist);                                        // waits for the copy
+    a->hist = grown;
+    a->hist_cap = cap;
+    return ARROW_OK;
+}
 // reads back the optional edge counter of a path-count / dependency pass (synchronises)
 int read_scanned(arrow_ctx *ctx, const DevTmp &cnt, int64_t *edges_scanned) {
     if (!edges_scanned) return ARROW_OK;
@@ -5630,24 +5813,11 @@ int arrow_adj_keep_record(arrow_ctx *ctx, int adj, int level) {
         return fail(ctx, ARROW_ERR_ARG, "level %d: the history holds levels 0..%d, the next one kept is %d (or 0 to restart)", level,
                     kept - 1, kept);
     if (level == 0) a->hist_off.assign(1, 0);
+    a->wp_tag_p = nullptr;                                    // the history no longer holds arrow_wpaths_counts' rounds
     const int64_t at = a->hist_off.back(), need = at + a->n_front;
-    cudaStream_t s = cur_stream(ctx);
-    if (need > a->hist_cap) {
-        const int64_t cap = std::max<int64_t>({need, 2 * a->hist_cap, 1024});
-        int *grown = nullptr;
-        CUDA_TRY(ctx, cudaMalloc(&grown, (size_t)cap * 4));
-        if (at > 0) {
-            const cudaError_t e = cudaMemcpyAsync(grown, a->hist, (size_t)at * 4, cudaMemcpyDeviceToDevice, s);
-            if (e != cudaSuccess) {
-                cudaFree(grown);
-                return fail(ctx, ARROW_ERR_CUDA, "history copy: %s", cudaGetErrorString(e));
-            }
-        }
-        cudaFree(a->hist);                                    // waits for the copy
-        a->hist = grown;
-        a->hist_cap = cap;
-    }
-    if (a->n_front > 0) CUDA_TRY(ctx, cudaMemcpyAsync(a->hist + at, a->front_rows, (size_t)a->n_front * 4, cudaMemcpyDeviceToDevice, s));
+    if (const int rc = hist_reserve(ctx, a, need)) return rc;
+    if (a->n_front > 0)
+        CUDA_TRY(ctx, cudaMemcpyAsync(a->hist + at, a->front_rows, (size_t)a->n_front * 4, cudaMemcpyDeviceToDevice, cur_stream(ctx)));
     a->hist_off.push_back(need);
     return ARROW_OK;
 }
@@ -5728,6 +5898,165 @@ int arrow_dense_row_sum(arrow_ctx *ctx, int in_buf, int out_buf) {
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     return ARROW_OK;
+}
+
+namespace {
+// the tiles of the weighted path calls: x0 / dist float32, state int32, sigma (and delta) float64, all n x k; k >= 1
+int wpaths_tiles(arrow_ctx *ctx, const Adj *a, int x0_buf, int dist_buf, int state_buf, int sigma_buf, int delta_buf,
+                 DenseBuf *t[5]) {
+    const int h[5] = {x0_buf, dist_buf, state_buf, sigma_buf, delta_buf};
+    const int want[5] = {ARROW_F32, ARROW_F32, ARROW_I32, ARROW_F64, ARROW_F64};
+    const char *name[5] = {"x0", "dist", "state", "sigma", "delta"};
+    const int n_tiles = delta_buf < 0 ? 4 : 5;
+    for (int i = 0; i < n_tiles; ++i) {
+        t[i] = get_dense(ctx, h[i]);
+        if (!t[i]) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle %s=%d", name[i], h[i]);
+        if (t[i]->dtype != want[i])
+            return fail(ctx, ARROW_ERR_ARG, "%s is a %s tile, expected %s", name[i], dtype_name(t[i]->dtype), dtype_name(want[i]));
+        if (t[i]->rows != a->n || t[i]->k != t[0]->k)
+            return fail(ctx, ARROW_ERR_ARG, "shape: %s %lld x %d, x0 %lld x %d, adjacency %lld rows", name[i], (long long)t[i]->rows,
+                        t[i]->k, (long long)t[0]->rows, t[0]->k, (long long)a->n);
+        for (int j = 0; j < i; ++j)
+            if (h[j] == h[i] || t[j]->p == t[i]->p) return fail(ctx, ARROW_ERR_ARG, "%s aliases %s", name[i], name[j]);
+    }
+    if (t[0]->k > BITS_MAX_K) return fail(ctx, ARROW_ERR_UNSUPPORTED, "k=%d > %d", t[0]->k, BITS_MAX_K);
+    if (a->n * (long long)((t[0]->k + 31) / 32) > INT_MAX)
+        return fail(ctx, ARROW_ERR_RANGE, "%lld rows x %d words exceed the int32 item count", (long long)a->n, (t[0]->k + 31) / 32);
+    return ARROW_OK;
+}
+
+WPathArgs wpaths_args(DenseBuf *const t[5], const Adj *lists) {
+    WPathArgs w{};
+    w.p.ptr = lists->indptr;
+    w.p.idx = lists->indices;
+    w.wt = lists->values;
+    w.D = t[1]->p;
+    w.x0 = t[0]->p;
+    w.state = reinterpret_cast<int *>(t[2]->p);
+    w.p.sigma = reinterpret_cast<double *>(t[3]->p);
+    w.p.k = t[0]->k;
+    w.p.used = (t[0]->k + 31) / 32;
+    return w;
+}
+}  // namespace
+
+int arrow_wpaths_counts(arrow_ctx *ctx, int in_adj, int out_adj, int x0_buf, int dist_buf, int state_buf, int sigma_buf,
+                        int64_t *rounds, int64_t *entries_read) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    Adj *in = get_adj(ctx, in_adj), *out = get_adj(ctx, out_adj);
+    if (!in || !out) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle (in=%d out=%d)", in_adj, out_adj);
+    if (!in->loopfree || !in->incoming || !out->loopfree || out->incoming)
+        return fail(ctx, ARROW_ERR_ARG, "in_adj / out_adj are the loop-free in- and out-adjacencies (arrow_adj_build_loopfree)");
+    if (in->n != out->n)
+        return fail(ctx, ARROW_ERR_ARG, "the adjacencies differ in vertices: in %lld, out %lld", (long long)in->n, (long long)out->n);
+    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_wpaths_counts synchronises: not during graph capture");
+    DenseBuf *t[5];
+    if (const int rc = wpaths_tiles(ctx, out, x0_buf, dist_buf, state_buf, sigma_buf, -1, t)) return rc;
+    cudaStream_t s = cur_stream(ctx);
+    out->wp_tag_p = nullptr;
+    out->hist_off.assign(1, 0);
+    if (rounds) *rounds = 0;
+    if (entries_read) *entries_read = 0;
+    const int64_t n = out->n;
+    if (n == 0 || t[0]->k == 0) {
+        out->wp_tag_p = t[2]->p;
+        out->wp_tag_k = t[2]->k;
+        return ARROW_OK;
+    }
+    DevTmp mark, cnt;                                         // the rows' last round; {cursor, entries read}
+    CUDA_TRY(ctx, cudaMalloc(&mark.p, (size_t)n * 4));
+    CUDA_TRY(ctx, cudaMalloc(&cnt.p, 2 * sizeof(unsigned long long)));
+    CUDA_TRY(ctx, cudaMemsetAsync(mark.p, 0xff, (size_t)n * 4, s));
+    CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, 2 * sizeof(unsigned long long), s));
+    unsigned long long *cursor = reinterpret_cast<unsigned long long *>(cnt.p);
+    WPathArgs w = wpaths_args(t, in);
+    w.mark = reinterpret_cast<int *>(mark.p);
+    w.cursor = cursor;
+    w.p.scanned = entries_read ? cursor + 1 : nullptr;
+    // runs a pass over `items` items, rows from history offset rows_at, that lists at most n rows at the end of the
+    // history, and keeps them as the next round (synchronises)
+    auto list_round = [&](auto kernel, int items, int64_t rows_at) -> int {
+        const int64_t at = out->hist_off.back();
+        if (const int rc = hist_reserve(ctx, out, at + n)) return rc;
+        w.p.rows = out->hist + rows_at;
+        w.next = out->hist + at;
+        w.p.n_items = items;
+        CUDA_TRY(ctx, cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s));
+        kernel<<<path_grid(ctx, items), 256, 0, s>>>(w);
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+        unsigned long long listed = 0;
+        CUDA_TRY(ctx, cudaMemcpyAsync(&listed, cursor, sizeof listed, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaStreamSynchronize(s));
+        out->hist_off.push_back(at + (int64_t)listed);
+        return ARROW_OK;
+    };
+    w.p.level = 0;
+    if (const int rc = list_round(k_wpaths<WP_PENDING>, (int)(n * w.p.used), 0)) return rc;
+    for (int r = 0; out->hist_off[r + 1] > out->hist_off[r]; ++r) {
+        const long long n_rows = out->hist_off[r + 1] - out->hist_off[r];
+        w.p.level = r;
+        w.p.rows = out->hist + out->hist_off[r];
+        if (r > 0) {                                          // round 0's counts are the pending pass's
+            WPathArgs c = w;
+            c.p.ptr = in->indptr;
+            c.p.idx = in->indices;
+            c.wt = in->values;
+            const int rc = launch_seg_passes(ctx, c.p, in, n_rows, [&](int grid, const PathArgs &q) {
+                c.p = q;
+                k_wpaths<WP_COUNTS><<<grid, 256, 0, s>>>(c);
+            });
+            if (rc) return rc;
+        }
+        w.p.ptr = out->indptr;
+        w.p.idx = out->indices;
+        w.wt = out->values;
+        if (const int rc = list_round(k_wpaths<WP_RELEASE>, (int)(n_rows * w.p.used), out->hist_off[r])) return rc;
+    }
+    out->hist_off.pop_back();                                 // the empty round that ended the loop
+    out->wp_tag_p = t[2]->p;
+    out->wp_tag_k = t[2]->k;
+    if (rounds) *rounds = (int64_t)out->hist_off.size() - 1;
+    if (entries_read) {
+        unsigned long long h = 0;
+        CUDA_TRY(ctx, cudaMemcpyAsync(&h, cursor + 1, sizeof h, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(ctx, cudaStreamSynchronize(s));
+        *entries_read = (int64_t)h;
+    }
+    return ARROW_OK;
+}
+
+int arrow_wpaths_dependencies(arrow_ctx *ctx, int out_adj, int x0_buf, int dist_buf, int state_buf, int sigma_buf, int delta_buf,
+                              int64_t *entries_read) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    Adj *out = get_adj(ctx, out_adj);
+    if (!out) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", out_adj);
+    if (!out->loopfree || out->incoming)
+        return fail(ctx, ARROW_ERR_ARG, "out_adj is the loop-free out-adjacency (arrow_adj_build_loopfree)");
+    DenseBuf *t[5];
+    if (const int rc = wpaths_tiles(ctx, out, x0_buf, dist_buf, state_buf, sigma_buf, delta_buf, t)) return rc;
+    if (!out->wp_tag_p || out->wp_tag_p != t[2]->p || out->wp_tag_k != t[2]->k)
+        return fail(ctx, ARROW_ERR_ARG, "the adjacency holds no rounds of arrow_wpaths_counts for state tile %d", state_buf);
+    PathArgs scan{};
+    DevTmp cnt;
+    if (const int rc = alloc_scanned(ctx, cnt, entries_read, scan)) return rc;
+    WPathArgs w = wpaths_args(t, out);
+    w.p.delta = reinterpret_cast<double *>(t[4]->p);
+    w.p.scanned = scan.scanned;
+    cudaStream_t s = cur_stream(ctx);
+    for (int r = (int)out->hist_off.size() - 2; r >= 0; --r) {
+        w.p.level = r;
+        w.p.rows = out->hist + out->hist_off[r];
+        const int rc = launch_seg_passes(ctx, w.p, out, out->hist_off[r + 1] - out->hist_off[r], [&](int grid, const PathArgs &q) {
+            WPathArgs d = w;
+            d.p = q;
+            k_wpaths<WP_DEPENDENCIES><<<grid, 256, 0, s>>>(d);
+        });
+        if (rc) return rc;
+    }
+    return read_scanned(ctx, cnt, entries_read);
 }
 
 int arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int64_t *rows_changed, int64_t *frontier_rows,

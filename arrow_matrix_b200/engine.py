@@ -88,6 +88,25 @@ def semiring_code(semiring: str, dtype, fused_style: str = "gather") -> int:
     return code
 
 
+_SCAN_CHUNK = 1 << 24      # entries per chunk of the weight scan: bounds its host memory
+
+
+def _nonpositive_edge(ip, idx, dat, cmap) -> bool:
+    """some entry (r, c) of a level is an edge of the operator -- r != c (u != v: the row maps are injective) and both
+    ends map to level-0 rows (``cmap``, -1 where not) -- whose weight is not > 0 (0, -0, negative or NaN).  Only the
+    entries that are not > 0 get their row; the scan runs in chunks."""
+    ip, idx, dat = np.asarray(ip), np.asarray(idx), np.asarray(dat)
+    for e0 in range(0, dat.size, _SCAN_CHUNK):
+        e = np.flatnonzero(~(dat[e0:e0 + _SCAN_CHUNK] > 0)) + e0
+        if e.size == 0:
+            continue
+        r, c = np.searchsorted(ip, e, side="right") - 1, idx[e].astype(np.int64)
+        ok = (r != c) & (c >= 0)
+        if np.any(ok & (cmap[r] >= 0) & (cmap[np.where(ok, c, 0)] >= 0)):
+            return True
+    return False
+
+
 class _LevelState:
     __slots__ = ("rows", "n_blocks", "csr", "csr_fused", "to_prev", "to_next_dev", "to_prev_dev", "cmap_dev",
                  "bufs", "xi", "ci", "nnz", "dropped", "cbuf")
@@ -143,6 +162,11 @@ class ArrowEngine:
         self.last_fixed_point_directions: List[str] = []         # "push" / "pull" per step of iterate_to_fixed_point()
         self._sr_adj: Optional[_lib.Adjacency] = None            # iterate_to_fixed_point(): weighted push adjacency
         self._neg_zero_weight = False                            # a -0 entry in some level: the tropical push is not exact
+        self._nonpos_weight = False                              # an edge of weight not > 0: no weighted betweenness
+        self._wp_adjs: Optional[Tuple[_lib.Adjacency, ...]] = None   # weighted betweenness: loop-free (in, out) lists
+        self._wp_tiles: Optional[Tuple[_lib.Dense, ...]] = None      # weighted betweenness: X0, state, sigma tiles
+        self._wp_delta: Optional[Tuple[_lib.Dense, ...]] = None      # weighted_betweenness(): delta and [n x 1] bc
+        self.last_path_rounds = 0                                # tight-DAG rounds of the last weighted path call
         fused_ok = True
         cmap_prev = None                      # level j-1 row -> level-0 row (host, int64, -1 invalid)
         for j, (B, _) in enumerate(decomposition):
@@ -151,6 +175,7 @@ class ArrowEngine:
             st.rows = st.n_blocks * width
             ip, idx, dat, dropped = decomp.arrow_rows(B, width, st.n_blocks, block_diagonal, 0, st.rows, dtype=self.dtype)
             st.dropped = dropped
+            entries = (ip, idx, dat)              # the level's own entries, before the identity diagonal
             if j == 0 and self.add_identity:
                 ip, idx, dat = decomp.with_diagonal(ip, idx, dat, st.rows, _TIMES_ONE[self.sr], self.dtype)
             st.nnz = int(ip[-1])
@@ -176,6 +201,8 @@ class ArrowEngine:
                 st.cmap_dev = self.ctx.map_upload(cmap, self.levels[0].rows)
             else:
                 cmap_prev = np.arange(st.rows, dtype=np.int64)
+            if self.sr == _lib.SR_MIN_PLUS and _nonpositive_edge(*entries, cmap_prev):
+                self._nonpos_weight = True
             self.levels.append(st)
         if mode == "fused" and not fused_ok:
             raise ValueError("fused mode requested but a level reads rows behind the sentinel; use mode='exchange'")
@@ -611,11 +638,7 @@ class ArrowEngine:
         tile) is allocated on the first call and kept until ``close()``.  Raises ``ValueError`` before any CUDA work where
         ``bfs_tree`` does.  Synchronises."""
         self._paths_checks("betweenness")
-        n = self.levels[0].rows
-        for name, arr, shape in (("out", out, (n,)), ("dependencies_out", dependencies_out, (n, self.k))):
-            if arr is not None and (arr.dtype != np.float64 or arr.shape != shape or not arr.flags.c_contiguous):
-                raise ValueError(f"{name} must be a C-contiguous float64 array of shape {shape}, got {arr.dtype} "
-                                 f"{arr.shape}{'' if arr.flags.c_contiguous else ' (not contiguous)'}")
+        self._check_bc_outputs(out, dependencies_out)
         delta, bc = self._betweenness_run(max_steps)
         if dependencies_out is not None:
             delta.d2h(dependencies_out)
@@ -647,6 +670,110 @@ class ArrowEngine:
         if self._bfs_sigma is None:
             self._bfs_sigma = self.ctx.dense_alloc(self.levels[0].rows, self.k, np.float64)
         return self._bfs_run(max_steps, sigma=self._bfs_sigma), self._bfs_sigma
+
+    # -- weighted betweenness (min_plus) ---------------------------------------------------------------------------
+    def shortest_path_counts(self, max_steps: int, distances_out: Optional[np.ndarray] = None,
+                             counts_out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """``iterate_to_fixed_point(max_steps)`` that also returns the number of shortest paths to every element (``D``
+        float32 and ``sigma`` float64, both [n x k] in level-0 row order like ``result()``).  An entry ``u -> v`` of weight
+        ``a`` of the fused step's operator (``u != v``) is *tight* in column ``s`` when ``D[u, s] < D[v, s] < +inf`` and
+        ``fl(a + D[u, s]) == D[v, s]`` (so a ``+inf`` weight or an overflowing sum never counts); a pair ``(u, v)`` is tight when one of its entries is.  The sources ``S_s`` are the
+        ``v`` with ``D[v, s]`` finite and equal to the features the call started from (the 0 / +inf start, or any offsets:
+        a column with several sources acts as one super-source).  ``sigma[v, s]`` is 0 where ``D[v, s]`` is not finite,
+        otherwise ``[v in S_s]`` plus the sum of ``sigma[u, s]`` over the distinct tight pairs ``u -> v``, in ascending
+        ``u``, 512 in-list entries at a time, the partials added in order (DESIGN.md §4): exact below 2^53 and
+        bit-reproducible beyond.  On unit weights from 0 / +inf features this is ``bfs_path_counts`` bit for bit.  When
+        ``max_steps`` stops the loop before the fixed point, everything is defined on the ``D`` reached.  The step count
+        and ``last_fixed_point_directions`` are those of ``iterate_to_fixed_point``, the features end at ``D``, and
+        ``last_path_rounds`` holds the rounds of the tight-pair DAG.
+
+        The loop-free weighted in- and out-adjacencies (8 bytes per edge each) and the tiles (the starting features 4,
+        the round state 4 and the counts 8 bytes per element: 20.5 GB at 10M rows and k = 128, beside the two 5.1 GB
+        feature tiles) are made on the first call and kept until ``close()``.  Needs ``min_plus`` with ``add_identity``,
+        a level-0 row behind every non-zero and every edge's weight ``> 0`` (an edge: an off-diagonal entry with both
+        ends routed; ``+inf`` is allowed); raises ``ValueError`` before any CUDA work otherwise.  Synchronises."""
+        D, sigma = self._wpaths_run(max_steps, "shortest_path_counts")
+        return D.d2h(distances_out), sigma.d2h(counts_out)
+
+    def weighted_betweenness(self, max_steps: int, out: Optional[np.ndarray] = None,
+                             dependencies_out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Brandes betweenness over the weighted shortest paths from the engine's ``k`` source columns: float64
+        ``bc[v] = sum over s < k of delta[v, s]`` in level-0 row order, summed in column order.  ``delta[v, s]`` is 0
+        where ``D[v, s]`` is not finite and for ``v`` in ``S_s``, otherwise ``sigma[v, s]`` (``shortest_path_counts``)
+        times the sum of ``fl((1 + delta[w, s]) / sigma[w, s])`` over the distinct tight pairs ``v -> w`` with
+        ``sigma[w, s] != 0``, summed in ascending ``w`` like the counts.  (A finite element outside ``S_s`` with no tight
+        predecessor has no paths, ``sigma = 0``: a loop cut short by ``max_steps`` can leave such elements, and their
+        successors add nothing, so every dependency stays finite.)  With one source per column this is the unnormalised weighted betweenness
+        restricted to those sources, counting ordered pairs; on unit weights it is ``betweenness`` bit for bit.
+        ``dependencies_out`` (float64 [n x k]) receives ``delta``.  The loop, features and ``last_path_rounds`` are those
+        of ``shortest_path_counts``.
+
+        The backward sweep visits the rounds of the tight-pair DAG from the deepest to 0 along the out-lists; the
+        round rows take 4 bytes per row and round in which the row has an element.  The dependency tile (8 bytes per
+        element) is allocated on the first call and kept until ``close()``.  Raises ``ValueError`` before any CUDA work
+        where ``shortest_path_counts`` does, and for an ``out`` or ``dependencies_out`` that is not a C-contiguous float64
+        array of the right shape.  Synchronises."""
+        self._wpaths_checks("weighted_betweenness")
+        self._check_bc_outputs(out, dependencies_out)
+        delta, bc = self._wbc_run(max_steps)
+        if dependencies_out is not None:
+            delta.d2h(dependencies_out)
+        if out is None:
+            return bc.d2h().reshape(-1)
+        bc.d2h(out[:, None])
+        return out
+
+    def _wbc_run(self, max_steps: int) -> Tuple[_lib.Dense, _lib.Dense]:
+        """the device part of ``weighted_betweenness``: the float64 dependency and [n x 1] betweenness tiles"""
+        D, sigma = self._wpaths_run(max_steps, "weighted_betweenness")
+        if self._wp_delta is None:
+            n = self.levels[0].rows
+            self._wp_delta = (self.ctx.dense_alloc(n, self.k, np.float64), self.ctx.dense_alloc(n, 1, np.float64))
+        delta, bc = self._wp_delta
+        x0, state, _ = self._wp_tiles
+        delta.fill(0.0)
+        self.ctx.wpaths_dependencies(self._wp_adjs[1], x0, D, state, sigma, delta)
+        self.ctx.row_sum(delta, bc)
+        return delta, bc
+
+    def _wpaths_run(self, max_steps: int, what: str) -> Tuple[_lib.Dense, _lib.Dense]:
+        """the device part of ``shortest_path_counts``: the fixed point (the level-0 features tile) and the float64 count
+        tile, with the rounds kept in the loop-free out-adjacency's history"""
+        self._wpaths_checks(what)
+        self.sync()
+        st0 = self.levels[0]
+        if self._wp_adjs is None:
+            parts = [(st.csr, st.cmap_dev) for st in self.levels]
+            self._wp_adjs = (self.ctx.adj_build_loopfree(parts, st0.rows, direction="in"),
+                             self.ctx.adj_build_loopfree(parts, st0.rows))
+        if self._wp_tiles is None:
+            self._wp_tiles = (self.ctx.dense_alloc(st0.rows, self.k), self.ctx.dense_alloc(st0.rows, self.k, np.int32),
+                              self.ctx.dense_alloc(st0.rows, self.k, np.float64))
+        x0, state, sigma = self._wp_tiles
+        x0.copy_from(st0.bufs[st0.xi])          # the loop overwrites both level-0 tiles
+        self.iterate_to_fixed_point(max_steps)
+        D = st0.bufs[st0.xi]
+        self.last_path_rounds, _ = self.ctx.wpaths_counts(self._wp_adjs[0], self._wp_adjs[1], x0, D, state, sigma)
+        return D, sigma
+
+    def _wpaths_checks(self, what: str):
+        if self.sr != _lib.SR_MIN_PLUS:
+            raise ValueError(f"{what} runs the min_plus semiring, the engine runs {self.semiring}")
+        if not self.add_identity:
+            raise ValueError(f"{what} needs add_identity=True: a step must keep the distances it already has")
+        if not self.fused_ok:
+            raise ValueError(f"{what} needs a level-0 row behind every non-zero, but a level reads rows behind the "
+                             "sentinel")
+        if self._nonpos_weight:
+            raise ValueError(f"{what} needs every off-diagonal weight > 0: a zero, negative or NaN weight lets ties "
+                             "close cycles of tight pairs")
+
+    def _check_bc_outputs(self, out: Optional[np.ndarray], dependencies_out: Optional[np.ndarray]):
+        n = self.levels[0].rows
+        for name, arr, shape in (("out", out, (n,)), ("dependencies_out", dependencies_out, (n, self.k))):
+            if arr is not None and (arr.dtype != np.float64 or arr.shape != shape or not arr.flags.c_contiguous):
+                raise ValueError(f"{name} must be a C-contiguous float64 array of shape {shape}, got {arr.dtype} "
+                                 f"{arr.shape}{'' if arr.flags.c_contiguous else ' (not contiguous)'}")
 
     def _paths_checks(self, what: str):
         self._bfs_checks(what)
@@ -845,8 +972,10 @@ class ArrowEngine:
             if a is not None:
                 a.free()
         self._wit_labels, self._wit_values, self._bfs_tiles, self._adj, self._sr_adj = None, {}, None, None, None
-        for b in (self._bfs_sigma,) + (self._bfs_delta or ()):
+        for b in (self._bfs_sigma,) + (self._bfs_delta or ()) + (self._wp_adjs or ()) + (self._wp_tiles or ()) + \
+                (self._wp_delta or ()):
             if b is not None:
                 b.free()
         self._in_adj = self._bfs_parents = self._bfs_sigma = self._bfs_delta = None
+        self._wp_adjs = self._wp_tiles = self._wp_delta = None
         self.ctx.close()

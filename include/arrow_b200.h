@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 11
+#define ARROW_ABI_VERSION 12
 
 /* error codes */
 #define ARROW_OK              0
@@ -348,6 +348,40 @@ int  arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, i
  * other than the adjacency's, out of another shape or k, an unknown semiring code; ARROW_ERR_UNSUPPORTED: PLUS_TIMES,
  * OR_AND. */
 int  arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int semiring);
+
+/* ---- weighted betweenness (one GPU, min-plus on fp32 tiles): shortest-path counts and Brandes dependencies ------------- */
+/* The weighted adjacency of M without the edges u == v: the lists of arrow_adj_build (incoming == 0) or arrow_adj_build_in
+ * (incoming != 0), in the same order, each entry carrying its fp32 weight (duplicates of (u, v) in any order).  Lists
+ * longer than 512 entries are also listed as 512-entry segments.  The out-adjacency gets the frontier record of
+ * arrow_adj_build_weighted and serves every call that takes a weighted push adjacency (as one without self-loops).
+ * Memory and refusals: those of arrow_adj_build_weighted.  Synchronises. */
+int  arrow_adj_build_loopfree(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int incoming,
+                              int *adj_out);
+/* Shortest-path counts over the tight pairs of a min-plus fixed point.  dist (D) and x0 (X0, the features the fixed-point
+ * loop started from) are fp32, state int32 and sigma float64 tiles, all [n x k] with n the adjacencies' vertices.  An
+ * entry u -> v of weight a is tight in column s when D[u, s] < D[v, s] < +inf and fl(a + D[u, s]) == D[v, s] (a +inf
+ * weight or an overflowing sum never reaches an element that is not reached); the pair (u, v) is tight when one of its
+ * entries is.  S_s = {v : D[v, s] finite and D[v, s] == X0[v, s]}.  sigma[v, s] = 0 where D[v, s]
+ * is not finite, else [v in S_s] + the sum of sigma[u, s] over the distinct tight pairs u -> v, summed over v's in-list in
+ * ascending order, 512 entries at a time, the partials added in order (no floating-point atomics).  The tight pairs form
+ * a DAG per column: state receives -1 where D is not finite, else -(depth + 2), the depth being the round of Kahn's
+ * algorithm that finalised the element; the rows of each round are kept in out_adj's history (4 bytes per row and round
+ * with an element at that depth; the buffer doubles and holds up to twice that, plus 4 n bytes).  *rounds (may be NULL)
+ * receives the rounds, *entries_read (may be NULL) the list entries read, once per row and 32-column word taking part in
+ * a pass.  Temporary device memory of 4 n bytes.  ARROW_ERR_ARG: adjacencies that are not the loop-free in- and
+ * out-adjacency of the same vertices, other tile types or shapes, two tiles aliasing; ARROW_ERR_UNSUPPORTED: k > 8192,
+ * graph capture.  Synchronises after every round. */
+int  arrow_wpaths_counts(arrow_ctx *ctx, int in_adj, int out_adj, int x0_buf, int dist_buf, int state_buf, int sigma_buf,
+                         int64_t *rounds, int64_t *entries_read);
+/* Dependencies over the rounds kept by the last arrow_wpaths_counts on out_adj with this state tile, from the deepest to
+ * round 0: delta[v, s] = 0 for v in S_s, else sigma[v, s] * the sum of fl((1 + delta[w, s]) / sigma[w, s]) over the
+ * distinct tight pairs v -> w with sigma[w, s] != 0 (a successor without paths, which a loop cut short by max_steps can
+ * leave, adds nothing), summed like the counts over v's out-list, for every element with a finite D; the other
+ * elements of delta are left alone.  The tiles are those of arrow_wpaths_counts, unchanged since, and delta a float64 tile
+ * of their shape.  *entries_read (may be NULL; then the call does not synchronise) receives the out-list entries read.
+ * ARROW_ERR_ARG: those of arrow_wpaths_counts, and no rounds of it kept for the state tile. */
+int  arrow_wpaths_dependencies(arrow_ctx *ctx, int out_adj, int x0_buf, int dist_buf, int state_buf, int sigma_buf, int delta_buf,
+                               int64_t *entries_read);
 
 /* ---- predecessors of the tropical semirings (one GPU, fp32) ------------------------------------------ */
 /* The product of arrow_spmm_sr over (value, label) pairs.  A candidate of row r is an entry p whose column c is valid
