@@ -26,7 +26,9 @@ _TILE_CODE = {**_DTYPE_CODE, np.dtype(np.int32): I32}
 _CODE_TILE = {**{c: dt for dt, c in _TILE_CODE.items()}, B1: BITS}
 VARIANT_AUTO, VARIANT_DIRECT, VARIANT_SHFL, VARIANT_TMA, VARIANT_TILES = -1, 0, 1, 2, 3
 SR_PLUS_TIMES, SR_MIN_PLUS, SR_MAX_PLUS, SR_OR_AND = 0, 1, 2, 3   # ARROW_SR_*: the semiring of arrow_spmm_sr / arrow_gather_rows_sr
-SEMIRINGS = {"plus_times": SR_PLUS_TIMES, "min_plus": SR_MIN_PLUS, "max_plus": SR_MAX_PLUS, "or_and": SR_OR_AND}
+SR_MAX_MIN, SR_MIN_MAX = 4, 5                                       # the bottleneck semirings: widest / minimax paths
+SEMIRINGS = {"plus_times": SR_PLUS_TIMES, "min_plus": SR_MIN_PLUS, "max_plus": SR_MAX_PLUS, "or_and": SR_OR_AND,
+             "max_min": SR_MAX_MIN, "min_max": SR_MIN_MAX}
 IPC_HANDLE_BYTES = 80
 
 EXPORTS = [
@@ -52,8 +54,9 @@ EXPORTS = [
     "arrow_sr_push_frontier", "arrow_adj_build_in", "arrow_bits_parents", "arrow_bits_path_counts",
     "arrow_adj_keep_record", "arrow_bits_dependencies", "arrow_bits_fill_f64", "arrow_dense_row_sum",
     "arrow_adj_build_loopfree", "arrow_wpaths_counts", "arrow_wpaths_dependencies",
+    "arrow_sr_mark_frontier_steps", "arrow_sr_tree_parents", "arrow_dense_count_diff_bits",
 ]
-ABI_VERSION = 12       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 13       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -175,6 +178,9 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_adj_build_loopfree": (c_int, [P, I, pI, pI, I64, I, pI]),
         "arrow_wpaths_counts": (c_int, [P, I, I, I, I, I, I, pI64, pI64]),
         "arrow_wpaths_dependencies": (c_int, [P, I, I, I, I, I, I, pI64]),
+        "arrow_sr_mark_frontier_steps": (c_int, [P, I, I, I, I, I, pI64, pI64, pI64]),
+        "arrow_sr_tree_parents": (c_int, [P, I, I, I, I, I, pI64]),
+        "arrow_dense_count_diff_bits": (c_int, [P, I, I, pI64]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -605,15 +611,41 @@ class Context:
         return int(n.value), int(rows.value), int(edges.value)
 
     def sr_push_frontier(self, adj: "Adjacency", x: "Dense", out: "Dense", semiring: int):
-        """out = canon(x), then out[v] ⊕= fl(a + x[u]) along the weighted adjacency's edges of the recorded frontier rows u
-        (``arrow_sr_push_frontier``, ``semiring`` SR_MIN_PLUS or SR_MAX_PLUS); ``x`` must be the tile of the last
-        ``sr_mark_frontier`` on ``adj``"""
+        """out = canon(x), then out[v] ⊕= a ⊗ x[u] along the weighted adjacency's edges of the recorded frontier rows u
+        (``arrow_sr_push_frontier``, ``semiring`` SR_MIN_PLUS, SR_MAX_PLUS, SR_MAX_MIN or SR_MIN_MAX); ``x`` must be the
+        tile of the last ``sr_mark_frontier`` on ``adj``"""
         self._check(self.lib.arrow_sr_push_frontier(self._h, adj.h, x.h, out.h, int(semiring)))
+
+    def sr_mark_frontier_steps(self, adj: "Adjacency", new: "Dense", old: "Dense", steps: "Dense", level: int):
+        """``sr_mark_frontier``, and in the same pass steps[r, c] = ``level`` where ``new`` and ``old`` differ in bits
+        (level 0: 0 everywhere) in the int32 tile ``steps`` (``arrow_sr_mark_frontier_steps``); synchronises"""
+        n, rows, edges = c_int64(), c_int64(), c_int64()
+        self._check(self.lib.arrow_sr_mark_frontier_steps(self._h, adj.h, new.h, old.h, steps.h, int(level), byref(n),
+                                                          byref(rows), byref(edges)))
+        return int(n.value), int(rows.value), int(edges.value)
+
+    def sr_tree_parents(self, in_adj: "Adjacency", dist: "Dense", steps: "Dense", parent: "Dense", semiring: int,
+                        count: bool = False) -> Optional[int]:
+        """parent[v, s] = the smallest u of the loop-free in-adjacency's row v with a ⊗ D[u, s] == D[v, s] in bits and D[u, s]
+        strictly better than D[v, s] or equal to it with T[u, s] < T[v, s]; -1 where T[v, s] == 0, D[v, s] is the ⊕
+        identity or no such u exists (``arrow_sr_tree_parents``, ``semiring`` SR_MAX_MIN or SR_MIN_MAX; ``dist`` fp32,
+        ``steps`` T and ``parent`` int32).  With ``count`` returns the in-list entries read (synchronises), else None."""
+        n = c_int64()
+        self._check(self.lib.arrow_sr_tree_parents(self._h, in_adj.h, dist.h, steps.h, parent.h, int(semiring),
+                                                   byref(n) if count else None))
+        return int(n.value) if count else None
 
     def count_diff(self, a: "Dense", b: "Dense") -> int:
         """rows in which two equally shaped tiles differ in some element (-0 == +0, NaN != NaN); synchronises"""
         n = c_int64()
         self._check(self.lib.arrow_dense_count_diff(self._h, a.h, b.h, byref(n)))
+        return int(n.value)
+
+    def count_diff_bits(self, a: "Dense", b: "Dense") -> int:
+        """rows in which two equally shaped fp32 tiles differ in some element's bits (-0 != +0)
+        (``arrow_dense_count_diff_bits``); synchronises"""
+        n = c_int64()
+        self._check(self.lib.arrow_dense_count_diff_bits(self._h, a.h, b.h, byref(n)))
         return int(n.value)
 
     def gather_rows_multi(self, dst: "Dense", srcs: Sequence["Dense"], row_bounds: Sequence[int], m: "RowMap",

@@ -76,7 +76,8 @@ class ArrowDecompositionMPI:
         """Same arguments as the reference (``:106-115``).  ``slim`` only selects the reference's rank
         layout; on a GPU both layouts are the same row-partitioned kernels, so it is accepted and ignored.
         Extensions (one GPU): ``semiring`` -- ``"plus_times"`` (the reference's product), ``"min_plus"`` or
-        ``"max_plus"`` (float32), or ``"or_and"`` (bit features: ``set_features`` takes booleans, non-zero is true, and
+        ``"max_plus"`` (float32), ``"max_min"`` or ``"min_max"`` (float32 bottleneck semirings: widest and minimax paths,
+        see ``bottleneck_tree``), or ``"or_and"`` (bit features: ``set_features`` takes booleans, non-zero is true, and
         ``result_tile()`` returns booleans; with ``add_identity`` a step is one hop of multi-source BFS, see
         ``bfs_levels``) -- and ``add_identity``, which makes a step compute ``X ⊕ (A ⊗ X)`` (see ``engine.py``)."""
         assert not slim or block_diagonal
@@ -216,6 +217,14 @@ class ArrowDecompositionMPI:
         Level 0's permutation maps the rows to vertex ids."""
         return self._bfs_engine("weighted_betweenness").weighted_betweenness(max_steps, out, dependencies_out)
 
+    def bottleneck_tree(self, max_steps: int, distances_out: Optional[np.ndarray] = None,
+                        parents_out: Optional[np.ndarray] = None):
+        """Extension (one GPU, ``max_min`` / ``min_max`` with ``add_identity``): ``iterate_to_fixed_point`` and a path tree
+        of the widest or minimax values, float32 values and int32 parents in ``result_tile()`` row order; a parent is a
+        level-0 row, ``-1`` for sources and elements not reached (see ``ArrowEngine.bottleneck_tree``).  Level 0's
+        permutation maps the parents to vertex ids like the rows."""
+        return self._bfs_engine("bottleneck_tree").bottleneck_tree(max_steps, distances_out, parents_out)
+
     def _bfs_engine(self, what: str) -> ArrowEngine:
         if self.comm.Get_size() > 1:
             raise ValueError(f"{what} runs on one GPU only")
@@ -226,8 +235,9 @@ class ArrowDecompositionMPI:
 
     def iterate_to_fixed_point(self, max_steps: int) -> int:
         """Extension (one GPU): ``step()`` until a step changes no level-0 row, at most ``max_steps`` times; returns the
-        number of steps taken.  Direction-optimising in ``min_plus`` / ``max_plus`` with ``add_identity`` (multi-source
-        shortest and critical paths; see ``ArrowEngine.iterate_to_fixed_point``)."""
+        number of steps taken.  Direction-optimising in ``min_plus`` / ``max_plus`` / ``max_min`` / ``min_max`` with
+        ``add_identity`` (multi-source shortest, critical, widest and minimax paths; see
+        ``ArrowEngine.iterate_to_fixed_point``)."""
         eng = self._require_engine()
         if not isinstance(eng, ArrowEngine):
             raise ValueError("iterate_to_fixed_point runs on one GPU only")

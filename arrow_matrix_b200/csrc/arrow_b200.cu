@@ -2198,6 +2198,7 @@ struct SrMinPlus {
     using T = float;
     static constexpr bool kValues = true;
     __device__ __forceinline__ static float zero() { return __int_as_float(0x7f800000); }       // +inf
+    __device__ __forceinline__ static float one() { return 0.0f; }                               // the ⊗ identity
     __device__ __forceinline__ static float plus(float a, float b) { return fminf(a, b); }
     __device__ __forceinline__ static float times(float a, float x) { return __fadd_rn(a, x); }
     __device__ __forceinline__ static float mac(float acc, float v, float x) { return plus(acc, times(v, x)); }
@@ -2206,10 +2207,37 @@ struct SrMaxPlus {
     using T = float;
     static constexpr bool kValues = true;
     __device__ __forceinline__ static float zero() { return __int_as_float(0xff800000); }       // -inf
+    __device__ __forceinline__ static float one() { return 0.0f; }
     __device__ __forceinline__ static float plus(float a, float b) { return fmaxf(a, b); }
     __device__ __forceinline__ static float times(float a, float x) { return __fadd_rn(a, x); }
     __device__ __forceinline__ static float mac(float acc, float v, float x) { return plus(acc, times(v, x)); }
 };
+// The bottleneck semirings: ⊕ and ⊗ are both min or max, so every result is one of the operands (no rounding).  FMNMX
+// drops a NaN operand (a NaN weight passes the feature through, a NaN feature becomes the ⊗ identity at the first level
+// with the identity) and orders -0 below +0 (DESIGN.md §4).  (max, min): widest paths; (min, max): minimax paths.
+struct SrMaxMin {
+    using T = float;
+    static constexpr bool kValues = true;
+    __device__ __forceinline__ static float zero() { return __int_as_float(0xff800000); }       // -inf
+    __device__ __forceinline__ static float one() { return __int_as_float(0x7f800000); }        // +inf
+    __device__ __forceinline__ static float plus(float a, float b) { return fmaxf(a, b); }
+    __device__ __forceinline__ static float times(float a, float x) { return fminf(a, x); }
+    __device__ __forceinline__ static float mac(float acc, float v, float x) { return plus(acc, times(v, x)); }
+};
+struct SrMinMax {
+    using T = float;
+    static constexpr bool kValues = true;
+    __device__ __forceinline__ static float zero() { return __int_as_float(0x7f800000); }       // +inf
+    __device__ __forceinline__ static float one() { return __int_as_float(0xff800000); }        // -inf
+    __device__ __forceinline__ static float plus(float a, float b) { return fminf(a, b); }
+    __device__ __forceinline__ static float times(float a, float x) { return fmaxf(a, x); }
+    __device__ __forceinline__ static float mac(float acc, float v, float x) { return plus(acc, times(v, x)); }
+};
+// the semirings of arrow_spmm_sr / arrow_gather_rows_sr on fp32 tiles
+bool fp32_semiring(int semiring) {
+    return semiring == ARROW_SR_MIN_PLUS || semiring == ARROW_SR_MAX_PLUS || semiring == ARROW_SR_MAX_MIN ||
+           semiring == ARROW_SR_MIN_MAX;
+}
 
 template <class SR>
 __device__ __forceinline__ float4 sr4_zero() {
@@ -2349,8 +2377,9 @@ __global__ void __launch_bounds__(TILE_THREADS, 4) k_spmm_tiles_sr(TileArgs t) {
                 if (e - p >= 1) batch(std::integral_constant<int, 1>{});
             }
             // tail (and the general case): predicated batches of TAIL.  A skipped entry (column -1) or a slot past the
-            // row's end gets the ⊕ identity as its weight and zeros as its X row: ∓inf + 0 = ∓inf leaves acc unchanged
-            // (one select per slot instead of one per element).  Columns past k4 are computed on zeros and never stored.
+            // row's end gets the ⊕ identity as its weight and zeros as its X row, whose term is the ⊕ identity again and
+            // leaves acc unchanged: ∓inf + 0 = ∓inf in (min, +) / (max, +), min(-inf, 0) = -inf in (max, min) and
+            // max(+inf, 0) = +inf in (min, max) (one select per slot instead of one per element).  Columns past k4 are computed on zeros and never stored.
             // Here and in the batches the weights are read from shared memory once the gathers are back (fewer live
             // registers across the gathers).
             for (; p < e; p += TAIL) {
@@ -2437,7 +2466,8 @@ int launch_tiles_sr_one(arrow_ctx *ctx, const TileArgs &t) {
 }
 
 // (lanes per row, float4 per lane) and tile size as launch_tiles picks them for a plain launch with the default options
-int launch_tiles_sr_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A, bool min_plus) {
+template <class SR>
+int launch_tiles_sr_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A) {
     const int k4 = t.a.k4;
     const int vpl = (k4 >= 32) ? 4 : (k4 >= 8 ? 2 : 1);
     const int lanes = (k4 + vpl - 1) / vpl;           // <= 16: k4 <= 64
@@ -2447,8 +2477,7 @@ int launch_tiles_sr_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A, bool min_pl
     const bool big = list == TILE_LIST_BIG;
     t.tiles = A->tiles[list];
     t.n_tiles = A->n_tiles[list];
-#define TSR(GG, VV, TR, TN)                                                                              \
-    return min_plus ? launch_tiles_sr_one<GG, VV, SrMinPlus, TR, TN>(ctx, t) : launch_tiles_sr_one<GG, VV, SrMaxPlus, TR, TN>(ctx, t)
+#define TSR(GG, VV, TR, TN) return launch_tiles_sr_one<GG, VV, SR, TR, TN>(ctx, t)
 #define SRB(GG, VV) if (big && g == GG && vpl == VV) TSR(GG, VV, TILE_ROWS_BIG, TILE_NNZ_BIG)
 #define SRS(GG, VV) if (g == GG && vpl == VV) TSR(GG, VV, TILE_ROWS, TILE_NNZ)
     SRB(1, 1); SRB(2, 1); SRB(4, 1); SRB(8, 1); SRB(4, 2);
@@ -2459,9 +2488,9 @@ int launch_tiles_sr_shape(arrow_ctx *ctx, TileArgs &t, const Csr *A, bool min_pl
     return fail(ctx, ARROW_ERR_UNSUPPORTED, "no semiring tile kernel for k4=%d vpl=%d", k4, vpl);
 }
 
-// the product of arrow_spmm_sr for (min, +) / (max, +); `a` carries the validated fp32 operands (identity output rows)
+// the product of arrow_spmm_sr for the fp32 semirings; `a` carries the validated fp32 operands (identity output rows)
 template <class SR>
-int spmm_sr(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool min_plus) {
+int spmm_sr(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a) {
     const int k = a.k;
     if (k % 4 != 0 || k > 256) {
         launch_generic<SR>(ctx, a, false, false);
@@ -2472,7 +2501,7 @@ int spmm_sr(arrow_ctx *ctx, const Csr *A, const SpmmArgs &a, bool min_plus) {
         t.ticket = ctx->tile_ticket + 2 * ctx->cur_lane;
         t.l2_hints = ctx->l2_hints_plain;
         t.prefetch = 0;
-        const int rc = launch_tiles_sr_shape(ctx, t, A, min_plus);
+        const int rc = launch_tiles_sr_shape<SR>(ctx, t, A);
         if (rc != ARROW_OK) return rc;
     }
     CUDA_TRY(ctx, cudaGetLastError());
@@ -3440,14 +3469,14 @@ int path_grid(const arrow_ctx *ctx, long long items) {
     return (int)std::min<long long>((items + 7) / 8, (long long)per_sm * sms);
 }
 
-// the segment pass over the adjacency's segments (their partials into a.seg_part, grown to n_segs x k), then the row pass
-// over `n_rows` rows, each as launch(grid, args)
+// the segment pass over the adjacency's segments (their partials into a.seg_part, grown to n_segs x k, unless the passes
+// keep no partials), then the row pass over `n_rows` rows, each as launch(grid, args)
 template <class Launch>
-int launch_seg_passes(arrow_ctx *ctx, PathArgs p, Adj *adj, long long n_rows, Launch &&launch) {
+int launch_seg_passes(arrow_ctx *ctx, PathArgs p, Adj *adj, long long n_rows, Launch &&launch, bool partials = true) {
     if (n_rows == 0) return ARROW_OK;
     if (std::max<long long>(n_rows, adj->n_segs) * p.used > INT_MAX)
         return fail(ctx, ARROW_ERR_RANGE, "%lld rows x %d words exceed the int32 item count", std::max<long long>(n_rows, adj->n_segs), p.used);
-    const size_t part_bytes = (size_t)adj->n_segs * p.k * sizeof(double);
+    const size_t part_bytes = partials ? (size_t)adj->n_segs * p.k * sizeof(double) : 0;
     if (part_bytes > adj->seg_part_bytes) {
         cudaFree(adj->seg_part);                              // waits for the launches that read it
         adj->seg_part = nullptr;
@@ -3457,7 +3486,7 @@ int launch_seg_passes(arrow_ctx *ctx, PathArgs p, Adj *adj, long long n_rows, La
     }
     p.segs = adj->segs;
     p.n_segs = adj->n_segs;
-    p.seg_part = adj->seg_part;
+    p.seg_part = partials ? adj->seg_part : nullptr;
     const int *rows = p.rows;
     for (int pass = 0; pass < 2; ++pass) {
         p.rows = pass == 0 ? nullptr : rows;
@@ -3624,11 +3653,14 @@ __global__ void __launch_bounds__(256) k_wpaths(WPathArgs a) {
 // k_count_diff's figure (rows that differ by value: -0 == +0, NaN != NaN) and the frontier record of the rows that differ
 // in bits, each with its first edge offset in the push adjacency.  A warp takes its 32 rows of a pass one at a time (lanes
 // over the columns) and lane i keeps the claim of the i-th; a CTA claims its slice of the list with one 64-bit atomicAdd
-// on counts[1], packed like k_bits_mark_frontier's.
+// on counts[1], packed like k_bits_mark_frontier's.  STEPS (arrow_sr_mark_frontier_steps) also writes steps[r, c] = level
+// where the two differ in bits, and 0 to every element at level 0.
+template <bool STEPS>
 __global__ void __launch_bounds__(MARK_THREADS) k_sr_mark_frontier(const float *__restrict__ nw, const float *__restrict__ old,
                                                                    long long rows, int k, const int *__restrict__ adj_ptr,
                                                                    int *__restrict__ front_rows, int *__restrict__ front_off,
-                                                                   unsigned long long *__restrict__ counts) {
+                                                                   unsigned long long *__restrict__ counts,
+                                                                   int *__restrict__ steps, int level) {
     constexpr int WARPS = MARK_THREADS / 32;
     __shared__ unsigned long long s_warp[WARPS];
     __shared__ unsigned long long s_base;
@@ -3644,6 +3676,10 @@ __global__ void __launch_bounds__(MARK_THREADS) k_sr_mark_frontier(const float *
                 const float x = a[c], y = b[c];
                 by_value |= x != y;
                 by_bits |= __float_as_uint(x) != __float_as_uint(y);
+                if constexpr (STEPS) {
+                    const bool differ = __float_as_uint(x) != __float_as_uint(y);
+                    if (differ || level == 0) steps[(w0 + i) * k + c] = differ ? level : 0;
+                }
             }
             by_value = __any_sync(0xffffffffu, by_value);
             by_bits = __any_sync(0xffffffffu, by_bits);
@@ -3679,10 +3715,11 @@ __global__ void __launch_bounds__(MARK_THREADS) k_sr_mark_frontier(const float *
     if (changed) atomicAdd(counts, changed);
 }
 
-// canon(x) = fl(0 + x) ⊕ the identity: what the identity diagonal contributes to a pull step (NaN -> identity, -0 -> +0)
+// canon(x) = (the ⊗ identity ⊗ x) ⊕ the ⊕ identity: what the identity diagonal contributes to a pull step.  Tropical:
+// fl(0 + x), NaN -> the ⊕ identity, -0 -> +0.  Bottleneck: x, NaN -> the ⊗ identity (FMNMX drops it), -0 kept.
 template <class SR>
 __device__ __forceinline__ float sr_canon(float x) {
-    return SR::plus(SR::zero(), SR::times(0.0f, x));
+    return SR::plus(SR::zero(), SR::times(SR::one(), x));
 }
 template <class SR>
 __global__ void __launch_bounds__(256) k_sr_canon(const float4 *__restrict__ x, float4 *__restrict__ out, long long n4,
@@ -3709,6 +3746,17 @@ __device__ __forceinline__ void red_fold(SrMaxPlus, float *p, float t) {
 }
 __device__ __forceinline__ bool improves(SrMinPlus, float t, float c) { return t < c; }   // false for a NaN t
 __device__ __forceinline__ bool improves(SrMaxPlus, float t, float c) { return t > c; }
+// The bottleneck targets may hold -0 and t may be -0: the integer folds above already order -0 below +0 (sign set: below
+// every sign-clear pattern), and so must the test, or a +0 term would be dropped against a -0 target.  Among equal
+// values only the two zeros differ in bits, and there the signed integers order them the same way.
+__device__ __forceinline__ void red_fold(SrMaxMin, float *p, float t) { red_fold(SrMaxPlus(), p, t); }
+__device__ __forceinline__ void red_fold(SrMinMax, float *p, float t) { red_fold(SrMinPlus(), p, t); }
+__device__ __forceinline__ bool improves(SrMaxMin, float t, float c) {
+    return t > c || (t == c && __float_as_int(t) > __float_as_int(c));                   // false for a NaN t
+}
+__device__ __forceinline__ bool improves(SrMinMax, float t, float c) {
+    return t < c || (t == c && __float_as_int(t) < __float_as_int(c));
+}
 
 // fold t = fl(a + xu) into *o when it improves on canon(xv), xv the read-only x[v] (failed relaxations cost no atomic)
 template <class SR>
@@ -3762,6 +3810,106 @@ __global__ void __launch_bounds__(PUSH_THREADS) k_sr_push(const V *__restrict__ 
         }
         __syncthreads();                                      // s_lo / s_hi are rewritten by the next chunk
     }
+}
+
+// the push launch of the bottleneck semirings (arrow_sr_push_frontier): k_sr_push on float4 groups or floats
+template <class SR>
+void launch_bottleneck_push(cudaStream_t stream, int grid, const Adj *a, const DenseBuf *X, DenseBuf *O, long long items, int vecs) {
+    if (X->k % 4 == 0)
+        k_sr_push<SR, float4><<<grid, PUSH_THREADS, 0, stream>>>(reinterpret_cast<const float4 *>(X->p), O->p, a->indptr,
+                                                                 a->indices, a->values, a->front_rows, a->front_off,
+                                                                 (int)a->n_front, items, vecs);
+    else
+        k_sr_push<SR, float><<<grid, PUSH_THREADS, 0, stream>>>(X->p, O->p, a->indptr, a->indices, a->values, a->front_rows,
+                                                                a->front_off, (int)a->n_front, items, vecs);
+}
+
+// ------------------------------------------------------------------------------------------------
+// bottleneck path trees (max-min, min-max).  D is a fixed point of the step with the identity and T the level at which each
+// element last changed (k_sr_mark_frontier<true>).  The parent of (v, s) is the smallest in-neighbour u != v with an entry
+// of weight a such that a ⊗ D[u] == D[v] in bits and D[u] is strictly better than D[v] in the ⊕ order, or equal to it
+// with T[u] < T[v]; -1 for T[v] == 0, for D[v] the ⊕ identity and where there is none.  The parent edges strictly improve D
+// or strictly lower T, so they form a forest (DESIGN.md §4).
+// ------------------------------------------------------------------------------------------------
+struct TreeArgs {
+    PathArgs p;                         // the loop-free in-lists, segments, k, used; p.rows: the row pass (every row)
+    const float *__restrict__ wt;       // the lists' weights
+    const float *__restrict__ D;        // the fixed point [n x k]
+    const int *__restrict__ T;          // the step record [n x k]
+    int *__restrict__ parent;           // [n x k], -1 everywhere before the passes
+    bool seg_pass;                      // the segment pass (items: segments x used words), else rows x used words
+};
+
+// the ⊕ order as unsigned integers, -0 below +0 (D never holds NaN where T > 0)
+__device__ __forceinline__ unsigned sr_order_key(float x) {
+    const unsigned u = __float_as_uint(x);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+template <class SR>
+__device__ __forceinline__ bool tree_better(float du, float dv) {
+    if constexpr (std::is_same<SR, SrMaxMin>::value) return sr_order_key(du) > sr_order_key(dv);
+    else return sr_order_key(du) < sr_order_key(dv);
+}
+
+// A warp takes one (row, 32-column word) -- a row's whole list (row pass; lists longer than PATH_SEG are left to the
+// segment pass) or one segment of it (segment pass) -- with a lane per column.  Per batch of 32 list entries lane j loads
+// entry j; the entries are then taken in order, each pending lane testing its own column, until no lane is pending.  The
+// row pass stores a hit, the segment pass folds it with a non-returning unsigned min into the -1 already there.
+template <class SR>
+__global__ void __launch_bounds__(256) k_sr_tree(TreeArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int warps_total = gridDim.x * (blockDim.x >> 5);
+    unsigned long long scanned = 0;
+    for (int it = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); it < a.p.n_items; it += warps_total) {
+        PathItem t;
+        if (a.seg_pass) {
+            t = path_item(a.p, it);
+        } else {
+            t.v = it / a.p.used;
+            t.w = it - t.v * a.p.used;
+            t.b = t.sb = __ldg(a.p.ptr + t.v);
+            t.e = t.se = __ldg(a.p.ptr + t.v + 1);
+            if (t.e - t.b > PATH_SEG) continue;
+        }
+        const int c = t.w * 32 + lane;
+        const long long vc = (long long)t.v * a.p.k + c;
+        float dv = 0.0f;
+        int tv = 0;
+        if (c < a.p.k) {
+            dv = __ldg(a.D + vc);
+            tv = __ldg(a.T + vc);
+        }
+        bool pending = c < a.p.k && tv > 0 && dv != SR::zero();
+        if (!__any_sync(0xffffffffu, pending)) continue;
+        for (int base = t.sb; base < t.se; base += 32) {
+            const int e = base + lane;
+            int x = 0;
+            float w = 0.0f;
+            if (e < t.se) {
+                x = __ldg(a.p.idx + e);
+                w = __ldg(a.wt + e);
+            }
+            const int n = min(32, t.se - base);
+            scanned += (unsigned long long)n;
+            for (int j = 0; j < n; ++j) {
+                const int u = __shfl_sync(0xffffffffu, x, j);
+                const float wj = __shfl_sync(0xffffffffu, w, j);
+                if (pending) {
+                    const long long at = (long long)u * a.p.k + c;
+                    const float du = __ldg(a.D + at);
+                    if (__float_as_uint(SR::times(wj, du)) == __float_as_uint(dv) &&
+                        (tree_better<SR>(du, dv) || (__float_as_uint(du) == __float_as_uint(dv) && __ldg(a.T + at) < tv))) {
+                        if (a.seg_pass) asm volatile("red.global.min.u32 [%0], %1;" ::"l"(a.parent + vc), "r"(u) : "memory");
+                        else a.parent[vc] = u;
+                        pending = false;
+                    }
+                }
+                if (!__any_sync(0xffffffffu, pending)) break;
+            }
+            if (!__any_sync(0xffffffffu, pending)) break;
+        }
+    }
+    if (a.p.scanned && lane == 0 && scanned) atomicAdd(a.p.scanned, scanned);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -5141,8 +5289,7 @@ int arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, in
         if (add_buf < 0 && add_map < 0) return arrow_spmm(ctx, csr, x_buf, c_buf, -1, 0, ARROW_VARIANT_AUTO);
         return arrow_spmm_add(ctx, csr, x_buf, c_buf, add_buf, add_map, ARROW_VARIANT_AUTO);
     }
-    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS && semiring != ARROW_SR_OR_AND)
-        return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
+    if (!fp32_semiring(semiring) && semiring != ARROW_SR_OR_AND) return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
     CHECK_POISON(ctx);
     Csr *A = get_csr(ctx, csr);
     DenseBuf *X = get_dense(ctx, x_buf);
@@ -5188,7 +5335,7 @@ int arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, in
         a.long_threshold = A->long_threshold;
         return spmm_bits(ctx, A, a);
     }
-    if (A->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the (min, +) / (max, +) semirings are float32 only");
+    if (A->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the (min, +) / (max, +) / (max, min) / (min, max) semirings are float32 only");
     if (A->n_rows == 0) return ARROW_OK;
     a.indptr = A->indptr;
     a.indices = A->indices;
@@ -5199,15 +5346,16 @@ int arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, in
     a.k = k;
     a.k4 = k / 4;
     a.long_threshold = A->long_threshold;
-    if (semiring == ARROW_SR_MIN_PLUS) return spmm_sr<SrMinPlus>(ctx, A, a, true);
-    return spmm_sr<SrMaxPlus>(ctx, A, a, false);
+    if (semiring == ARROW_SR_MIN_PLUS) return spmm_sr<SrMinPlus>(ctx, A, a);
+    if (semiring == ARROW_SR_MAX_PLUS) return spmm_sr<SrMaxPlus>(ctx, A, a);
+    if (semiring == ARROW_SR_MAX_MIN) return spmm_sr<SrMaxMin>(ctx, A, a);
+    return spmm_sr<SrMinMax>(ctx, A, a);
 }
 
 int arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int semiring) {
     CHECK_CTX(ctx);
     if (semiring == ARROW_SR_PLUS_TIMES) return arrow_gather_rows(ctx, dst_buf, src_buf, map, ARROW_ACCUMULATE);
-    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS && semiring != ARROW_SR_OR_AND)
-        return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
+    if (!fp32_semiring(semiring) && semiring != ARROW_SR_OR_AND) return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
     CHECK_POISON(ctx);
     DenseBuf *D = get_dense(ctx, dst_buf), *S = get_dense(ctx, src_buf);
     IdxMap *m = get_map(ctx, map);
@@ -5222,9 +5370,11 @@ int arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int 
     if ((semiring == ARROW_SR_OR_AND) != (D->dtype == ARROW_B1))
         return fail(ctx, ARROW_ERR_ARG, "(or, and) runs on bit tiles and only there: semiring %d, tiles of %s", semiring, dtype_name(D->dtype));
     if (semiring == ARROW_SR_OR_AND) return gather_rows_or(ctx, D, S, m);
-    if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the (min, +) / (max, +) semirings are float32 only");
+    if (D->dtype != ARROW_F32) return fail(ctx, ARROW_ERR_UNSUPPORTED, "the (min, +) / (max, +) / (max, min) / (min, max) semirings are float32 only");
     if (semiring == ARROW_SR_MIN_PLUS) return gather_rows_sr<SrMinPlus>(ctx, D, S, m);
-    return gather_rows_sr<SrMaxPlus>(ctx, D, S, m);
+    if (semiring == ARROW_SR_MAX_PLUS) return gather_rows_sr<SrMaxPlus>(ctx, D, S, m);
+    if (semiring == ARROW_SR_MAX_MIN) return gather_rows_sr<SrMaxMin>(ctx, D, S, m);
+    return gather_rows_sr<SrMinMax>(ctx, D, S, m);
 }
 
 // ---- predecessors ---------------------------------------------------------------------------------
@@ -5233,6 +5383,8 @@ int arrow_spmm_sr_witness(arrow_ctx *ctx, int csr, int x_buf, int row_labels, in
     CHECK_CTX(ctx);
     if (semiring == ARROW_SR_PLUS_TIMES)
         return fail(ctx, ARROW_ERR_UNSUPPORTED, "predecessors exist in the (min, +) / (max, +) semirings only");
+    if (semiring == ARROW_SR_MAX_MIN || semiring == ARROW_SR_MIN_MAX)
+        return fail(ctx, ARROW_ERR_UNSUPPORTED, "the witness rule makes cycles in the bottleneck semirings: use arrow_sr_tree_parents");
     if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS)
         return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
     CHECK_POISON(ctx);
@@ -5333,6 +5485,34 @@ int arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed) 
         k_count_diff<double><<<grid, 256, 0, stream>>>(reinterpret_cast<const double *>(A->p), reinterpret_cast<const double *>(B->p), A->rows, A->k, c);
     else
         k_count_diff<float><<<grid, 256, 0, stream>>>(A->p, B->p, A->rows, A->k, c);
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    unsigned long long h = 0;
+    CUDA_TRY(ctx, cudaMemcpyAsync(&h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(stream));
+    *rows_changed = (int64_t)h;
+    return ARROW_OK;
+}
+
+int arrow_dense_count_diff_bits(arrow_ctx *ctx, int a, int b, int64_t *rows_changed) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    DenseBuf *A = get_dense(ctx, a), *B = get_dense(ctx, b);
+    if (!A || !B) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (a=%d b=%d)", a, b);
+    if (!rows_changed) return fail(ctx, ARROW_ERR_ARG, "null rows_changed");
+    if (A->dtype != ARROW_F32 || B->dtype != ARROW_F32 || A->rows != B->rows || A->k != B->k)
+        return fail(ctx, ARROW_ERR_ARG, "two fp32 tiles of one shape: %lld x %d %s vs %lld x %d %s", (long long)A->rows, A->k,
+                    dtype_name(A->dtype), (long long)B->rows, B->k, dtype_name(B->dtype));
+    *rows_changed = 0;
+    if (A->rows == 0 || A->k == 0) return ARROW_OK;
+    cudaStream_t stream = cur_stream(ctx);
+    DevTmp cnt;
+    CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof(unsigned long long)));
+    CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof(unsigned long long), stream));
+    const int grid = (int)std::min<long long>((A->rows + 7) / 8, (long long)ctx->sm_count * 8);
+    // a row of k fp32 elements read as k words of 32 bits each: the bit-tile comparison over all 32 k bits
+    k_count_diff_bits<<<grid, 256, 0, stream>>>(reinterpret_cast<const unsigned int *>(A->p), reinterpret_cast<const unsigned int *>(B->p),
+                                                A->rows, 32 * A->k, A->k, reinterpret_cast<unsigned long long *>(cnt.p));
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     unsigned long long h = 0;
@@ -6059,10 +6239,10 @@ int arrow_wpaths_dependencies(arrow_ctx *ctx, int out_adj, int x0_buf, int dist_
     return read_scanned(ctx, cnt, entries_read);
 }
 
-int arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int64_t *rows_changed, int64_t *frontier_rows,
-                           int64_t *frontier_edges) {
-    CHECK_CTX(ctx);
-    CHECK_POISON(ctx);
+namespace {
+// arrow_sr_mark_frontier, and with steps_buf >= 0 arrow_sr_mark_frontier_steps
+int sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int steps_buf, int level, int64_t *rows_changed,
+                     int64_t *frontier_rows, int64_t *frontier_edges) {
     Adj *a = get_adj(ctx, adj);
     if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
     if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
@@ -6074,6 +6254,16 @@ int arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, in
     if (N->rows != O->rows || N->k != O->k || N->rows != a->n)
         return fail(ctx, ARROW_ERR_ARG, "tiles differ in shape: new %lld x %d, old %lld x %d, adjacency %lld rows",
                     (long long)N->rows, N->k, (long long)O->rows, O->k, (long long)a->n);
+    DenseBuf *S = nullptr;
+    if (steps_buf >= 0) {
+        S = get_dense(ctx, steps_buf);
+        if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (steps=%d)", steps_buf);
+        if (S->dtype != ARROW_I32 || S->rows != N->rows || S->k != N->k)
+            return fail(ctx, ARROW_ERR_ARG, "steps is an int32 tile of new's shape (%lld x %d): got %s %lld x %d", (long long)N->rows,
+                        N->k, dtype_name(S->dtype), (long long)S->rows, S->k);
+        if (S->p == N->p || S->p == O->p) return fail(ctx, ARROW_ERR_ARG, "steps aliases new or old");
+        if (level < 0) return fail(ctx, ARROW_ERR_ARG, "level %d < 0", level);
+    }
     *rows_changed = *frontier_rows = *frontier_edges = 0;
     a->tag = -1;                                              // the record is rewritten below
     cudaStream_t stream = cur_stream(ctx);
@@ -6083,8 +6273,13 @@ int arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, in
         CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof h));
         CUDA_TRY(ctx, cudaMemsetAsync(cnt.p, 0, sizeof h, stream));
         const int grid = (int)std::min<long long>((N->rows + MARK_THREADS - 1) / MARK_THREADS, (long long)ctx->sm_count * 8);
-        k_sr_mark_frontier<<<grid, MARK_THREADS, 0, stream>>>(N->p, O->p, N->rows, N->k, a->indptr, a->front_rows,
-                                                              a->front_off, reinterpret_cast<unsigned long long *>(cnt.p));
+        unsigned long long *counts = reinterpret_cast<unsigned long long *>(cnt.p);
+        if (S)
+            k_sr_mark_frontier<true><<<grid, MARK_THREADS, 0, stream>>>(N->p, O->p, N->rows, N->k, a->indptr, a->front_rows,
+                                                                        a->front_off, counts, reinterpret_cast<int *>(S->p), level);
+        else
+            k_sr_mark_frontier<false><<<grid, MARK_THREADS, 0, stream>>>(N->p, O->p, N->rows, N->k, a->indptr, a->front_rows,
+                                                                         a->front_off, counts, nullptr, 0);
         ctx->launches++;
         CUDA_TRY(ctx, cudaGetLastError());
         CUDA_TRY(ctx, cudaMemcpyAsync(h, cnt.p, sizeof h, cudaMemcpyDeviceToHost, stream));
@@ -6100,13 +6295,29 @@ int arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, in
     *frontier_edges = a->front_edges;
     return ARROW_OK;
 }
+}  // namespace
+
+int arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int64_t *rows_changed, int64_t *frontier_rows,
+                           int64_t *frontier_edges) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    return sr_mark_frontier(ctx, adj, new_buf, old_buf, -1, 0, rows_changed, frontier_rows, frontier_edges);
+}
+
+int arrow_sr_mark_frontier_steps(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int steps_buf, int level,
+                                 int64_t *rows_changed, int64_t *frontier_rows, int64_t *frontier_edges) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    if (steps_buf < 0) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (steps=%d)", steps_buf);
+    return sr_mark_frontier(ctx, adj, new_buf, old_buf, steps_buf, level, rows_changed, frontier_rows, frontier_edges);
+}
 
 int arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int semiring) {
     CHECK_CTX(ctx);
     CHECK_POISON(ctx);
     if (semiring == ARROW_SR_PLUS_TIMES || semiring == ARROW_SR_OR_AND)
-        return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_sr_push_frontier runs min-plus and max-plus, not semiring %d", semiring);
-    if (semiring != ARROW_SR_MIN_PLUS && semiring != ARROW_SR_MAX_PLUS) return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
+        return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_sr_push_frontier runs the fp32 semirings, not semiring %d", semiring);
+    if (!fp32_semiring(semiring)) return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
     const Adj *a = get_adj(ctx, adj);
     if (!a) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", adj);
     if (a->incoming) return fail(ctx, ARROW_ERR_ARG, "adjacency %d is an in-adjacency (arrow_adj_build_in)", adj);
@@ -6133,7 +6344,9 @@ int arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int 
         const float4 *x4 = reinterpret_cast<const float4 *>(X->p);
         float4 *o4 = reinterpret_cast<float4 *>(O->p);
         if (mn) k_sr_canon<SrMinPlus><<<grid, 256, 0, stream>>>(x4, o4, n4, X->p, O->p, n);
-        else k_sr_canon<SrMaxPlus><<<grid, 256, 0, stream>>>(x4, o4, n4, X->p, O->p, n);
+        else if (semiring == ARROW_SR_MAX_PLUS) k_sr_canon<SrMaxPlus><<<grid, 256, 0, stream>>>(x4, o4, n4, X->p, O->p, n);
+        else if (semiring == ARROW_SR_MAX_MIN) k_sr_canon<SrMaxMin><<<grid, 256, 0, stream>>>(x4, o4, n4, X->p, O->p, n);
+        else k_sr_canon<SrMinMax><<<grid, 256, 0, stream>>>(x4, o4, n4, X->p, O->p, n);
         ctx->launches++;
         CUDA_TRY(ctx, cudaGetLastError());
     }
@@ -6145,6 +6358,13 @@ int arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int 
     const int per_sm = ctx->spmm_ctas_per_sm > 0 ? std::min(ctx->spmm_ctas_per_sm, 8) : 8;
     const int sms = ctx->spmm_sm_limit > 0 ? std::min(ctx->sm_count, ctx->spmm_sm_limit) : ctx->sm_count;
     const int grid = (int)std::min<long long>(chunks, (long long)per_sm * sms);
+    if (semiring == ARROW_SR_MAX_MIN) launch_bottleneck_push<SrMaxMin>(stream, grid, a, X, O, items, vecs);
+    if (semiring == ARROW_SR_MIN_MAX) launch_bottleneck_push<SrMinMax>(stream, grid, a, X, O, items, vecs);
+    if (semiring == ARROW_SR_MAX_MIN || semiring == ARROW_SR_MIN_MAX) {
+        ctx->launches++;
+        CUDA_TRY(ctx, cudaGetLastError());
+        return ARROW_OK;
+    }
     const float4 *x4 = reinterpret_cast<const float4 *>(X->p);
 #define SRP(SR, V, XP) k_sr_push<SR, V><<<grid, PUSH_THREADS, 0, stream>>>(XP, O->p, a->indptr, a->indices, a->values, \
                                                                        a->front_rows, a->front_off, (int)a->n_front, items, vecs)
@@ -6156,6 +6376,57 @@ int arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int 
     ctx->launches++;
     CUDA_TRY(ctx, cudaGetLastError());
     return ARROW_OK;
+}
+
+int arrow_sr_tree_parents(arrow_ctx *ctx, int in_adj, int dist_buf, int steps_buf, int parent_buf, int semiring,
+                          int64_t *entries_read) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    if (semiring == ARROW_SR_PLUS_TIMES || semiring == ARROW_SR_MIN_PLUS || semiring == ARROW_SR_MAX_PLUS || semiring == ARROW_SR_OR_AND)
+        return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_sr_tree_parents runs max-min and min-max, not semiring %d", semiring);
+    if (semiring != ARROW_SR_MAX_MIN && semiring != ARROW_SR_MIN_MAX) return fail(ctx, ARROW_ERR_ARG, "unknown semiring %d", semiring);
+    Adj *in = get_adj(ctx, in_adj);
+    if (!in) return fail(ctx, ARROW_ERR_HANDLE, "bad adjacency handle %d", in_adj);
+    if (!in->loopfree || !in->incoming)
+        return fail(ctx, ARROW_ERR_ARG, "in_adj is the loop-free in-adjacency (arrow_adj_build_loopfree, incoming)");
+    DenseBuf *D = get_dense(ctx, dist_buf), *T = get_dense(ctx, steps_buf), *P = get_dense(ctx, parent_buf);
+    if (!D || !T || !P) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (dist=%d steps=%d parent=%d)", dist_buf, steps_buf, parent_buf);
+    if (D->dtype != ARROW_F32 || T->dtype != ARROW_I32 || P->dtype != ARROW_I32)
+        return fail(ctx, ARROW_ERR_ARG, "dist is fp32, steps and parent int32: got %s / %s / %s", dtype_name(D->dtype),
+                    dtype_name(T->dtype), dtype_name(P->dtype));
+    if (D->rows != in->n || T->rows != in->n || P->rows != in->n || T->k != D->k || P->k != D->k)
+        return fail(ctx, ARROW_ERR_ARG, "shape: dist %lld x %d, steps %lld x %d, parent %lld x %d, adjacency %lld rows",
+                    (long long)D->rows, D->k, (long long)T->rows, T->k, (long long)P->rows, P->k, (long long)in->n);
+    if (P->p == D->p || P->p == T->p) return fail(ctx, ARROW_ERR_ARG, "parent aliases dist or steps");
+    TreeArgs t{};
+    DevTmp cnt;
+    if (const int rc = alloc_scanned(ctx, cnt, entries_read, t.p)) return rc;
+    const long long n = in->n;
+    const int k = D->k;
+    if (n == 0 || k == 0) return read_scanned(ctx, cnt, entries_read);
+    cudaStream_t s = cur_stream(ctx);
+    // -1 everywhere: the row pass stores the hits of the short lists, the segment pass folds those of the long ones
+    CUDA_TRY(ctx, cudaMemsetAsync(P->p, 0xff, (size_t)n * k * 4, s));
+    t.p.ptr = in->indptr;
+    t.p.idx = in->indices;
+    t.p.k = k;
+    t.p.used = (k + 31) / 32;
+    t.wt = in->values;
+    t.D = D->p;
+    t.T = reinterpret_cast<const int *>(T->p);
+    t.parent = reinterpret_cast<int *>(P->p);
+    // launch_seg_passes runs the segment pass first (when there are segments), then the row pass over every row
+    bool first = true;
+    const int rc = launch_seg_passes(ctx, t.p, in, n, [&](int grid, const PathArgs &q) {
+        TreeArgs a = t;
+        a.p = q;
+        a.seg_pass = first && in->n_segs > 0;
+        first = false;
+        if (semiring == ARROW_SR_MAX_MIN) k_sr_tree<SrMaxMin><<<grid, 256, 0, s>>>(a);
+        else k_sr_tree<SrMinMax><<<grid, 256, 0, s>>>(a);
+    }, false);                                                // the hits fold into P: no segment partials
+    if (rc) return rc;
+    return read_scanned(ctx, cnt, entries_read);
 }
 
 int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, const int64_t *row_bounds, int n_src, int map, int flags) {

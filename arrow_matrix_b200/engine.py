@@ -35,6 +35,12 @@ was first reached.
 ``predecessors()`` returns, in the tropical semirings, the level-0 row each element's value came from (the parent array
 of a BFS tree, the predecessor of a shortest or critical path): one more pass of the fused step over (value, label)
 pairs, see DESIGN.md §4.
+
+``max_min`` and ``min_max`` are the bottleneck semirings (float32): ⊕ and ⊗ are max and min (``max_min``, widest paths:
+the largest capacity of a path, a path's capacity being its smallest edge) or min and max (``min_max``, minimax paths: the
+smallest possible largest edge).  Every result is one of the operands, so no rounding enters.  ``bottleneck_tree()``
+returns the fixed point with a path tree: ties are the rule in these semirings, so its parents follow the level at which
+each value last changed rather than ``predecessors()``' witness rule.
 """
 from __future__ import annotations
 
@@ -48,8 +54,11 @@ from . import decomp
 
 # the semiring's ⊕ identity (its "zero": what zero_rhs and fresh tiles hold) and ⊗ identity (what add_identity puts on
 # level 0's diagonal)
-_PLUS_ZERO = {_lib.SR_PLUS_TIMES: 0.0, _lib.SR_MIN_PLUS: float("inf"), _lib.SR_MAX_PLUS: float("-inf"), _lib.SR_OR_AND: 0.0}
-_TIMES_ONE = {_lib.SR_PLUS_TIMES: 1.0, _lib.SR_MIN_PLUS: 0.0, _lib.SR_MAX_PLUS: 0.0, _lib.SR_OR_AND: 1.0}
+_PLUS_ZERO = {_lib.SR_PLUS_TIMES: 0.0, _lib.SR_MIN_PLUS: float("inf"), _lib.SR_MAX_PLUS: float("-inf"), _lib.SR_OR_AND: 0.0,
+              _lib.SR_MAX_MIN: float("-inf"), _lib.SR_MIN_MAX: float("inf")}
+_TIMES_ONE = {_lib.SR_PLUS_TIMES: 1.0, _lib.SR_MIN_PLUS: 0.0, _lib.SR_MAX_PLUS: 0.0, _lib.SR_OR_AND: 1.0,
+              _lib.SR_MAX_MIN: float("inf"), _lib.SR_MIN_MAX: float("-inf")}
+_BOTTLENECK = (_lib.SR_MAX_MIN, _lib.SR_MIN_MAX)
 
 
 # bfs_levels(): a level is a push when its frontier's edges times this are fewer than the non-zeros a pull step gathers.
@@ -64,8 +73,9 @@ def bfs_direction(frontier_edges: int, total_nnz: int, alpha: float = BFS_PUSH_A
     return "push" if frontier_edges * alpha < total_nnz else "pull"
 
 
-# iterate_to_fixed_point() in min_plus / max_plus: a level is a push when its frontier's edges times this are fewer than
-# the non-zeros a pull step gathers (bfs_direction with this alpha).  A tropical push moves k fp32 values per edge and
+# iterate_to_fixed_point() in min_plus / max_plus (and max_min / min_max, whose push moves and compares as many values): a
+# level is a push when its frontier's edges times this are fewer than the non-zeros a pull step gathers (bfs_direction with
+# this alpha).  A tropical push moves k fp32 values per edge and
 # compares each, so it costs more per edge than the bit push.  Per level on an H100 80 GB HBM3 at 700 W
 # (scripts/sssp_direction_bench.py, DESIGN.md §8) push and pull cross at total_nnz / frontier_edges of about 9-10 on G2 at
 # k = 128 (pull 10.8 ms, push 3.6 ms plus about 0.4 ns per edge), 7-9 at k = 16 and about 2 on the 10**6-vertex BA graph at
@@ -167,6 +177,8 @@ class ArrowEngine:
         self._wp_tiles: Optional[Tuple[_lib.Dense, ...]] = None      # weighted betweenness: X0, state, sigma tiles
         self._wp_delta: Optional[Tuple[_lib.Dense, ...]] = None      # weighted_betweenness(): delta and [n x 1] bc
         self.last_path_rounds = 0                                # tight-DAG rounds of the last weighted path call
+        self._bt_in_adj: Optional[_lib.Adjacency] = None         # bottleneck_tree(): the loop-free in-adjacency
+        self._bt_tiles: Optional[Tuple[_lib.Dense, ...]] = None  # bottleneck_tree(): int32 steps and parent tiles
         fused_ok = True
         cmap_prev = None                      # level j-1 row -> level-0 row (host, int64, -1 invalid)
         for j, (B, _) in enumerate(decomposition):
@@ -447,22 +459,42 @@ class ArrowEngine:
         level.  The step count and, after every level, the level-0 features (so ``result()``, ``features()``,
         ``count_changed()``, ``predecessors()`` and the next ``step()``) are bit-identical to pull steps only.  After a
         push level the tiles of the levels ``j >= 1`` (``result(j)``) are not that level's product; the next ``step()``
-        rewrites them.  Every other engine, and one with a -0 weight, pulls every level."""
+        rewrites them.  The same holds in ``max_min`` / ``min_max``, -0 weights included; there the loop stops when a step
+        changes no level-0 row in bits, since their order puts -0 below +0 (a step that only turns -0 into +0 is
+        progress).  Every other engine, and a tropical one with a -0 weight, pulls every level."""
         adj = self._sr_push_adjacency() if self._sr_push_ok() and int(max_steps) >= 1 else None
         if adj is None:
+            st0 = self.levels[0]
             for n in range(1, int(max_steps) + 1):
                 self.step()
-                if self.count_changed() == 0:
+                changed = self.ctx.count_diff_bits(st0.bufs[0], st0.bufs[1]) if self.sr in _BOTTLENECK \
+                    else self.count_changed()
+                if changed == 0:
                     self.last_fixed_point_directions = ["pull"] * n
                     return n
             self.last_fixed_point_directions = ["pull"] * max(int(max_steps), 0)
             return int(max_steps)
+        return self._marked_fixed_point(max_steps, adj, True)
+
+    def _marked_fixed_point(self, max_steps: int, adj: _lib.Adjacency, pushes: bool,
+                            steps: Optional[_lib.Dense] = None) -> int:
+        """the direction-optimising loop of ``iterate_to_fixed_point`` on the weighted push adjacency ``adj``; every level
+        is a pull unless ``pushes``.  With ``steps`` (int32) the mark pass after level h also writes h where the level
+        changed an element's bits (0 everywhere after level 0): T of ``bottleneck_tree``."""
         st0 = self.levels[0]
         limit = self._push_limit
 
-        def mark(new, old):
-            """(rows changed, push next): the stop test, and the direction of the next level"""
-            changed, _, edges = self.ctx.sr_mark_frontier(adj, new, old)
+        def mark(new, old, level):
+            """(rows changed, push next): the stop test -- rows changed by value, in bits in the bottleneck semirings --
+            and the direction of the next level"""
+            if steps is None:
+                changed, rows, edges = self.ctx.sr_mark_frontier(adj, new, old)
+            else:
+                changed, rows, edges = self.ctx.sr_mark_frontier_steps(adj, new, old, steps, level)
+            if self.sr in _BOTTLENECK:
+                changed = rows
+            if not pushes:
+                return changed, False
             push = edges < limit if limit is not None else bfs_direction(edges, self.total_nnz, SR_PUSH_ALPHA) == "push"
             return changed, push
 
@@ -470,7 +502,7 @@ class ArrowEngine:
         # writes holds it meanwhile.
         xi = st0.xi
         st0.bufs[1 - xi].fill(_PLUS_ZERO[self.sr])
-        _, push = mark(st0.bufs[xi], st0.bufs[1 - xi])
+        _, push = mark(st0.bufs[xi], st0.bufs[1 - xi], 0)
         directions = []
         for n in range(1, int(max_steps) + 1):
             xi = st0.xi
@@ -480,7 +512,7 @@ class ArrowEngine:
             else:
                 self.step()                      # reads bufs[xi], leaves the result in bufs[1 - xi]
             directions.append("push" if push else "pull")
-            changed, push = mark(st0.bufs[1 - xi], st0.bufs[xi])
+            changed, push = mark(st0.bufs[1 - xi], st0.bufs[xi], n)
             if changed == 0:
                 self.last_fixed_point_directions = directions
                 return n
@@ -488,10 +520,11 @@ class ArrowEngine:
         return int(max_steps)
 
     def _sr_push_ok(self) -> bool:
-        """iterate_to_fixed_point() may push: a tropical engine with the identity, every non-zero behind a level-0 row, no
-        -0 weight, and a step that advances level 0's features (an exchange-mode step of one level does not)"""
-        return (self.sr in (_lib.SR_MIN_PLUS, _lib.SR_MAX_PLUS) and self.add_identity and self.fused_ok
-                and not self._neg_zero_weight and (self.mode == "fused" or self.L > 1))
+        """iterate_to_fixed_point() may push: a tropical engine without a -0 weight or a bottleneck engine, with the
+        identity, every non-zero behind a level-0 row, and a step that advances level 0's features (an exchange-mode step
+        of one level does not)"""
+        return ((self.sr in (_lib.SR_MIN_PLUS, _lib.SR_MAX_PLUS) and not self._neg_zero_weight or self.sr in _BOTTLENECK)
+                and self.add_identity and self.fused_ok and (self.mode == "fused" or self.L > 1))
 
     def _sr_push_adjacency(self) -> _lib.Adjacency:
         """the weighted transposed operator of the fused step with the identity (built on the first call): every level's
@@ -519,6 +552,9 @@ class ArrowEngine:
             raise ValueError("predecessors exist in the min_plus / max_plus semirings only, the engine runs plus_times")
         if self.sr == _lib.SR_OR_AND:
             raise ValueError("predecessors exist in the min_plus / max_plus semirings only, the engine runs or_and")
+        if self.sr in _BOTTLENECK:
+            raise ValueError(f"predecessors' witness rule makes cycles in the {self.semiring} semiring, where ties are the "
+                             "rule: use bottleneck_tree()")
         if not self.fused_ok:
             raise ValueError("predecessors need a level-0 row behind every non-zero, but a level reads rows behind the "
                              "sentinel")
@@ -554,6 +590,61 @@ class ArrowEngine:
             add = dict(add_values=values[1], add_labels=self._wit_labels[1], add_map=nxt.to_next_dev)
         self.ctx.spmm_sr_witness(st0.csr, x, self._wit_labels[0], dist=x, semiring=self.sr, **add)
         return self._wit_labels[0]
+
+    # -- bottleneck path trees (max_min / min_max) ------------------------------------------------------------------
+    def bottleneck_tree(self, max_steps: int, distances_out: Optional[np.ndarray] = None,
+                        parents_out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """``iterate_to_fixed_point(max_steps)`` that also returns a path tree of the fixed point reached (``D`` float32
+        and ``P`` int32, both [n x k] in level-0 row order like ``result()``).  ``D[v, s]`` is the widest (``max_min``)
+        or minimax (``min_max``) value from the sources of column ``s``.  Let ``T[v, s]`` be the level at which the loop
+        last changed the element's bits (0 if never).  ``P[v, s]`` is -1 where ``T[v, s] == 0`` (the sources) or
+        ``D[v, s]`` is the ⊕ identity (not reached).  Otherwise it is the smallest level-0 row ``u != v`` with an entry
+        ``u -> v`` of weight ``a`` of the fused step's operator such that ``a ⊗ D[u, s] == D[v, s]`` in bits and either
+        ``D[u, s]`` is strictly better than ``D[v, s]`` in the ⊕ order or the two are equal and ``T[u, s] < T[v, s]``;
+        -1 when there is none.  Along every parent edge ``D`` strictly improves or ``T`` strictly drops, so ``P`` has no
+        cycles, and at a fixed point every element with ``T > 0`` that is reached has a parent (DESIGN.md §4), with the
+        NaN exceptions below.  The loop stops after a level that changes no row in bits.  ``max_steps`` may stop it
+        early, which can leave such elements at -1.  ⊕ and ⊗ drop a NaN operand: a NaN weight passes the feature
+        through, and a NaN feature becomes the ⊗ identity at the first level (a source whose ``T`` is 1); an element that
+        the first level gives the ⊗ identity through an edge of weight ⊗ identity from a NaN feature has no parent either.
+        -0 orders below +0 everywhere.
+
+        The step count, ``last_fixed_point_directions`` and the features are those of ``iterate_to_fixed_point``; the
+        mark pass after each level also writes ``T``, and one pass over the in-lists then finds the parents.  An engine
+        that does not push (exchange mode with one level) still builds the weighted push adjacency for the frontier record
+        and pulls every level.  The loop-free in-adjacency (8 bytes per edge) and the int32 ``T`` and parent tiles (4
+        bytes per element each: 5.1 GB apiece at 10M rows and k = 128, beside the two feature tiles and the weighted push
+        adjacency) are made on the first call and kept until ``close()``.  Raises ``ValueError`` before any CUDA work for
+        another semiring, ``add_identity=False``, and when a level reads rows behind the sentinel (``fused_ok`` is false:
+        such a row has no vertex identity).  Synchronises."""
+        D, P = self._bottleneck_tree_run(max_steps)
+        return D.d2h(distances_out), P.d2h(parents_out)
+
+    def _bottleneck_tree_run(self, max_steps: int) -> Tuple[_lib.Dense, _lib.Dense]:
+        """the device part of ``bottleneck_tree``: the level-0 feature tile holding D and the int32 parent tile"""
+        self._bottleneck_checks("bottleneck_tree")
+        self.sync()
+        st0 = self.levels[0]
+        if self._bt_in_adj is None:
+            parts = [(st.csr, st.cmap_dev) for st in self.levels]
+            self._bt_in_adj = self.ctx.adj_build_loopfree(parts, st0.rows, direction="in")
+        if self._bt_tiles is None:
+            self._bt_tiles = (self.ctx.dense_alloc(st0.rows, self.k, np.int32),
+                              self.ctx.dense_alloc(st0.rows, self.k, np.int32))
+        steps, parents = self._bt_tiles
+        self._marked_fixed_point(max_steps, self._sr_push_adjacency(), self._sr_push_ok(), steps)
+        D = self.result_buffer(0)
+        self.ctx.sr_tree_parents(self._bt_in_adj, D, steps, parents, self.sr)
+        return D, parents
+
+    def _bottleneck_checks(self, what: str):
+        if self.sr not in _BOTTLENECK:
+            raise ValueError(f"{what} runs the max_min / min_max semirings, the engine runs {self.semiring}")
+        if not self.add_identity:
+            raise ValueError(f"{what} needs add_identity=True: a step must keep the values it already has")
+        if not self.fused_ok:
+            raise ValueError(f"{what} needs a level-0 row behind every non-zero, but a level reads rows behind the "
+                             "sentinel")
 
     # -- multi-source BFS (or_and) ----------------------------------------------------------------------------------
     def bfs_levels(self, max_steps: int, out: Optional[np.ndarray] = None) -> np.ndarray:
@@ -978,4 +1069,8 @@ class ArrowEngine:
                 b.free()
         self._in_adj = self._bfs_parents = self._bfs_sigma = self._bfs_delta = None
         self._wp_adjs = self._wp_tiles = self._wp_delta = None
+        for b in (self._bt_in_adj,) + (self._bt_tiles or ()):
+            if b is not None:
+                b.free()
+        self._bt_in_adj = self._bt_tiles = None
         self.ctx.close()

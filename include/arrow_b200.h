@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 12
+#define ARROW_ABI_VERSION 13
 
 /* error codes */
 #define ARROW_OK              0
@@ -230,6 +230,11 @@ int  arrow_gather_rows(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int fl
                                    entry exists" (the block's values, of either precision, are not read), ⊕ is OR.  Every
                                    operand is a bit tile, else ARROW_ERR_ARG; a bit operand with another semiring: ARROW_ERR_ARG.
                                    arrow_gather_rows without ARROW_ACCUMULATE moves bit rows (with it: ARROW_ERR_ARG) */
+/* The bottleneck semirings (fp32, validated and refused like MIN_PLUS / MAX_PLUS).  ⊕ and ⊗ are both min or max, so every
+ * result element is one of the operands, exactly.  A NaN operand is dropped by ⊕ and ⊗ (a NaN weight passes the feature
+ * through), and -0 orders below +0 everywhere. */
+#define ARROW_SR_MAX_MIN    4   /* widest paths: ⊕ = max (identity -inf), ⊗ = min (identity +inf) */
+#define ARROW_SR_MIN_MAX    5   /* minimax paths: ⊕ = min (identity +inf), ⊗ = max (identity -inf) */
 /* C[r] = (⊕_p A[r,p] ⊗ X[col_p]) ⊕ add[add_map[r]]  (add_buf / add_map may be -1; rows with add_map[r] == -1 get the
  * product only; a row without entries, or whose entries are all skipped columns, gets the ⊕ identity) */
 int  arrow_spmm_sr(arrow_ctx *ctx, int csr, int x_buf, int c_buf, int add_buf, int add_map, int semiring);
@@ -238,6 +243,10 @@ int  arrow_gather_rows_sr(arrow_ctx *ctx, int dst_buf, int src_buf, int map, int
 /* number of rows of two equally shaped tiles (same rows, k and element type) that differ in some element, compared by
  * value (-0 == +0, NaN != NaN; bit tiles over their k columns); synchronises the context's current lane */
 int  arrow_dense_count_diff(arrow_ctx *ctx, int a, int b, int64_t *rows_changed);
+/* number of rows of two fp32 tiles of one shape that differ in some element's bits (-0 != +0, a NaN equal to the same NaN):
+ * the stop test of the bottleneck fixed point, whose order puts -0 below +0; ARROW_ERR_ARG for other types or shapes;
+ * synchronises the context's current lane */
+int  arrow_dense_count_diff_bits(arrow_ctx *ctx, int a, int b, int64_t *rows_changed);
 /* BFS level record of the (or, and) step: dist[r, c] = level for every (r, c < k) whose bit is set in new_buf and clear in
  * old_buf (bit tiles); every other element of dist_buf (ARROW_I32, same rows and k) is left alone.  *n_new = the number of
  * such bits (0: the step reached its fixed point); synchronises the context's current lane. */
@@ -348,6 +357,33 @@ int  arrow_sr_mark_frontier(arrow_ctx *ctx, int adj, int new_buf, int old_buf, i
  * other than the adjacency's, out of another shape or k, an unknown semiring code; ARROW_ERR_UNSUPPORTED: PLUS_TIMES,
  * OR_AND. */
 int  arrow_sr_push_frontier(arrow_ctx *ctx, int adj, int x_buf, int out_buf, int semiring);
+/* MAX_MIN / MIN_MAX: out = canon(x) = x ⊗ the ⊗ identity (NaN -> that identity, every other value, -0 included, kept),
+ * then t = a ⊗ x[u, s] is folded into out[v, s] with a non-returning max (MAX_MIN) or min (MIN_MAX) where it improves on
+ * canon(x[v, s]) in the ⊕ order with -0 below +0.  Out is the step of X_h bit for bit under the conditions above, -0
+ * weights included. */
+
+/* ---- bottleneck path trees (one GPU, max-min / min-max on fp32 tiles) ------------------------------------------------ */
+/* arrow_sr_mark_frontier, and in the same pass steps[r, c] = level for every element where new_buf and old_buf differ in
+ * bits; level 0 writes 0 to every element instead.  steps_buf is an ARROW_I32 tile of new_buf's rows and k.  In a
+ * fixed-point loop steps then holds T, the level at which every element last changed.  ARROW_ERR_ARG: those of
+ * arrow_sr_mark_frontier, another steps type or shape, steps aliasing new or old, a negative level.  Synchronises. */
+int  arrow_sr_mark_frontier_steps(arrow_ctx *ctx, int adj, int new_buf, int old_buf, int steps_buf, int level,
+                                  int64_t *rows_changed, int64_t *frontier_rows, int64_t *frontier_edges);
+/* Parents of a bottleneck fixed point D (dist_buf, fp32) with its step record T (steps_buf, int32), over the loop-free
+ * weighted in-adjacency (arrow_adj_build_loopfree, incoming != 0).  parent[v, s] = -1 where T[v, s] == 0 or D[v, s] is the
+ * ⊕ identity; otherwise the smallest u of in_adj's row v with an entry of weight a such that a ⊗ D[u, s] == D[v, s] in
+ * bits and either D[u, s] is strictly better than D[v, s] in the ⊕ order (-0 below +0) or the two are equal and
+ * T[u, s] < T[v, s]; -1 when there is none.  Along every parent edge D strictly improves or T strictly drops, so the
+ * parents form a forest whose roots have T == 0 or no parent.  At a fixed point in bits every element with T > 0 that is
+ * reached has a parent, except NaN features and the elements the first level gives the ⊗ identity from one through an
+ * edge of weight ⊗ identity.  A warp walks a row's ascending in-list for one 32-column
+ * word until every element of it has a hit; lists longer than 512 entries are split at the adjacency's segments and folded
+ * with an unsigned min into -1, so the result depends on neither the grid nor the order.  *entries_read (may be NULL; then
+ * the call does not synchronise) receives the in-list entries read.  ARROW_ERR_ARG: in_adj not the loop-free
+ * in-adjacency, dist not fp32, steps or parent not ARROW_I32, shapes other than the adjacency's rows and dist's k, parent
+ * aliasing dist or steps, a semiring other than MAX_MIN / MIN_MAX (ARROW_ERR_UNSUPPORTED for the other known codes). */
+int  arrow_sr_tree_parents(arrow_ctx *ctx, int in_adj, int dist_buf, int steps_buf, int parent_buf, int semiring,
+                           int64_t *entries_read);
 
 /* ---- weighted betweenness (one GPU, min-plus on fp32 tiles): shortest-path counts and Brandes dependencies ------------- */
 /* The weighted adjacency of M without the edges u == v: the lists of arrow_adj_build (incoming == 0) or arrow_adj_build_in
@@ -395,8 +431,9 @@ int  arrow_wpaths_dependencies(arrow_ctx *ctx, int out_adj, int x0_buf, int dist
  *   dist_buf >= 0: parents to lab_out: P[r] = label where D[r] (row r of dist_buf; it may be x_buf) is not the ⊕
  *                  identity and the witness value equals it, else -1; values to val_out when val_out >= 0
  *   add_val / add_lab / add_map: all three or none (-1)
- * Every output has the block's rows and X's k; no output aliases an input or the other output.  ARROW_SR_PLUS_TIMES
- * and fp64 operands: ARROW_ERR_UNSUPPORTED; mixed or wrong element types, bad shapes, aliasing, an unknown semiring
+ * Every output has the block's rows and X's k; no output aliases an input or the other output.  ARROW_SR_PLUS_TIMES,
+ * MAX_MIN / MIN_MAX (ties are the rule there and this witness makes cycles: arrow_sr_tree_parents) and fp64 operands:
+ * ARROW_ERR_UNSUPPORTED; mixed or wrong element types, bad shapes, aliasing, an unknown semiring
  * code: ARROW_ERR_ARG. */
 int  arrow_spmm_sr_witness(arrow_ctx *ctx, int csr, int x_buf, int row_labels, int val_out, int lab_out, int add_val,
                            int add_lab, int add_map, int dist_buf, int semiring);
