@@ -17,7 +17,7 @@ from oracle import oracle
 from tests import spmm_bound64 as sb
 from tests import tile_dispatch as td
 from tests.golden_util import GPU_CASES, GoldenCase
-from tests.spmm_bound import gamma, tree_height
+from tests.step_bound import abs_decomposition, bound_of, step_height
 from tests.test_gpu_kernels import assert_close
 
 pytestmark = pytest.mark.gpu
@@ -234,23 +234,18 @@ def test_mixed_and_multi_gpu_launches_are_refused(ctx):
 
 
 # ---- the engine ----------------------------------------------------------------------------------------------------
-def _abs_decomposition(dec):
-    return [(abs(sparse.csr_matrix(B)), p) for B, p in dec]
-
-
-def _step_height(po):
-    """an upper bound on the rounded operations any element of one step passes through: every level's tree
-    (tests/spmm_bound.py, which the float64 kernels share) plus the add that carries it to the level above"""
-    return sum(int(tree_height(np.diff(M.indptr)).max(initial=0)) + 1 for M in po.mats)
+def _bound64(mag, m):
+    """tests/step_bound.py's per-element step bound at the float64 unit roundoff"""
+    return bound_of(mag, m, u=sb.U64, eta=sb.ETA64, u_ref=sb.ULD)
 
 
 def _check_engine_steps(eng, dec, width, k, block_diagonal, X0, steps=3):
     """``steps`` chained steps, each against the extended-precision oracle started from the device's state"""
     po = oracle.ReferenceProtocolOracle(dec, width, k, block_diagonal=block_diagonal, n_blocks=eng.n_blocks,
                                         dtype=np.longdouble)
-    pa = oracle.ReferenceProtocolOracle(_abs_decomposition(dec), width, k, block_diagonal=block_diagonal,
+    pa = oracle.ReferenceProtocolOracle(abs_decomposition(dec), width, k, block_diagonal=block_diagonal,
                                         n_blocks=eng.n_blocks, dtype=np.longdouble)
-    m = _step_height(po)
+    m = step_height(po)
     eng.set_features(X0)
     for it in range(steps):
         x = eng.features(0).astype(np.longdouble) if it else X0.astype(np.longdouble)
@@ -264,7 +259,7 @@ def _check_engine_steps(eng, dec, width, k, block_diagonal, X0, steps=3):
         got = eng.result()
         assert got.dtype == np.float64
         exact, mag = po.step(), pa.step()
-        bound = (gamma(m, sb.U64) + gamma(m, sb.ULD)) * mag.astype(np.float64) + m * sb.ETA64
+        bound = _bound64(mag, m)
         err = np.abs(got.astype(np.longdouble) - exact).astype(np.float64)
         bad = ~(err <= bound)
         assert not bad.any(), (f"step {it} ({eng.mode}): {int(bad.sum())} elements outside the bound, worst ratio "
@@ -318,14 +313,13 @@ def test_surface_float64_end_to_end(cuda_device, tmp_path):
     X0 = np.random.default_rng(3).uniform(-1, 1, (eng.n_rows, k))
     arrow.B.set_features(X0)
     po = oracle.ReferenceProtocolOracle(dec, w, k, n_blocks=eng.n_blocks, dtype=np.longdouble)
-    pa = oracle.ReferenceProtocolOracle(_abs_decomposition(dec), w, k, n_blocks=eng.n_blocks, dtype=np.longdouble)
+    pa = oracle.ReferenceProtocolOracle(abs_decomposition(dec), w, k, n_blocks=eng.n_blocks, dtype=np.longdouble)
     po.set_features(X0.astype(np.longdouble))
     pa.set_features(np.abs(X0).astype(np.longdouble))
     arrow.step()
     got = arrow.B.result_tile()
     assert got.dtype == np.float64 and arrow.B.feature_tile().dtype == np.float64
-    m = _step_height(po)
-    bound = (gamma(m, sb.U64) + gamma(m, sb.ULD)) * pa.step().astype(np.float64) + m * sb.ETA64
+    bound = _bound64(pa.step(), step_height(po))
     assert (np.abs(got.astype(np.longdouble) - po.step()).astype(np.float64) <= bound).all()
     full = np.empty_like(got)
     arrow.B.allgather_result(full)

@@ -53,16 +53,26 @@ def _worker(rank, world, port, case, exchange, q):
             assert eng.fp is not None, eng.mode
         if exchange.endswith("+graph"):
             eng.use_graphs = True
+        from tests import step_bound as stb
+        from tests.test_gpu_step_bound import _assert_push_runs_identical, _push_option_runs
         po = oracle.ReferenceProtocolOracle(dec, w, k, block_diagonal=not banded)
         po64 = oracle.ReferenceProtocolOracle(dec, w, k, block_diagonal=not banded, dtype=np.float64)
+        # the fused step (no state behind the sentinel) is also held to the per-element bound of tests/step_bound.py,
+        # every step started from the device's own level-0 rows of all ranks
+        ex = stb.ExactStep(dec, w, k, block_diagonal=not banded, world=world) if eng.fp is not None else None
+        comm = world_comm()
         rng = np.random.default_rng(2)
         sh0 = eng.plan.levels[0]
+        x_dev = None
         for it in range(3):
             X = synth.generate_dense_matrix(t0 * w, k, np.float32, rng)
             if it != 1:                                     # iteration 1 is chained (X := A X)
                 arrow.B.set_features(X[sh0.r0:sh0.r1])
                 po.set_features(X.copy())
                 po64.set_features(X)
+                x_dev = X
+            if ex is not None:
+                exact, mag = ex.run(x_dev)
             arrow.step()
             po.step()
             po64.step()
@@ -70,6 +80,14 @@ def _worker(rank, world, port, case, exchange, q):
                 sh = eng.plan.levels[j]
                 close_rows(eng.result(j), po.C[j], po64.C[j], sh.r0, sh.r1)
             po64.C[0][:] = po.C[0]                          # the chained product starts from the same point in both
+            if ex is not None:
+                got = eng.result(0)
+                r0, r1 = sh0.r0, sh0.r1
+                stb.assert_step(got, exact[r0:r1], mag[r0:r1], ex.M[r0:r1], route=f"{case} {exchange} world {world} step {it}",
+                                row0=r0)
+                x_dev = np.concatenate(comm.allgather(got))
+        if eng.fp is not None:                              # the push schedule options move the same rows: same bits
+            _assert_push_runs_identical(_push_option_runs(eng, X[sh0.r0:sh0.r1]), f"{case} {exchange} rank {rank}")
         arrow.synchronize()
         dist.barrier()
         dist.destroy_process_group()
