@@ -55,8 +55,9 @@ EXPORTS = [
     "arrow_adj_keep_record", "arrow_bits_dependencies", "arrow_bits_fill_f64", "arrow_dense_row_sum",
     "arrow_adj_build_loopfree", "arrow_wpaths_counts", "arrow_wpaths_dependencies",
     "arrow_sr_mark_frontier_steps", "arrow_sr_tree_parents", "arrow_dense_count_diff_bits",
+    "arrow_out_weights", "arrow_csr_scale_columns", "arrow_pagerank_restart", "arrow_pagerank_update",
 ]
-ABI_VERSION = 13       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 14       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -181,6 +182,10 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_sr_mark_frontier_steps": (c_int, [P, I, I, I, I, I, pI64, pI64, pI64]),
         "arrow_sr_tree_parents": (c_int, [P, I, I, I, I, I, pI64]),
         "arrow_dense_count_diff_bits": (c_int, [P, I, I, pI64]),
+        "arrow_out_weights": (c_int, [P, I, pI, pI, I64, I, I, pI64, pI64, pI64]),
+        "arrow_csr_scale_columns": (c_int, [P, I, I, I, pI]),
+        "arrow_pagerank_restart": (c_int, [P, I, I, I, I, I, POINTER(c_double), pI64, pI64]),
+        "arrow_pagerank_update": (c_int, [P, I, I, I, I, I, I, c_double, POINTER(c_double)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -635,6 +640,38 @@ class Context:
                                                    byref(n) if count else None))
         return int(n.value) if count else None
 
+    def out_weights(self, parts: Sequence[tuple], n_vertices: int, w: "Dense", inv: "Dense") -> Tuple[int, int, int]:
+        """Out-weights of the operator of ``adj_build(parts, n_vertices)`` with its self-loops (``arrow_out_weights``):
+        ``w`` (float64 [n x 1]) receives the float64 sum of each source's edge values in (part, entry) order, ``inv`` (the
+        blocks' type, [n x 1]) fl(1 / w), 0 where w == 0.  Returns (edges with a negative, NaN or +-inf value, dangling
+        vertices, other vertices whose inverse is not finite or 0); synchronises."""
+        n = len(parts)
+        csrs = (c_int * max(n, 1))(*[A.h for A, _ in parts])
+        maps = (c_int * max(n, 1))(*[m.h if m is not None else -1 for _, m in parts])
+        bad, dangling, bad_inv = c_int64(), c_int64(), c_int64()
+        self._check(self.lib.arrow_out_weights(self._h, n, csrs, maps, int(n_vertices), w.h, inv.h, byref(bad), byref(dangling),
+                                               byref(bad_inv)))
+        return int(bad.value), int(dangling.value), int(bad_inv.value)
+
+    def pagerank_restart(self, x: "Dense", inv: "Dense", s: "Dense", scratch: "Dense", state: "Dense") -> Tuple[np.ndarray, int, int]:
+        """sigma = the chunked float64 column sums of ``x``; when no column is bad (a negative, NaN or +-inf value, or a
+        sigma that is not positive and finite) ``s`` = fl(x / sigma) and state row 0 the dangling mass of ``s``
+        (``arrow_pagerank_restart``).  Returns (sigma, bad columns, first bad column or -1); synchronises."""
+        sums = np.zeros(x.k, np.float64)
+        bad, first = c_int64(), c_int64()
+        self._check(self.lib.arrow_pagerank_restart(self._h, x.h, inv.h, s.h, scratch.h, state.h,
+                                                    sums.ctypes.data_as(POINTER(c_double)), byref(bad), byref(first)))
+        return sums, int(bad.value), int(first.value)
+
+    def pagerank_update(self, y: "Dense", p: "Dense", s: "Dense", inv: "Dense", scratch: "Dense", state: "Dense",
+                        alpha: float) -> np.ndarray:
+        """p_{t+1} = fl(fl(alpha Y) + fl(c S)) over ``y`` in place, c = fl(fl(1 - alpha) + fl(alpha m_t)); returns the
+        float64 residuals sum |p_{t+1} - p_t| per column (``arrow_pagerank_update``); synchronises"""
+        res = np.zeros(y.k, np.float64)
+        self._check(self.lib.arrow_pagerank_update(self._h, y.h, p.h, s.h, inv.h, scratch.h, state.h, float(alpha),
+                                                   res.ctypes.data_as(POINTER(c_double))))
+        return res
+
     def count_diff(self, a: "Dense", b: "Dense") -> int:
         """rows in which two equally shaped tiles differ in some element (-0 == +0, NaN != NaN); synchronises"""
         n = c_int64()
@@ -733,6 +770,16 @@ class Csr(_Handle):
         self.ctx._check(self.ctx.lib.arrow_csr_remap_columns(self.ctx._h, self.h, m.h, int(new_n_cols), byref(h)))
         out = Csr(self.ctx, h.value, self.n_rows, int(new_n_cols), self.nnz, self.dtype)
         out._parent = self           # shares indptr/values: keep the source alive
+        return out
+
+    def scale_columns(self, scale: "Dense", m: Optional["RowMap"] = None) -> "Csr":
+        """a values-only copy whose entry (r, c) holds fl(a * scale[m(c)]) (``arrow_csr_scale_columns``; ``m`` None: the
+        identity); it shares this block's structure, so this block cannot be freed while the copy lives"""
+        h = c_int()
+        self.ctx._check(self.ctx.lib.arrow_csr_scale_columns(self.ctx._h, self.h, m.h if m is not None else -1, scale.h,
+                                                             byref(h)))
+        out = Csr(self.ctx, h.value, self.n_rows, self.n_cols, self.nnz, self.dtype)
+        out._parent = self
         return out
 
     def free(self):

@@ -225,6 +225,12 @@ class ArrowDecompositionMPI:
         permutation maps the parents to vertex ids like the rows."""
         return self._bfs_engine("bottleneck_tree").bottleneck_tree(max_steps, distances_out, parents_out)
 
+    def pagerank(self, max_steps: int, alpha: float = 0.85, tol: float = 1e-6, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension (one GPU, ``plus_times``): personalized PageRank with one restart distribution per feature column,
+        in ``result_tile()`` row order (see ``ArrowEngine.pagerank``).  Level 0's permutation maps the rows to vertex
+        ids."""
+        return self._bfs_engine("pagerank").pagerank(max_steps, alpha, tol, out)
+
     def _bfs_engine(self, what: str) -> ArrowEngine:
         if self.comm.Get_size() > 1:
             raise ValueError(f"{what} runs on one GPU only")

@@ -27,6 +27,7 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <mutex>
 #include <type_traits>
@@ -4288,6 +4289,235 @@ int spmm_wit(arrow_ctx *ctx, const Csr *A, WitArgs &w, bool min_plus) {
 
 }  // namespace
 
+// ------------------------------------------------------------------------------------------------
+// personalized PageRank (one GPU, plus-times, float32 or float64).  The walk steps with the engine's own SpMM on a
+// values-only copy of every block whose entries are divided by their source's out-weight; the passes here build those
+// weights and copies, normalise the restart columns and fold one step into the next iterate.  Every column reduction
+// (sigma, dangling mass, residual) runs in float64 over fixed PR_CHUNK-row chunks from row 0: sequential in ascending
+// rows inside a chunk, the chunk partials then added in ascending chunk order by one thread per column.  No
+// floating-point atomics, so the results depend neither on the grid nor on the schedule.
+// ------------------------------------------------------------------------------------------------
+namespace {
+constexpr int PR_CHUNK = 512;
+
+inline long long pr_chunks(long long n) { return (n + PR_CHUNK - 1) / PR_CHUNK; }
+
+__device__ __forceinline__ double pr_mul(float a, float b) { return (double)__fmul_rn(a, b); }
+__device__ __forceinline__ double pr_mul(double a, double b) { return __dmul_rn(a, b); }
+
+// one key per entry of a part, at its (part, entry) slot: the level-0 source u = map(c) of the edge map(c) -> map(r), or
+// n_vertices when the entry is not an edge of M (c < 0 or an end at -1); the value goes beside it as float64.  Counts the
+// edges whose value is negative, NaN or +-inf (-0 is allowed) with one integer atomic per warp.
+template <class T>
+__global__ void __launch_bounds__(256) k_pr_out_keys(AdjPart p, const T *__restrict__ vals, int n_vertices,
+                                                     int *__restrict__ keys, double *__restrict__ w_out,
+                                                     unsigned long long *__restrict__ bad) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    unsigned nbad = 0;
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < p.nnz; e += stride) {
+        const int c = __ldg(p.indices + e);
+        int u = n_vertices;
+        if (c >= 0) {
+            const int r = last_le(p.indptr, 0, p.n_rows - 1, e);
+            const int src = p.map ? __ldg(p.map + c) : c;
+            const int dst = p.map ? __ldg(p.map + r) : r;
+            if (src >= 0 && dst >= 0) u = src;
+        }
+        const double a = (double)vals[e];
+        keys[e] = u;
+        w_out[e] = a;
+        if (u < n_vertices && !(a >= 0.0 && a <= 1.7976931348623157e308)) ++nbad;
+    }
+    for (int o = 16; o > 0; o >>= 1) nbad += __shfl_xor_sync(0xffffffffu, nbad, o);
+    if ((threadIdx.x & 31) == 0 && nbad) atomicAdd(bad, (unsigned long long)nbad);
+}
+
+__device__ __forceinline__ long long pr_lower_bound(const int *__restrict__ keys, long long m, int want) {
+    long long lo = 0, hi = m;
+    while (lo < hi) {
+        const long long mid = (lo + hi) >> 1;
+        if (keys[mid] < want) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// w[u] = the sequential float64 sum (from +0) of the values of u's entries in (part, entry) order -- the stable sort kept
+// it -- and inv[u] = fl_T(1 / w[u]), 0 where w[u] == 0 (dangling).  counts[0] gets the dangling vertices, counts[1] the
+// others whose inverse is not finite or 0.
+template <class T>
+__global__ void __launch_bounds__(256) k_pr_out_sums(const int *__restrict__ keys, const double *__restrict__ vals, long long m,
+                                                     long long n, double *__restrict__ w, T *__restrict__ inv,
+                                                     unsigned long long *__restrict__ counts) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    unsigned dangling = 0, bad = 0;
+    for (long long u = (long long)blockIdx.x * blockDim.x + threadIdx.x; u < n; u += stride) {
+        const long long lo = pr_lower_bound(keys, m, (int)u), hi = pr_lower_bound(keys, m, (int)u + 1);
+        double acc = 0.0;
+        for (long long e = lo; e < hi; ++e) acc = __dadd_rn(acc, vals[e]);
+        T q = (T)0;
+        if (acc == 0.0) {
+            ++dangling;
+        } else {
+            q = (T)__ddiv_rn(1.0, acc);
+            if (!isfinite((double)q) || q == (T)0) ++bad;
+        }
+        w[u] = acc;
+        inv[u] = q;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        dangling += __shfl_xor_sync(0xffffffffu, dangling, o);
+        bad += __shfl_xor_sync(0xffffffffu, bad, o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+        if (dangling) atomicAdd(counts, (unsigned long long)dangling);
+        if (bad) atomicAdd(counts + 1, (unsigned long long)bad);
+    }
+}
+
+// out[e] = fl_T(a_e * scale[map(c_e)]) (map nullptr: the identity); 0 for an entry whose column is -1 or maps to -1
+template <class T>
+__global__ void __launch_bounds__(256) k_pr_scale(const int *__restrict__ indices, const T *__restrict__ vals,
+                                                  const int *__restrict__ map, const T *__restrict__ scale, T *__restrict__ out,
+                                                  long long nnz) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
+        const int c = __ldg(indices + e);
+        const int u = c < 0 ? -1 : (map ? __ldg(map + c) : c);
+        out[e] = u < 0 ? (T)0 : (T)pr_mul(vals[e], __ldg(scale + u));
+    }
+}
+
+// chunk partials of the restart, one thread per (chunk, column), chunk-major so that a warp reads adjacent columns of one
+// row: part[s][b] = the sum of X[v, s] over the chunk's rows, part[k + s][b] = 1 where a value is negative, NaN or +-inf
+template <class T>
+__global__ void __launch_bounds__(256) k_pr_restart_partials(const T *__restrict__ X, long long n, int k, long long nch,
+                                                             double *__restrict__ part) {
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < nch * k; t += (long long)gridDim.x * blockDim.x) {
+        const long long b = t / k;
+        const int s = (int)(t - b * k);
+        const long long v1 = min(n, (b + 1) * PR_CHUNK);
+        double acc = 0.0;
+        bool bad = false;
+#pragma unroll 8
+        for (long long v = b * PR_CHUNK; v < v1; ++v) {
+            const double x = (double)X[v * k + s];
+            acc = __dadd_rn(acc, x);
+            bad |= !(x >= 0.0 && x <= 1.7976931348623157e308);
+        }
+        part[(long long)s * nch + b] = acc;
+        part[(long long)(k + s) * nch + b] = bad ? 1.0 : 0.0;
+    }
+}
+
+// S[v, s] = fl_T(X[v, s] / sigma_s) with sigma from the state tile's row 2; part[s][b] = the chunk's dangling mass of S
+template <class T>
+__global__ void __launch_bounds__(256) k_pr_restart_write(const T *__restrict__ X, const T *__restrict__ inv,
+                                                          const double *__restrict__ state, T *__restrict__ S, long long n,
+                                                          int k, long long nch, double *__restrict__ part) {
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < nch * k; t += (long long)gridDim.x * blockDim.x) {
+        const long long b = t / k;
+        const int s = (int)(t - b * k);
+        const double sigma = state[2 * k + s];
+        const long long v1 = min(n, (b + 1) * PR_CHUNK);
+        double m = 0.0;
+#pragma unroll 8
+        for (long long v = b * PR_CHUNK; v < v1; ++v) {
+            const T q = (T)__ddiv_rn((double)X[v * k + s], sigma);
+            S[v * k + s] = q;
+            if (__ldg(inv + v) == (T)0) m = __dadd_rn(m, (double)q);
+        }
+        part[(long long)s * nch + b] = m;
+    }
+}
+
+// one step's update, one thread per (chunk, column): with c = fl(beta + fl(alpha * m_t[s])) (m_t in the state tile's row 0)
+// p_{t+1} = fl_T(fl(fl(alpha * Y) + fl(c * S))) over Y in place; part[s][b] = the chunk's dangling mass of p_{t+1},
+// part[k + s][b] = its sum of |fl(p_{t+1} - p_t)|.  Separately rounded float64 operations, no contraction.
+template <class T>
+__global__ void __launch_bounds__(256) k_pr_update(T *__restrict__ Y, const T *__restrict__ P, const T *__restrict__ S,
+                                                   const T *__restrict__ inv, const double *__restrict__ state, double alpha,
+                                                   double beta, long long n, int k, long long nch, double *__restrict__ part) {
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < nch * k; t += (long long)gridDim.x * blockDim.x) {
+        const long long b = t / k;
+        const int s = (int)(t - b * k);
+        const double c = __dadd_rn(beta, __dmul_rn(alpha, state[s]));
+        const long long v1 = min(n, (b + 1) * PR_CHUNK);
+        double m = 0.0, r = 0.0;
+#pragma unroll 8
+        for (long long v = b * PR_CHUNK; v < v1; ++v) {
+            const long long i = v * k + s;
+            const T q = (T)__dadd_rn(__dmul_rn(alpha, (double)Y[i]), __dmul_rn(c, (double)__ldg(S + i)));
+            const double old = (double)__ldg(P + i);
+            Y[i] = q;
+            r = __dadd_rn(r, fabs(__dsub_rn((double)q, old)));
+            if (__ldg(inv + v) == (T)0) m = __dadd_rn(m, (double)q);
+        }
+        part[(long long)s * nch + b] = m;
+        part[(long long)(k + s) * nch + b] = r;
+    }
+}
+
+// out[q] = part[q][0] + part[q][1] + ... + part[q][nch - 1], left to right from +0: one CTA per row q, which stages the
+// row through shared memory and sums it on one thread
+__global__ void __launch_bounds__(256) k_pr_chunk_sums(const double *__restrict__ part, long long nch, double *__restrict__ out) {
+    constexpr int STAGE = 2048;
+    __shared__ double buf[STAGE];
+    const double *row = part + (long long)blockIdx.x * nch;
+    double acc = 0.0;
+    for (long long b0 = 0; b0 < nch; b0 += STAGE) {
+        const int len = (int)min((long long)STAGE, nch - b0);
+        for (int i = threadIdx.x; i < len; i += blockDim.x) buf[i] = row[b0 + i];
+        __syncthreads();
+        if (threadIdx.x == 0)
+            for (int i = 0; i < len; ++i) acc = __dadd_rn(acc, buf[i]);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) out[blockIdx.x] = acc;
+}
+
+// the tiles of the restart / update passes: x (or y), p and S of one element type T [n x k], inv T [n x 1], scratch float64
+// [pr_chunks(n) x 2k], state float64 [4 x k]; the restart has no p (x_buf is then X0)
+int pr_tiles(arrow_ctx *ctx, const char *fn, bool restart, int x_buf, int p_buf, int s_buf, int inv_buf, int scratch_buf,
+             int state_buf, DenseBuf *t[6]) {
+    const int h[6] = {x_buf, p_buf, s_buf, inv_buf, scratch_buf, state_buf};
+    const char *name[6] = {restart ? "x" : "y", "p", "s", "inv", "scratch", "state"};
+    for (int i = 0; i < 6; ++i) {
+        t[i] = nullptr;
+        if (i == 1 && restart) continue;
+        t[i] = get_dense(ctx, h[i]);
+        if (!t[i]) return fail(ctx, ARROW_ERR_HANDLE, "%s: bad dense handle %s=%d", fn, name[i], h[i]);
+    }
+    const int T = t[0]->dtype;
+    if (T != ARROW_F32 && T != ARROW_F64) return fail(ctx, ARROW_ERR_ARG, "%s: %s is a %s tile, expected float32 or float64", fn, name[0], dtype_name(T));
+    const long long n = t[0]->rows;
+    const int k = t[0]->k;
+    const long long want_rows[6] = {n, n, n, n, pr_chunks(n), 4};
+    const int want_k[6] = {k, k, k, 1, 2 * k, k};
+    for (int i = 0; i < 6; ++i) {
+        if (!t[i]) continue;
+        const int want = i >= 4 ? ARROW_F64 : T;
+        if (t[i]->dtype != want)
+            return fail(ctx, ARROW_ERR_ARG, "%s: %s is a %s tile, expected %s", fn, name[i], dtype_name(t[i]->dtype), dtype_name(want));
+        if (t[i]->rows != want_rows[i] || t[i]->k != want_k[i])
+            return fail(ctx, ARROW_ERR_ARG, "%s: %s is %lld x %d, expected %lld x %d", fn, name[i], (long long)t[i]->rows, t[i]->k,
+                        want_rows[i], want_k[i]);
+        for (int j = 0; j < i; ++j)
+            if (t[j] && (h[j] == h[i] || t[j]->p == t[i]->p)) return fail(ctx, ARROW_ERR_ARG, "%s: %s aliases %s", fn, name[i], name[j]);
+    }
+    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "%s synchronises: not during graph capture", fn);
+    return ARROW_OK;
+}
+
+// grid of the chunk passes (grid-stride over (chunk, column) items): ARROW_OPT_SPMM_SM_LIMIT and ARROW_OPT_SPMM_CTAS_PER_SM cap
+// it as they cap a SpMM grid; the results do not depend on it
+int pr_grid(const arrow_ctx *ctx, long long items) {
+    const long long sms = ctx->spmm_sm_limit > 0 ? std::min(ctx->spmm_sm_limit, ctx->sm_count) : ctx->sm_count;
+    const long long per_sm = ctx->spmm_ctas_per_sm > 0 ? ctx->spmm_ctas_per_sm : 8;
+    return (int)std::max<long long>(1, std::min<long long>((items + 255) / 256, sms * per_sm));
+}
+}  // namespace
+
 // ================================================================================================
 // C ABI
 // ================================================================================================
@@ -6427,6 +6657,248 @@ int arrow_sr_tree_parents(arrow_ctx *ctx, int in_adj, int dist_buf, int steps_bu
     }, false);                                                // the hits fold into P: no segment partials
     if (rc) return rc;
     return read_scanned(ctx, cnt, entries_read);
+}
+
+int arrow_out_weights(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int w_buf, int inv_buf,
+                      int64_t *bad_entries, int64_t *dangling, int64_t *bad_inverses) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    if (n_parts < 0 || (n_parts > 0 && (!csrs || !maps)) || n_vertices < 0)
+        return fail(ctx, ARROW_ERR_ARG, "bad arguments (n_parts=%d, n_vertices=%lld)", n_parts, (long long)n_vertices);
+    if (n_vertices > 2147483646LL) return fail(ctx, ARROW_ERR_RANGE, "%lld vertices exceed the int32 device layout", (long long)n_vertices);
+    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_out_weights allocates and synchronises: not during graph capture");
+    DenseBuf *W = get_dense(ctx, w_buf), *I = get_dense(ctx, inv_buf);
+    if (!W || !I) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (w=%d inv=%d)", w_buf, inv_buf);
+    int T = -1;
+    std::vector<AdjPart> parts;
+    std::vector<const void *> vals;
+    long long m = 0;
+    for (int i = 0; i < n_parts; ++i) {
+        const Csr *c = get_csr(ctx, csrs[i]);
+        if (!c) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad csr handle %d", i, csrs[i]);
+        if (T >= 0 && c->dtype != T) return fail(ctx, ARROW_ERR_ARG, "part %d is %s, part 0 %s", i, dtype_name(c->dtype), dtype_name(T));
+        T = c->dtype;
+        const IdxMap *mp = nullptr;
+        if (maps[i] != -1) {
+            mp = get_map(ctx, maps[i]);
+            if (!mp) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad map handle %d", i, maps[i]);
+            if (mp->n < std::max(c->n_rows, c->n_cols))
+                return fail(ctx, ARROW_ERR_ARG, "part %d: the map has %lld entries, the block %lld rows and %lld columns", i,
+                            (long long)mp->n, (long long)c->n_rows, (long long)c->n_cols);
+            if (mp->limit > n_vertices)
+                return fail(ctx, ARROW_ERR_ARG, "part %d: the map reaches row %lld, there are %lld vertices", i, (long long)mp->limit,
+                            (long long)n_vertices);
+        } else if (c->n_rows > n_vertices || c->n_cols > n_vertices) {
+            return fail(ctx, ARROW_ERR_ARG, "part %d: a %lld x %lld block with the identity map exceeds %lld vertices", i,
+                        (long long)c->n_rows, (long long)c->n_cols, (long long)n_vertices);
+        }
+        if (c->nnz > 0 && !c->vals) return fail(ctx, ARROW_ERR_ARG, "part %d: the block has no values", i);
+        if (c->nnz > 0) {
+            parts.push_back(AdjPart{c->indptr, c->indices, mp ? mp->p : nullptr, (long long)c->nnz, (int)c->n_rows});
+            vals.push_back(c->vals);
+            m += c->nnz;
+        }
+    }
+    if (T < 0) T = I->dtype;
+    if (W->dtype != ARROW_F64 || I->dtype != T || W->rows != n_vertices || I->rows != n_vertices || W->k != 1 || I->k != 1)
+        return fail(ctx, ARROW_ERR_ARG, "w is float64 and inv %s, both %lld x 1: got %s %lld x %d and %s %lld x %d", dtype_name(T),
+                    (long long)n_vertices, dtype_name(W->dtype), (long long)W->rows, W->k, dtype_name(I->dtype), (long long)I->rows, I->k);
+    if (T != ARROW_F32 && T != ARROW_F64) return fail(ctx, ARROW_ERR_ARG, "inv is a %s tile, expected float32 or float64", dtype_name(T));
+    if (W->p == I->p) return fail(ctx, ARROW_ERR_ARG, "inv aliases w");
+    if (m > 2147483647LL) return fail(ctx, ARROW_ERR_RANGE, "%lld entries exceed the int32 sort layout", m);
+    cudaStream_t s = ctx->stream;
+    auto grid = [&](long long items) { return (int)std::max<long long>(1, std::min<long long>((items + 255) / 256, (long long)ctx->sm_count * 8)); };
+    // 24 bytes per entry (key and float64 value, twice) and the sort's temporary storage
+    DevTmp cnt, keys, alt, wv, walt, temp;
+    unsigned long long h_cnt[3] = {0, 0, 0};
+    cudaError_t e = cudaMalloc(&cnt.p, sizeof h_cnt);
+    if (e == cudaSuccess) e = cudaMemsetAsync(cnt.p, 0, sizeof h_cnt, s);
+    unsigned long long *dc = reinterpret_cast<unsigned long long *>(cnt.p);
+    if (e == cudaSuccess && m > 0) {
+        e = cudaMalloc(&keys.p, (size_t)m * 4);
+        if (e == cudaSuccess) e = cudaMalloc(&alt.p, (size_t)m * 4);
+        if (e == cudaSuccess) e = cudaMalloc(&wv.p, (size_t)m * 8);
+        if (e == cudaSuccess) e = cudaMalloc(&walt.p, (size_t)m * 8);
+        long long off = 0;
+        for (size_t i = 0; e == cudaSuccess && i < parts.size(); ++i) {
+            int *kp = reinterpret_cast<int *>(keys.p) + off;
+            double *vp = reinterpret_cast<double *>(wv.p) + off;
+            if (T == ARROW_F64)
+                k_pr_out_keys<double><<<grid(parts[i].nnz), 256, 0, s>>>(parts[i], (const double *)vals[i], (int)n_vertices, kp, vp, dc + 2);
+            else
+                k_pr_out_keys<float><<<grid(parts[i].nnz), 256, 0, s>>>(parts[i], (const float *)vals[i], (int)n_vertices, kp, vp, dc + 2);
+            ctx->launches++;
+            off += parts[i].nnz;
+            e = cudaGetLastError();
+        }
+        int end_bit = 1;                                          // keys lie in [0, n_vertices]
+        while ((1LL << end_bit) <= n_vertices) ++end_bit;
+        cub::DoubleBuffer<int> db(reinterpret_cast<int *>(keys.p), reinterpret_cast<int *>(alt.p));
+        cub::DoubleBuffer<double> dv(reinterpret_cast<double *>(wv.p), reinterpret_cast<double *>(walt.p));
+        size_t temp_bytes = 0;
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, db, dv, (int)m, 0, end_bit, s);
+        if (e == cudaSuccess) e = cudaMalloc(&temp.p, std::max<size_t>(temp_bytes, 1));
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(temp.p, temp_bytes, db, dv, (int)m, 0, end_bit, s);
+        if (e == cudaSuccess && n_vertices > 0) {
+            if (T == ARROW_F64)
+                k_pr_out_sums<double><<<grid(n_vertices), 256, 0, s>>>(db.Current(), dv.Current(), m, n_vertices, (double *)W->p,
+                                                                       (double *)I->p, dc);
+            else
+                k_pr_out_sums<float><<<grid(n_vertices), 256, 0, s>>>(db.Current(), dv.Current(), m, n_vertices, (double *)W->p,
+                                                                      I->p, dc);
+            ctx->launches++;
+            e = cudaGetLastError();
+        }
+    } else if (e == cudaSuccess && n_vertices > 0) {          // no entries: every vertex is dangling
+        if (T == ARROW_F64)
+            k_pr_out_sums<double><<<grid(n_vertices), 256, 0, s>>>(nullptr, nullptr, 0, n_vertices, (double *)W->p, (double *)I->p, dc);
+        else
+            k_pr_out_sums<float><<<grid(n_vertices), 256, 0, s>>>(nullptr, nullptr, 0, n_vertices, (double *)W->p, I->p, dc);
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_cnt, cnt.p, sizeof h_cnt, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(ctx, e == cudaErrorMemoryAllocation ? ARROW_ERR_NOMEM : ARROW_ERR_CUDA, "out-weight pass failed: %s",
+                    cudaGetErrorString(e));
+    }
+    if (dangling) *dangling = (int64_t)h_cnt[0];
+    if (bad_inverses) *bad_inverses = (int64_t)h_cnt[1];
+    if (bad_entries) *bad_entries = (int64_t)h_cnt[2];
+    return ARROW_OK;
+}
+
+int arrow_csr_scale_columns(arrow_ctx *ctx, int csr, int map, int scale_buf, int *csr_out) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    Csr *c = get_csr(ctx, csr);
+    if (!c) return fail(ctx, ARROW_ERR_HANDLE, "bad csr handle %d", csr);
+    if (!csr_out) return fail(ctx, ARROW_ERR_ARG, "csr_out is null");
+    const IdxMap *m = nullptr;
+    if (map != -1 && !(m = get_map(ctx, map))) return fail(ctx, ARROW_ERR_HANDLE, "bad map handle %d", map);
+    DenseBuf *S = get_dense(ctx, scale_buf);
+    if (!S) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle scale=%d", scale_buf);
+    if (S->dtype != c->dtype || S->k != 1)
+        return fail(ctx, ARROW_ERR_ARG, "scale is a %s tile of %d columns, expected %s x 1", dtype_name(S->dtype), S->k, dtype_name(c->dtype));
+    if (m ? (m->n < c->n_cols || m->limit > S->rows) : c->n_cols > S->rows)
+        return fail(ctx, ARROW_ERR_ARG, "the block's %lld columns%s reach past the %lld scale rows", (long long)c->n_cols,
+                    m ? " mapped" : "", (long long)S->rows);
+    if (c->nnz > 0 && !c->vals) return fail(ctx, ARROW_ERR_ARG, "the block has no values to scale");
+    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_csr_scale_columns allocates: not during graph capture");
+    Csr d = *c;
+    d.owns_indptr = d.owns_indices = d.owns_long = false;     // shared with the source block (and its own source)
+    d.owns_vals = true;
+    d.vals = nullptr;
+    d.parent = csr;
+    d.children = 0;
+    const size_t esz = dtype_size(c->dtype);
+    CUDA_TRY(ctx, cudaMalloc(&d.vals, ((size_t)c->nnz + 8) * esz));
+    cudaError_t e = cudaSuccess;
+    if (c->nnz > 0) {
+        const int grid = (int)std::min<long long>((c->nnz + 255) / 256, (long long)ctx->sm_count * 8);
+        if (c->dtype == ARROW_F64)
+            k_pr_scale<double><<<grid, 256, 0, ctx->stream>>>(c->indices, (const double *)c->vals, m ? m->p : nullptr,
+                                                              (const double *)S->p, (double *)d.vals, c->nnz);
+        else
+            k_pr_scale<float><<<grid, 256, 0, ctx->stream>>>(c->indices, c->vals, m ? m->p : nullptr, S->p, d.vals, c->nnz);
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) {
+        cudaFree(d.vals);
+        return fail(ctx, ARROW_ERR_CUDA, "column scaling failed: %s", cudaGetErrorString(e));
+    }
+    const int h = new_slot(ctx->csrs);       // may grow the table: `c` is not used past this point
+    ctx->csrs[h] = d;
+    ctx->csrs[csr].children++;
+    *csr_out = h;
+    return ARROW_OK;
+}
+
+int arrow_pagerank_restart(arrow_ctx *ctx, int x_buf, int inv_buf, int s_buf, int scratch_buf, int state_buf, double *col_sums,
+                           int64_t *bad_columns, int64_t *first_bad_column) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    DenseBuf *t[6];
+    if (const int rc = pr_tiles(ctx, "arrow_pagerank_restart", true, x_buf, -1, s_buf, inv_buf, scratch_buf, state_buf, t)) return rc;
+    const long long n = t[0]->rows, nch = pr_chunks(n);
+    const int k = t[0]->k;
+    const bool f64 = t[0]->dtype == ARROW_F64;
+    double *part = reinterpret_cast<double *>(t[4]->p), *state = reinterpret_cast<double *>(t[5]->p);
+    cudaStream_t s = cur_stream(ctx);
+    if (k == 0) {
+        if (bad_columns) *bad_columns = 0;
+        if (first_bad_column) *first_bad_column = -1;
+        return ARROW_OK;
+    }
+    if (nch > 0) {
+        if (f64) k_pr_restart_partials<double><<<pr_grid(ctx, nch * k), 256, 0, s>>>((const double *)t[0]->p, n, k, nch, part);
+        else k_pr_restart_partials<float><<<pr_grid(ctx, nch * k), 256, 0, s>>>(t[0]->p, n, k, nch, part);
+        ctx->launches++;
+    }
+    k_pr_chunk_sums<<<2 * k, 256, 0, s>>>(part, nch, state + 2 * k);      // rows 2 (sigma) and 3 (bad flags)
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    std::vector<double> h((size_t)2 * k);
+    CUDA_TRY(ctx, cudaMemcpyAsync(h.data(), state + 2 * k, h.size() * 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    int64_t bad = 0, first = -1;
+    for (int c = 0; c < k; ++c) {
+        const double sigma = h[c];
+        if (h[k + c] != 0.0 || !(sigma > 0.0) || !std::isfinite(sigma)) {
+            if (first < 0) first = c;
+            ++bad;
+        }
+    }
+    if (col_sums) memcpy(col_sums, h.data(), (size_t)k * 8);
+    if (bad_columns) *bad_columns = bad;
+    if (first_bad_column) *first_bad_column = first;
+    if (bad > 0) return ARROW_OK;
+    if (nch > 0) {
+        if (f64)
+            k_pr_restart_write<double><<<pr_grid(ctx, nch * k), 256, 0, s>>>((const double *)t[0]->p, (const double *)t[3]->p, state,
+                                                                        (double *)t[2]->p, n, k, nch, part);
+        else
+            k_pr_restart_write<float><<<pr_grid(ctx, nch * k), 256, 0, s>>>(t[0]->p, t[3]->p, state, t[2]->p, n, k, nch, part);
+        ctx->launches++;
+    }
+    k_pr_chunk_sums<<<k, 256, 0, s>>>(part, nch, state);                  // row 0: m_0
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    return ARROW_OK;
+}
+
+int arrow_pagerank_update(arrow_ctx *ctx, int y_buf, int p_buf, int s_buf, int inv_buf, int scratch_buf, int state_buf,
+                          double alpha, double *residuals) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    if (!(alpha >= 0.0 && alpha < 1.0)) return fail(ctx, ARROW_ERR_ARG, "alpha = %g lies outside [0, 1)", alpha);
+    DenseBuf *t[6];
+    if (const int rc = pr_tiles(ctx, "arrow_pagerank_update", false, y_buf, p_buf, s_buf, inv_buf, scratch_buf, state_buf, t))
+        return rc;
+    const long long n = t[0]->rows, nch = pr_chunks(n);
+    const int k = t[0]->k;
+    if (k == 0) return ARROW_OK;
+    const double beta = 1.0 - alpha;
+    double *part = reinterpret_cast<double *>(t[4]->p), *state = reinterpret_cast<double *>(t[5]->p);
+    cudaStream_t s = cur_stream(ctx);
+    if (nch > 0) {
+        if (t[0]->dtype == ARROW_F64)
+            k_pr_update<double><<<pr_grid(ctx, nch * k), 256, 0, s>>>((double *)t[0]->p, (const double *)t[1]->p, (const double *)t[2]->p,
+                                                                 (const double *)t[3]->p, state, alpha, beta, n, k, nch, part);
+        else
+            k_pr_update<float><<<pr_grid(ctx, nch * k), 256, 0, s>>>(t[0]->p, t[1]->p, t[2]->p, t[3]->p, state, alpha, beta, n, k, nch, part);
+        ctx->launches++;
+    }
+    k_pr_chunk_sums<<<2 * k, 256, 0, s>>>(part, nch, state);              // rows 0 (m_{t+1}) and 1 (r_{t+1})
+    ctx->launches++;
+    CUDA_TRY(ctx, cudaGetLastError());
+    if (residuals) CUDA_TRY(ctx, cudaMemcpyAsync(residuals, state + k, (size_t)k * 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    return ARROW_OK;
 }
 
 int arrow_gather_rows_multi(arrow_ctx *ctx, int dst_buf, const int *src_bufs, const int64_t *row_bounds, int n_src, int map, int flags) {

@@ -179,6 +179,11 @@ class ArrowEngine:
         self.last_path_rounds = 0                                # tight-DAG rounds of the last weighted path call
         self._bt_in_adj: Optional[_lib.Adjacency] = None         # bottleneck_tree(): the loop-free in-adjacency
         self._bt_tiles: Optional[Tuple[_lib.Dense, ...]] = None  # bottleneck_tree(): int32 steps and parent tiles
+        self._pr_weights: Optional[Tuple[_lib.Dense, _lib.Dense]] = None   # pagerank(): out-weights w and inverses inv
+        self._pr_ops: Optional[List[_lib.Csr]] = None            # pagerank(): the scaled operand of every level (this mode)
+        self._pr_work: Optional[Tuple[_lib.Dense, ...]] = None    # pagerank(): restart S, chunk scratch, state
+        self._pr_refusal: Optional[str] = None                   # pagerank(): why the operator has no walk (bad weights)
+        self.last_pagerank_residuals = np.zeros((0, int(k)), np.float64)   # [steps x k] of the last pagerank()
         fused_ok = True
         cmap_prev = None                      # level j-1 row -> level-0 row (host, int64, -1 invalid)
         for j, (B, _) in enumerate(decomposition):
@@ -259,6 +264,7 @@ class ArrowEngine:
                 b.free()
             self.levels[0].bufs = list(self._slots[0])
             del self._slots
+        self._free_pagerank_operands()              # they share the arrays of the blocks freed below
         for st in self.levels:
             for b in st.bufs:
                 if b is not None:
@@ -645,6 +651,126 @@ class ArrowEngine:
         if not self.fused_ok:
             raise ValueError(f"{what} needs a level-0 row behind every non-zero, but a level reads rows behind the "
                              "sentinel")
+
+    # -- personalized PageRank (plus_times) --------------------------------------------------------------------------
+    def pagerank(self, max_steps: int, alpha: float = 0.85, tol: float = 1e-6, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Personalized PageRank (random walk with restart) from the current level-0 features, one restart distribution
+        per column; returns ``p`` (the engine's dtype ``T``, [n x k] in level-0 row order like ``result()``).
+
+        ``M`` is the operator ``step()`` applies (with the identity diagonal when ``add_identity``): entry ``(r, c)`` of
+        level ``j`` with value ``a`` is the edge ``cmap_j(c) -> cmap_j(r)``, duplicates counted separately.  ``w[u]`` is
+        the float64 sum of the values of the edges leaving ``u`` (levels ascending, then entry order), ``u`` is dangling
+        when ``w[u] == 0`` and ``inv[u] = fl_T(1 / w[u])`` (0 when dangling).  The walk steps on ``M^``, ``M`` with each
+        entry ``fl_T(a * inv[u])``.  The restart is ``S[:, s] = fl_T(X0[:, s] / sigma_s)``, ``sigma_s`` the column sum of
+        the features.  From ``p_0 = S`` every step computes ``Y = M^ p_t`` through the engine's own route, the dangling
+        mass ``m_t[s]``, ``c_t[s] = fl(fl(1 - alpha) + fl(alpha * m_t[s]))`` and ``p_{t+1} = fl_T(fl(fl(alpha * Y) +
+        fl(c_t * S)))``: dangling mass returns through the restart.  The loop stops after the first step whose largest
+        residual ``r[s] = sum_v |p_{t+1}[v, s] - p_t[v, s]|`` is ``<= tol``, or after ``max_steps`` steps
+        (``max_steps = 0`` returns ``S``); ``last_pagerank_residuals`` (float64 [steps x k]) holds every step's
+        residuals.  Every column reduction runs in float64 over fixed 512-row chunks (DESIGN.md §4), so two calls give
+        the same bits.  At the fixed point ``||p - p*||_1 <= alpha / (1 - alpha) * r`` per column.
+
+        The out-weights (12 or 16 bytes per row) and the scaled values of every level's operand (4 or 8 bytes per entry)
+        are built on the first call and kept until ``close()`` or a mode change; ``S`` (one tile), the chunk scratch (16 k
+        bytes per 512 rows) and the state are allocated on first use.  Afterwards the level-0 features are ``p``:
+        ``result()`` and ``features()`` return it and the next ``step()`` multiplies it by ``M``; the tiles of the levels
+        ``j >= 1`` are unspecified.  Raises ``ValueError`` before any CUDA work outside ``plus_times``, when a level reads
+        rows behind the sentinel, for ``alpha`` outside ``[0, 1)``, a negative or NaN ``tol``, a negative ``max_steps``
+        and an ``out`` that is not a C-contiguous ``T`` array of shape [n x k]; after the out-weight pass for an edge
+        whose weight is negative, NaN or +-inf, or a non-dangling vertex whose inverse is not finite (remembered: later
+        calls refuse at once); after the restart pass, with the features unchanged, for a column holding a negative,
+        NaN or +-inf value or summing to 0.  Synchronises."""
+        max_steps = self._pagerank_checks(max_steps, alpha, tol, out)
+        S, scratch, state = self._pagerank_prepare()
+        st0 = self.levels[0]
+        x = st0.bufs[st0.xi]
+        inv = self._pr_weights[1]
+        sums, bad, first = self.ctx.pagerank_restart(x, inv, S, scratch, state)
+        if bad:
+            raise ValueError(f"pagerank needs every restart column non-negative and finite with a positive sum: column "
+                             f"{first} is not ({bad} such column(s)); sum {sums[first]!r}")
+        x.copy_from(S)
+        residuals = []
+        for _ in range(max_steps):
+            p_tile = self._pagerank_step()
+            res = self.ctx.pagerank_update(st0.bufs[st0.xi], p_tile, S, inv, scratch, state, alpha)
+            residuals.append(res)
+            if res.max(initial=0.0) <= tol:
+                break
+        self.last_pagerank_residuals = np.array(residuals, np.float64).reshape(len(residuals), self.k)
+        return st0.bufs[st0.xi].d2h(out)
+
+    def _pagerank_checks(self, max_steps, alpha, tol, out) -> int:
+        if self.sr != _lib.SR_PLUS_TIMES:
+            raise ValueError(f"pagerank runs the plus_times semiring, the engine runs {self.semiring}")
+        if not self.fused_ok:
+            raise ValueError("pagerank needs a level-0 row behind every non-zero, but a level reads rows behind the sentinel")
+        alpha, tol = float(alpha), float(tol)
+        if not (0.0 <= alpha < 1.0):
+            raise ValueError(f"alpha must lie in [0, 1), got {alpha!r}")
+        if not (tol >= 0.0):
+            raise ValueError(f"tol must be >= 0, got {tol!r}")
+        if int(max_steps) != max_steps or int(max_steps) < 0:
+            raise ValueError(f"max_steps must be a non-negative integer, got {max_steps!r}")
+        shape = (self.levels[0].rows, self.k)
+        if out is not None and (not isinstance(out, np.ndarray) or out.dtype != self.dtype or out.shape != shape
+                                or not out.flags.c_contiguous):
+            raise ValueError(f"out must be a C-contiguous {self.dtype} array of shape {shape}")
+        if self._pr_refusal is not None:
+            raise ValueError(self._pr_refusal)
+        return int(max_steps)
+
+    def _pagerank_prepare(self) -> Tuple[_lib.Dense, _lib.Dense, _lib.Dense]:
+        """the out-weights, the scaled operands of the current mode and the work tiles, made where missing"""
+        self.sync()
+        st0 = self.levels[0]
+        n = st0.rows
+        if self._pr_weights is None:
+            w, inv = self.ctx.dense_alloc(n, 1, np.float64), self.ctx.dense_alloc(n, 1, self.dtype)
+            self._pr_weights = (w, inv)
+            bad, _, bad_inv = self.ctx.out_weights([(st.csr, st.cmap_dev) for st in self.levels], n, w, inv)
+            if bad:
+                self._pr_refusal = (f"pagerank needs every edge weight non-negative and finite: {bad} edge(s) of the operator "
+                                    "have a negative, NaN or infinite weight")
+            elif bad_inv:
+                self._pr_refusal = (f"pagerank needs a finite non-zero 1 / w for every vertex with out-weight w != 0: "
+                                    f"{bad_inv} vertex(es) have none in {self.dtype}")
+            if self._pr_refusal is not None:
+                raise ValueError(self._pr_refusal)
+        inv = self._pr_weights[1]
+        if self._pr_ops is None:
+            ops = [st0.csr.scale_columns(inv)]
+            for st in self.levels[1:]:
+                ops.append(st.csr_fused.scale_columns(inv) if self.mode == "fused" else st.csr.scale_columns(inv, st.cmap_dev))
+            self._pr_ops = ops
+        if self._pr_work is None:
+            chunks = (n + 511) // 512
+            self._pr_work = (self.ctx.dense_alloc(n, self.k, self.dtype), self.ctx.dense_alloc(chunks, 2 * self.k, np.float64),
+                             self.ctx.dense_alloc(4, self.k, np.float64))
+        return self._pr_work
+
+    def _pagerank_step(self) -> _lib.Dense:
+        """one ``step()`` on the scaled operands; returns the tile it read (p_t), level 0's features then being Y"""
+        st0 = self.levels[0]
+        p_tile = st0.bufs[st0.xi]
+        attr = "csr_fused" if self.mode == "fused" else "csr"
+        kept = [st0.csr] + [getattr(st, attr) for st in self.levels[1:]]
+        try:
+            st0.csr = self._pr_ops[0]
+            for st, op in zip(self.levels[1:], self._pr_ops[1:]):
+                setattr(st, attr, op)
+            self.step()
+        finally:
+            st0.csr = kept[0]
+            for st, op in zip(self.levels[1:], kept[1:]):
+                setattr(st, attr, op)
+        st0.xi = st0.ci                      # an exchange-mode step of one level leaves xi where it was
+        return p_tile
+
+    def _free_pagerank_operands(self):
+        for op in self._pr_ops or ():
+            op.free()
+        self._pr_ops = None
 
     # -- multi-source BFS (or_and) ----------------------------------------------------------------------------------
     def bfs_levels(self, max_steps: int, out: Optional[np.ndarray] = None) -> np.ndarray:
@@ -1073,4 +1199,8 @@ class ArrowEngine:
             if b is not None:
                 b.free()
         self._bt_in_adj = self._bt_tiles = None
+        self._free_pagerank_operands()
+        for b in (self._pr_weights or ()) + (self._pr_work or ()):
+            b.free()
+        self._pr_weights = self._pr_work = None
         self.ctx.close()

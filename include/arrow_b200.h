@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 13
+#define ARROW_ABI_VERSION 14
 
 /* error codes */
 #define ARROW_OK              0
@@ -418,6 +418,50 @@ int  arrow_wpaths_counts(arrow_ctx *ctx, int in_adj, int out_adj, int x0_buf, in
  * ARROW_ERR_ARG: those of arrow_wpaths_counts, and no rounds of it kept for the state tile. */
 int  arrow_wpaths_dependencies(arrow_ctx *ctx, int out_adj, int x0_buf, int dist_buf, int state_buf, int sigma_buf, int delta_buf,
                                int64_t *entries_read);
+
+/* ---- personalized PageRank (one GPU, plus-times on float32 or float64 tiles) ---------------------------------------------- */
+/* Every column reduction below (sigma, the dangling mass m, the residual r) runs in float64 over fixed 512-row chunks from
+ * row 0: sequential in ascending rows inside a chunk, the chunk partials then added in ascending chunk order.  No
+ * floating-point atomics: the results depend neither on the grid nor on the schedule.  The float64 arithmetic is separately
+ * rounded (no contraction). */
+/* Out-weights of the operator M of arrow_adj_build's parts, self-loops and duplicates included: w[u] (w_buf, ARROW_F64
+ * [n_vertices x 1]) is the float64 sum, from +0 and in (part, entry) order, of the values of the entries whose edge
+ * map(c) -> map(r) leaves u (an end at -1: not an edge); inv[u] (inv_buf, the blocks' element type T, [n_vertices x 1]) is
+ * fl_T(1 / w[u]) from a float64 divide, 0 where w[u] == 0 (u is dangling).  One pass writes a key per entry, a stable radix
+ * sort groups them by source and one thread per vertex sums its run.  *bad_entries receives the edges whose value is
+ * negative, NaN or +-inf (-0 is allowed), *dangling the vertices with w == 0, *bad_inverses the other vertices whose
+ * inverse is not finite or 0 (each pointer may be NULL).  Temporary device memory of 24 bytes per entry plus the sort's
+ * storage is freed before the call returns.  ARROW_ERR_ARG: the refusals of arrow_adj_build, parts of different element
+ * types, w / inv of another type or shape; ARROW_ERR_RANGE: 2^31 entries or more; ARROW_ERR_UNSUPPORTED: during graph
+ * capture.  Synchronises. */
+int  arrow_out_weights(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices, int w_buf, int inv_buf,
+                       int64_t *bad_entries, int64_t *dangling, int64_t *bad_inverses);
+/* A values-only copy of a block (ARROW_F32 or ARROW_F64) whose entry (r, c) of value a holds fl_T(a * scale[map(c)])
+ * (map -1: the identity; 0 where the column or its image is -1); scale_buf is a [rows x 1] tile of the block's type that
+ * covers every (mapped) column.  Row pointers, indices, long-row lists and tile lists are shared with the source, which
+ * may itself be a remapped copy (arrow_csr_remap_columns): arrow_csr_free refuses the source while the copy lives.  The
+ * copy owns (nnz + 8) values.  Synchronises. */
+int  arrow_csr_scale_columns(arrow_ctx *ctx, int csr, int map, int scale_buf, int *csr_out);
+/* The restart of personalized PageRank.  x_buf holds X0 (T [n x k], T float32 or float64), inv_buf the inverse
+ * out-weights (T [n x 1], 0 marking the dangling rows), s_buf receives S (T [n x k]), scratch_buf is float64
+ * [ceil(n / 512) x 2k] and state_buf float64 [4 x k].  sigma_s = the chunked float64 sum of column s.  A column is bad
+ * when it holds a negative, NaN or +-inf value or sigma_s is not a positive finite number; *bad_columns (may be NULL)
+ * receives their number, *first_bad_column (may be NULL) the smallest (-1: none) and col_sums (k host doubles, may be
+ * NULL) sigma.  When no column is bad, S[v, s] = fl_T(X0[v, s] / sigma_s) (float64 divide) and state row 0 receives m_0,
+ * the dangling mass of S; rows 2 and 3 hold sigma and the bad flags.  x_buf is never written.  The grid of this pass and of
+ * arrow_pagerank_update follows ARROW_OPT_SPMM_SM_LIMIT and ARROW_OPT_SPMM_CTAS_PER_SM and changes no bit.  ARROW_ERR_ARG:
+ * other types or shapes, two tiles aliasing; ARROW_ERR_UNSUPPORTED: graph capture.  Synchronises. */
+int  arrow_pagerank_restart(arrow_ctx *ctx, int x_buf, int inv_buf, int s_buf, int scratch_buf, int state_buf, double *col_sums,
+                            int64_t *bad_columns, int64_t *first_bad_column);
+/* One iterate of personalized PageRank after the step Y = M^ p_t (y_buf): with beta = fl(1 - alpha) and c_s = fl(beta +
+ * fl(alpha * m_t[s])), m_t in state row 0, p_{t+1}[v, s] = fl_T(fl(fl(alpha * Y[v, s]) + fl(c_s * S[v, s]))) is written over
+ * Y in place.  The same pass sums the chunk partials of m_{t+1} (the dangling mass of p_{t+1}) and of r_{t+1}[s] = the sum
+ * of |fl(p_{t+1}[v, s] - p_t[v, s])|; a second kernel adds them in order into state rows 0 and 1 and residuals (k host
+ * doubles, may be NULL) receives r_{t+1}.  Traffic: Y, p and S read, p_{t+1} written.  Tiles as arrow_pagerank_restart,
+ * p_buf and y_buf T [n x k].  ARROW_ERR_ARG: alpha outside [0, 1) or NaN, other types or shapes, two tiles aliasing;
+ * ARROW_ERR_UNSUPPORTED: graph capture.  Synchronises. */
+int  arrow_pagerank_update(arrow_ctx *ctx, int y_buf, int p_buf, int s_buf, int inv_buf, int scratch_buf, int state_buf,
+                           double alpha, double *residuals);
 
 /* ---- predecessors of the tropical semirings (one GPU, fp32) ------------------------------------------ */
 /* The product of arrow_spmm_sr over (value, label) pairs.  A candidate of row r is an entry p whose column c is valid
