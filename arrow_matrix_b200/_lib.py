@@ -56,8 +56,9 @@ EXPORTS = [
     "arrow_adj_build_loopfree", "arrow_wpaths_counts", "arrow_wpaths_dependencies",
     "arrow_sr_mark_frontier_steps", "arrow_sr_tree_parents", "arrow_dense_count_diff_bits",
     "arrow_out_weights", "arrow_csr_scale_columns", "arrow_pagerank_restart", "arrow_pagerank_update",
+    "arrow_connected_components",
 ]
-ABI_VERSION = 14       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
+ABI_VERSION = 15       # ARROW_ABI_VERSION of include/arrow_b200.h this binding was written against
 
 
 class ArrowError(RuntimeError):
@@ -186,6 +187,7 @@ def load_library(build_if_missing: bool = True) -> ctypes.CDLL:
         "arrow_csr_scale_columns": (c_int, [P, I, I, I, pI]),
         "arrow_pagerank_restart": (c_int, [P, I, I, I, I, I, POINTER(c_double), pI64, pI64]),
         "arrow_pagerank_update": (c_int, [P, I, I, I, I, I, I, c_double, POINTER(c_double)]),
+        "arrow_connected_components": (c_int, [P, I, pI, pI, I64, I, I, pI64]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export a declared symbol
@@ -671,6 +673,19 @@ class Context:
         self._check(self.lib.arrow_pagerank_update(self._h, y.h, p.h, s.h, inv.h, scratch.h, state.h, float(alpha),
                                                    res.ctypes.data_as(POINTER(c_double))))
         return res
+
+    def connected_components(self, parts: Sequence[tuple], n_vertices: int, labels: "Dense",
+                             sizes: Optional["Dense"] = None) -> int:
+        """Weakly connected components of the operator of ``adj_build(parts, n_vertices)`` (``arrow_connected_components``):
+        ``labels`` (int32 [n x 1]) receives the smallest vertex of each vertex's component, ``sizes`` (int32 [n x 1]) the
+        member count at each label's row and 0 elsewhere.  Returns the number of components; synchronises."""
+        n = len(parts)
+        csrs = (c_int * max(n, 1))(*[A.h for A, _ in parts])
+        maps = (c_int * max(n, 1))(*[m.h if m is not None else -1 for _, m in parts])
+        count = c_int64()
+        self._check(self.lib.arrow_connected_components(self._h, n, csrs, maps, int(n_vertices), labels.h,
+                                                        sizes.h if sizes is not None else -1, byref(count)))
+        return int(count.value)
 
     def count_diff(self, a: "Dense", b: "Dense") -> int:
         """rows in which two equally shaped tiles differ in some element (-0 == +0, NaN != NaN); synchronises"""

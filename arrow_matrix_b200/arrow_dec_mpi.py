@@ -231,6 +231,12 @@ class ArrowDecompositionMPI:
         ids."""
         return self._bfs_engine("pagerank").pagerank(max_steps, alpha, tol, out)
 
+    def connected_components(self, out: Optional[np.ndarray] = None, sizes_out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension (one GPU, any semiring): weakly connected components of the operator, int32 labels (the smallest row
+        of each row's component) in ``result_tile()`` row order (see ``ArrowEngine.connected_components``).  Level 0's
+        permutation maps the rows, and so the labels, to vertex ids."""
+        return self._bfs_engine("connected_components").connected_components(out, sizes_out)
+
     def _bfs_engine(self, what: str) -> ArrowEngine:
         if self.comm.Get_size() > 1:
             raise ValueError(f"{what} runs on one GPU only")

@@ -4516,6 +4516,126 @@ int pr_grid(const arrow_ctx *ctx, long long items) {
     const long long per_sm = ctx->spmm_ctas_per_sm > 0 ? ctx->spmm_ctas_per_sm : 8;
     return (int)std::max<long long>(1, std::min<long long>((items + 255) / 256, sms * per_sm));
 }
+
+// ------------------------------------------------------------------------------------------------
+// connected components (one GPU): a lock-free union-find over a parent array (the label tile), in the manner of ECL-CC
+// (Jaiganesh and Burtscher, HPDC 2018).  Invariant: parent[x] <= x for every x, with equality exactly for the roots.  It
+// holds after the init; a hook CASes a root hi, expected still parent[hi] == hi, to a smaller root lo; path halving stores
+// into a vertex that is not a root (so no CAS can target it again) a grandparent, which is below its parent.  A vertex
+// never becomes a root again and every store keeps it in its own tree, so trees only merge.  Hence each root is the
+// smallest vertex of its tree, and once every entry has joined its two ends, the smallest of its component.
+// Termination: a root walk moves to a strictly smaller vertex each round; a union's failed CAS means the larger root gained
+// a parent below it, so max(a, b) of the two roots strictly decreases each round.  Every read of parent inside those
+// loops is an ld.relaxed.gpu: never served from L1 or kept in a register across rounds.
+// ------------------------------------------------------------------------------------------------
+constexpr int CC_CHUNK = 256;          // entries of one warp chunk of the hook pass
+
+__device__ __forceinline__ int cc_load(const int *p) {
+    int v;
+    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+
+__device__ __forceinline__ void cc_store(int *p, int v) {
+    asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// the root of v's tree, halving the path: each round either returns or moves v to its grandparent g < parent < v
+__device__ __forceinline__ int cc_root(int *parent, int v) {
+    for (;;) {
+        const int p = cc_load(parent + v);
+        if (p == v) return v;
+        const int g = cc_load(parent + p);
+        if (g == p) return p;
+        cc_store(parent + v, g);
+        v = g;
+    }
+}
+
+// joins the trees of u and v: hooks the larger root onto the smaller; on a failed CAS both roots are found again, and
+// both lie below the old larger root (the CAS saw its new parent old < hi)
+__device__ __forceinline__ void cc_union(int *parent, int u, int v) {
+    int a = cc_root(parent, u), b = cc_root(parent, v);
+    while (a != b) {
+        const int hi = max(a, b), lo = min(a, b);
+        const int old = atomicCAS(parent + hi, hi, lo);
+        if (old == hi) return;
+        a = cc_root(parent, old);
+        b = cc_root(parent, lo);
+    }
+}
+
+__global__ void __launch_bounds__(256) k_cc_init(int *__restrict__ parent, long long n) {
+    for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < n; v += (long long)gridDim.x * blockDim.x)
+        parent[v] = (int)v;
+}
+
+// the hook pass over one part: warp-stride over CC_CHUNK-entry chunks, so a long row is spread over many warps.  Lanes 0
+// and 1 find the rows of the chunk's first and last entries over the whole block; each entry then searches only the rows
+// between them (none for a chunk inside one row).  Entry (r, c) joins map(c) and map(r); c < 0, an end at -1 and u == v
+// join nothing.  The value is never read.
+__global__ void __launch_bounds__(256) k_cc_hook(AdjPart p, int *parent) {
+    const int lane = threadIdx.x & 31;
+    const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
+    const long long chunks = (p.nnz + CC_CHUNK - 1) / CC_CHUNK;
+    for (long long ch = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; ch < chunks; ch += warps) {
+        const long long e0 = ch * CC_CHUNK, e1 = min(p.nnz, e0 + CC_CHUNK);
+        int r = 0;
+        if (lane < 2) r = last_le(p.indptr, 0, p.n_rows - 1, lane == 0 ? e0 : e1 - 1);
+        const int r_lo = __shfl_sync(0xffffffffu, r, 0), r_hi = __shfl_sync(0xffffffffu, r, 1);
+        for (long long e = e0 + lane; e < e1; e += 32) {
+            const int c = __ldg(p.indices + e);
+            if (c < 0) continue;
+            const int row = last_le(p.indptr, r_lo, r_hi, e);
+            const int u = p.map ? __ldg(p.map + c) : c;
+            const int v = p.map ? __ldg(p.map + row) : row;
+            if (u >= 0 && v >= 0 && u != v) cc_union(parent, u, v);
+        }
+    }
+}
+
+// labels[v] = root(v) in place, after the hook pass (the roots no longer change).  The walk stores nothing: parent[v] is
+// written by v's thread alone, so it ends at the root, and a concurrent walk through v reads its old parent or the root.
+// Counts the roots (one integer atomic per warp) and, with sizes, adds each vertex to its label's count.
+__global__ void __launch_bounds__(256) k_cc_label(int *parent, long long n, int *__restrict__ sizes,
+                                                  unsigned long long *__restrict__ roots) {
+    unsigned mine = 0;
+    for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < n; v += (long long)gridDim.x * blockDim.x) {
+        int r = cc_load(parent + v), next;
+        while ((next = cc_load(parent + r)) != r) r = next;      // next < r: strictly decreasing
+        if (r == (int)v) ++mine;
+        else cc_store(parent + v, r);
+        if (sizes) atomicAdd(sizes + r, 1);
+    }
+    for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
+    if ((threadIdx.x & 31) == 0 && mine) atomicAdd(roots, (unsigned long long)mine);
+}
+
+// the (block, row map) pairs of arrow_adj_build and of the passes over the same operator: valid handles, every map covering
+// its block's rows and columns and reaching no row past n_vertices, a block under the identity map within n_vertices
+int operator_parts(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices,
+                   std::vector<std::pair<const Csr *, const IdxMap *>> &out) {
+    for (int i = 0; i < n_parts; ++i) {
+        const Csr *c = get_csr(ctx, csrs[i]);
+        if (!c) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad csr handle %d", i, csrs[i]);
+        const IdxMap *m = nullptr;
+        if (maps[i] != -1) {
+            m = get_map(ctx, maps[i]);
+            if (!m) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad map handle %d", i, maps[i]);
+            if (m->n < std::max(c->n_rows, c->n_cols))
+                return fail(ctx, ARROW_ERR_ARG, "part %d: the map has %lld entries, the block %lld rows and %lld columns", i,
+                            (long long)m->n, (long long)c->n_rows, (long long)c->n_cols);
+            if (m->limit > n_vertices)
+                return fail(ctx, ARROW_ERR_ARG, "part %d: the map reaches row %lld, there are %lld vertices", i,
+                            (long long)m->limit, (long long)n_vertices);
+        } else if (c->n_rows > n_vertices || c->n_cols > n_vertices) {
+            return fail(ctx, ARROW_ERR_ARG, "part %d: a %lld x %lld block with the identity map exceeds %lld vertices", i,
+                        (long long)c->n_rows, (long long)c->n_cols, (long long)n_vertices);
+        }
+        out.emplace_back(c, m);
+    }
+    return ARROW_OK;
+}
 }  // namespace
 
 // ================================================================================================
@@ -5795,30 +5915,18 @@ int adj_build(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int
         return fail(ctx, ARROW_ERR_ARG, "bad arguments (n_parts=%d, n_vertices=%lld)", n_parts, (long long)n_vertices);
     if (n_vertices > 2147483646LL) return fail(ctx, ARROW_ERR_RANGE, "%lld vertices exceed the int32 device layout", (long long)n_vertices);
     if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "%s allocates and synchronises: not during graph capture", fn);
+    std::vector<std::pair<const Csr *, const IdxMap *>> blocks;
+    if (const int rc = operator_parts(ctx, n_parts, csrs, maps, n_vertices, blocks)) return rc;
     std::vector<AdjPart> parts;
     std::vector<const float *> weights;                       // the entries' values of each part (weighted only)
     for (int i = 0; i < n_parts; ++i) {
-        const Csr *c = get_csr(ctx, csrs[i]);
-        if (!c) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad csr handle %d", i, csrs[i]);
+        const Csr *c = blocks[i].first;
+        const IdxMap *m = blocks[i].second;
         if (weighted && c->dtype != ARROW_F32)
             return fail(ctx, ARROW_ERR_UNSUPPORTED, "part %d: %s carries fp32 weights, the block is %s", i, fn,
                         dtype_name(c->dtype));
         if (weighted && c->nnz > 0 && !c->vals)
             return fail(ctx, ARROW_ERR_ARG, "part %d: the block has no values to carry as weights", i);
-        const IdxMap *m = nullptr;
-        if (maps[i] != -1) {
-            m = get_map(ctx, maps[i]);
-            if (!m) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad map handle %d", i, maps[i]);
-            if (m->n < std::max(c->n_rows, c->n_cols))
-                return fail(ctx, ARROW_ERR_ARG, "part %d: the map has %lld entries, the block %lld rows and %lld columns", i,
-                            (long long)m->n, (long long)c->n_rows, (long long)c->n_cols);
-            if (m->limit > n_vertices)
-                return fail(ctx, ARROW_ERR_ARG, "part %d: the map reaches row %lld, there are %lld vertices", i,
-                            (long long)m->limit, (long long)n_vertices);
-        } else if (c->n_rows > n_vertices || c->n_cols > n_vertices) {
-            return fail(ctx, ARROW_ERR_ARG, "part %d: a %lld x %lld block with the identity map exceeds %lld vertices", i,
-                        (long long)c->n_rows, (long long)c->n_cols, (long long)n_vertices);
-        }
         if (c->nnz > 0) {
             parts.push_back(AdjPart{c->indptr, c->indices, m ? m->p : nullptr, (long long)c->nnz, (int)c->n_rows});
             weights.push_back(c->vals);
@@ -6670,28 +6778,16 @@ int arrow_out_weights(arrow_ctx *ctx, int n_parts, const int *csrs, const int *m
     DenseBuf *W = get_dense(ctx, w_buf), *I = get_dense(ctx, inv_buf);
     if (!W || !I) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle (w=%d inv=%d)", w_buf, inv_buf);
     int T = -1;
+    std::vector<std::pair<const Csr *, const IdxMap *>> blocks;
+    if (const int rc = operator_parts(ctx, n_parts, csrs, maps, n_vertices, blocks)) return rc;
     std::vector<AdjPart> parts;
     std::vector<const void *> vals;
     long long m = 0;
     for (int i = 0; i < n_parts; ++i) {
-        const Csr *c = get_csr(ctx, csrs[i]);
-        if (!c) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad csr handle %d", i, csrs[i]);
+        const Csr *c = blocks[i].first;
+        const IdxMap *mp = blocks[i].second;
         if (T >= 0 && c->dtype != T) return fail(ctx, ARROW_ERR_ARG, "part %d is %s, part 0 %s", i, dtype_name(c->dtype), dtype_name(T));
         T = c->dtype;
-        const IdxMap *mp = nullptr;
-        if (maps[i] != -1) {
-            mp = get_map(ctx, maps[i]);
-            if (!mp) return fail(ctx, ARROW_ERR_HANDLE, "part %d: bad map handle %d", i, maps[i]);
-            if (mp->n < std::max(c->n_rows, c->n_cols))
-                return fail(ctx, ARROW_ERR_ARG, "part %d: the map has %lld entries, the block %lld rows and %lld columns", i,
-                            (long long)mp->n, (long long)c->n_rows, (long long)c->n_cols);
-            if (mp->limit > n_vertices)
-                return fail(ctx, ARROW_ERR_ARG, "part %d: the map reaches row %lld, there are %lld vertices", i, (long long)mp->limit,
-                            (long long)n_vertices);
-        } else if (c->n_rows > n_vertices || c->n_cols > n_vertices) {
-            return fail(ctx, ARROW_ERR_ARG, "part %d: a %lld x %lld block with the identity map exceeds %lld vertices", i,
-                        (long long)c->n_rows, (long long)c->n_cols, (long long)n_vertices);
-        }
         if (c->nnz > 0 && !c->vals) return fail(ctx, ARROW_ERR_ARG, "part %d: the block has no values", i);
         if (c->nnz > 0) {
             parts.push_back(AdjPart{c->indptr, c->indices, mp ? mp->p : nullptr, (long long)c->nnz, (int)c->n_rows});
@@ -6898,6 +6994,54 @@ int arrow_pagerank_update(arrow_ctx *ctx, int y_buf, int p_buf, int s_buf, int i
     CUDA_TRY(ctx, cudaGetLastError());
     if (residuals) CUDA_TRY(ctx, cudaMemcpyAsync(residuals, state + k, (size_t)k * 8, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    return ARROW_OK;
+}
+
+int arrow_connected_components(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices,
+                               int labels_buf, int sizes_buf, int64_t *n_components) {
+    CHECK_CTX(ctx);
+    CHECK_POISON(ctx);
+    if (n_parts < 0 || (n_parts > 0 && (!csrs || !maps)) || n_vertices < 0)
+        return fail(ctx, ARROW_ERR_ARG, "bad arguments (n_parts=%d, n_vertices=%lld)", n_parts, (long long)n_vertices);
+    if (n_vertices > 2147483646LL) return fail(ctx, ARROW_ERR_RANGE, "%lld vertices exceed the int32 device layout", (long long)n_vertices);
+    DenseBuf *L = get_dense(ctx, labels_buf), *S = nullptr;
+    if (!L) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle labels=%d", labels_buf);
+    if (sizes_buf != -1 && !(S = get_dense(ctx, sizes_buf))) return fail(ctx, ARROW_ERR_HANDLE, "bad dense handle sizes=%d", sizes_buf);
+    for (const DenseBuf *t : {L, S}) {
+        if (t && (t->dtype != ARROW_I32 || t->rows != n_vertices || t->k != 1))
+            return fail(ctx, ARROW_ERR_ARG, "%s is a %s tile of %lld x %d, expected int32 %lld x 1", t == L ? "labels" : "sizes",
+                        dtype_name(t->dtype), (long long)t->rows, t->k, (long long)n_vertices);
+    }
+    if (S && (sizes_buf == labels_buf || S->p == L->p)) return fail(ctx, ARROW_ERR_ARG, "sizes aliases labels");
+    std::vector<std::pair<const Csr *, const IdxMap *>> blocks;
+    if (const int rc = operator_parts(ctx, n_parts, csrs, maps, n_vertices, blocks)) return rc;
+    if (ctx->capturing) return fail(ctx, ARROW_ERR_UNSUPPORTED, "arrow_connected_components synchronises: not during graph capture");
+    int *parent = reinterpret_cast<int *>(L->p);
+    int *sizes = S ? reinterpret_cast<int *>(S->p) : nullptr;
+    cudaStream_t s = cur_stream(ctx);
+    DevTmp cnt;
+    unsigned long long roots = 0;
+    CUDA_TRY(ctx, cudaMalloc(&cnt.p, sizeof roots));
+    unsigned long long *d_roots = reinterpret_cast<unsigned long long *>(cnt.p);
+    CUDA_TRY(ctx, cudaMemsetAsync(d_roots, 0, sizeof roots, s));
+    if (sizes) CUDA_TRY(ctx, cudaMemsetAsync(sizes, 0, (size_t)n_vertices * 4, s));
+    if (n_vertices > 0) {
+        k_cc_init<<<pr_grid(ctx, n_vertices), 256, 0, s>>>(parent, n_vertices);
+        ctx->launches++;
+        for (const auto &b : blocks) {
+            const Csr *c = b.first;
+            if (c->nnz == 0) continue;
+            const AdjPart p{c->indptr, c->indices, b.second ? b.second->p : nullptr, (long long)c->nnz, (int)c->n_rows};
+            k_cc_hook<<<pr_grid(ctx, (p.nnz + CC_CHUNK - 1) / CC_CHUNK * 32), 256, 0, s>>>(p, parent);
+            ctx->launches++;
+        }
+        k_cc_label<<<pr_grid(ctx, n_vertices), 256, 0, s>>>(parent, n_vertices, sizes, d_roots);
+        ctx->launches++;
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    CUDA_TRY(ctx, cudaMemcpyAsync(&roots, d_roots, sizeof roots, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    if (n_components) *n_components = (int64_t)roots;
     return ARROW_OK;
 }
 

@@ -184,6 +184,9 @@ class ArrowEngine:
         self._pr_work: Optional[Tuple[_lib.Dense, ...]] = None    # pagerank(): restart S, chunk scratch, state
         self._pr_refusal: Optional[str] = None                   # pagerank(): why the operator has no walk (bad weights)
         self.last_pagerank_residuals = np.zeros((0, int(k)), np.float64)   # [steps x k] of the last pagerank()
+        self._cc_labels: Optional[_lib.Dense] = None             # connected_components(): int32 [n x 1] labels
+        self._cc_sizes: Optional[_lib.Dense] = None              # connected_components(): int32 [n x 1] sizes
+        self.last_component_count = 0                            # components found by the last connected_components()
         fused_ok = True
         cmap_prev = None                      # level j-1 row -> level-0 row (host, int64, -1 invalid)
         for j, (B, _) in enumerate(decomposition):
@@ -772,6 +775,47 @@ class ArrowEngine:
             op.free()
         self._pr_ops = None
 
+    # -- connected components (any semiring) ------------------------------------------------------------------------
+    def connected_components(self, out: Optional[np.ndarray] = None,
+                             sizes_out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Weakly connected components of the operator ``step()`` applies: int32 ``labels[v]`` (``[n]``, level-0 row
+        order like ``result()``) is the smallest level-0 row in ``v``'s component; ``last_component_count`` receives the
+        number of components (the ``v`` with ``labels[v] == v``) and ``sizes_out`` (int32 ``[n]``), when given, the
+        member count of the component labelled ``r`` at row ``r`` and 0 at the rows that are not labels.
+
+        The vertices are the level-0 rows, padding rows included (they are singletons unless an entry names them).
+        Every entry ``(r, c)`` of level ``j`` as the step applies it (the arrow pattern, and the identity diagonal when
+        ``add_identity``) gives the undirected edge ``cmap_j(c) -- cmap_j(r)`` whatever its value (0, NaN and +-inf
+        included); ``u == v`` gives none.  The answer is unique, so it is bit-identical on every route, semiring, dtype,
+        ``k`` and grid.  One device pass of a lock-free union-find over the level blocks and the row maps the engine
+        keeps (DESIGN.md §4): no adjacency is built and nothing is sorted.
+
+        The label tile (4 bytes per row; another 4 with ``sizes_out``) is allocated on the first call and kept until
+        ``close()``.  Features, results and the next ``step()`` are untouched.  Raises ``ValueError`` before any CUDA
+        work when a level reads rows behind the sentinel (``fused_ok`` is false: such a row has no vertex identity) and
+        for an ``out`` or ``sizes_out`` that is not a C-contiguous int32 array of shape ``[n]``.  Synchronises."""
+        if not self.fused_ok:
+            raise ValueError("connected_components needs a level-0 row behind every non-zero, but a level reads rows "
+                             "behind the sentinel")
+        n = self.levels[0].rows
+        for name, arr in (("out", out), ("sizes_out", sizes_out)):
+            if arr is not None and (not isinstance(arr, np.ndarray) or arr.dtype != np.int32 or arr.shape != (n,)
+                                    or not arr.flags.c_contiguous):
+                raise ValueError(f"{name} must be a C-contiguous int32 array of shape {(n,)}")
+        if self._cc_labels is None:
+            self._cc_labels = self.ctx.dense_alloc(n, 1, np.int32)
+        if sizes_out is not None and self._cc_sizes is None:
+            self._cc_sizes = self.ctx.dense_alloc(n, 1, np.int32)
+        sizes = self._cc_sizes if sizes_out is not None else None
+        self.last_component_count = self.ctx.connected_components([(st.csr, st.cmap_dev) for st in self.levels], n,
+                                                                  self._cc_labels, sizes)
+        if sizes is not None:
+            sizes.d2h(sizes_out[:, None])           # a view of sizes_out: the rows land in it
+        if out is None:
+            return self._cc_labels.d2h().reshape(-1)
+        self._cc_labels.d2h(out[:, None])
+        return out
+
     # -- multi-source BFS (or_and) ----------------------------------------------------------------------------------
     def bfs_levels(self, max_steps: int, out: Optional[np.ndarray] = None) -> np.ndarray:
         """Hop levels of a multi-source BFS from the current level-0 features (int32 [n x k], level-0 row order like
@@ -1203,4 +1247,8 @@ class ArrowEngine:
         for b in (self._pr_weights or ()) + (self._pr_work or ()):
             b.free()
         self._pr_weights = self._pr_work = None
+        for b in (self._cc_labels, self._cc_sizes):
+            if b is not None:
+                b.free()
+        self._cc_labels = self._cc_sizes = None
         self.ctx.close()

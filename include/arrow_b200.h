@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct arrow_ctx arrow_ctx;
 
-#define ARROW_ABI_VERSION 14
+#define ARROW_ABI_VERSION 15
 
 /* error codes */
 #define ARROW_OK              0
@@ -462,6 +462,21 @@ int  arrow_pagerank_restart(arrow_ctx *ctx, int x_buf, int inv_buf, int s_buf, i
  * ARROW_ERR_UNSUPPORTED: graph capture.  Synchronises. */
 int  arrow_pagerank_update(arrow_ctx *ctx, int y_buf, int p_buf, int s_buf, int inv_buf, int scratch_buf, int state_buf,
                            double alpha, double *residuals);
+
+/* ---- connected components (one GPU, any element type of the blocks) ------------------------------------------------------ */
+/* Weakly connected components of the operator of arrow_adj_build's parts: the vertices are 0 .. n_vertices - 1 and every
+ * entry (r, c) gives the undirected edge map(c) -- map(r), whatever its value (0, NaN and +-inf included); an end at -1 and
+ * u == v give none.  labels_buf (ARROW_I32 [n_vertices x 1]) receives, for every vertex, the smallest vertex of its
+ * component; *n_components (may be NULL) the number of v with labels[v] == v; sizes_buf (ARROW_I32 [n_vertices x 1], -1:
+ * none) the member count of the component labelled r at row r and 0 at the rows that are not labels.  The answer is unique,
+ * so no bit depends on the grid (which follows ARROW_OPT_SPMM_SM_LIMIT and ARROW_OPT_SPMM_CTAS_PER_SM and changes no
+ * bit) or on the schedule.  A lock-free union-find over labels_buf itself (DESIGN.md §4): every parent is at most its vertex,
+ * a hook CASes the larger root onto the smaller, one pass takes every entry (warps over 256-entry chunks, so a long row is
+ * split across warps) and a second sets every label to its root.  No other device memory beyond an 8-byte counter.
+ * ARROW_ERR_HANDLE / ARROW_ERR_ARG: the refusals of arrow_adj_build, tiles of another type or shape, sizes aliasing
+ * labels; ARROW_ERR_RANGE: n_vertices of 2^31 - 1 or more; ARROW_ERR_UNSUPPORTED: during graph capture.  Synchronises. */
+int  arrow_connected_components(arrow_ctx *ctx, int n_parts, const int *csrs, const int *maps, int64_t n_vertices,
+                                int labels_buf, int sizes_buf, int64_t *n_components);
 
 /* ---- predecessors of the tropical semirings (one GPU, fp32) ------------------------------------------ */
 /* The product of arrow_spmm_sr over (value, label) pairs.  A candidate of row r is an entry p whose column c is valid
